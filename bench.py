@@ -1,14 +1,14 @@
 #!/usr/bin/env python
-"""bench.py — the MPPI command() hot path on B200, BASELINE.json's metric.
+"""bench.py — the MPPI command() hot path on H100, BASELINE.json's metric.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl engine|reference] [--workload NAME]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl engine|reference] [--workload NAME] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = one `command()` (shift + sample K x T noise + T-step rollout + softmin reweight + nominal update).
 Workloads (BASELINE.json `configs`; the default is configs[1], the north star):
     pendulum_c2   pendulum analytic, MPPI,  K=16384 T=30 fp32                       (configs[1])
     nav2d_c3      2-D navigation,    KMPPI RBF(sigma=2) S=5, K=8192 T=40 fp32       (configs[2])
-    mlp_c4        learned pendulum (3-32-32-2 tanh MLP), MPPI, K=32768 T=30, tcgen05 tensor-core rollout   (configs[3])
+    mlp_c4        learned pendulum (3-32-32-2 tanh MLP), MPPI, K=32768 T=30, wgmma tensor-core rollout   (configs[3])
     pendulum_c5   pendulum analytic, MPPI,  K=131072 per GPU T=50 fp32 (= K=2^20 on 8 GPUs)   (configs[4] shard)
 
 Printed JSON line (rank 0):
@@ -24,6 +24,8 @@ Printed JSON line (rank 0):
   cpu_baseline   : the reference's own implementation (oracle/_ref: the unmodified Python package on torch CPU ops;
                    the oracle port if that copy is absent) on this host's cores, bounded sample
 `--impl reference` times that CPU implementation alone, on the same config/metric.
+`--dump-outputs DIR` writes what the last timed command() computed (action, nominal U, per-sample costs) as
+DIR/<name>.npy; the inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -128,15 +130,8 @@ def load_peaks():
         return dict(hbm=float(d["hbm_gbs"]), tf_burst=float(d["bf16_tflops"]), tf_sustained=float(d["bf16_tflops_sustained"]),
                     src="measured (MEASURED_PEAKS.json)")
     except Exception:
-        return dict(hbm=6650.0, tf_burst=1500.0, tf_sustained=1500.0, src="fallback (B200_PROFILING.md)")
-
-
-def load_traffic(workload):
-    """dram bytes per launch from the committed `ncu --set full` capture (profiles/traffic.json)."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))[workload]["dram_bytes_per_launch"]
-    except Exception:
-        return None
+        # NVIDIA's H100 SXM data sheet: 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s (700 W card)
+        return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, src="H100 SXM data sheet")
 
 
 def trimmed_stats(ms):
@@ -262,12 +257,9 @@ def run_reference(args, wl):
     cores = pick_cpu_threads(wl, K)
     arm = CpuArm(wl, K)
     n_warm = max(min(args.warmup, 5), 1)
-    t0 = time.perf_counter()
     for _ in range(n_warm):
         arm.step()
-    t_step = (time.perf_counter() - t0) / n_warm
-    # bounded: the timed region stays under ~2 minutes whatever --steps asks for (at least 10 commands)
-    steps = max(min(args.steps, int(120.0 / t_step)), min(args.steps, 10))
+    steps = args.steps
     t0 = time.perf_counter()
     for _ in range(steps):
         arm.step()
@@ -342,7 +334,7 @@ def run_engine(args, wl):
     ctrl = make_engine(eng, wl, K_global, dev, pg, args.exchange)
     assert ctrl._model is not None, "fused route not selected"
     x_dev = torch.tensor(wl["x0"], dtype=torch.float32, device=dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > the 50 MB L2 of an H100
 
     def barrier():
         if world > 1:
@@ -388,13 +380,15 @@ def run_engine(args, wl):
         for e0, e1 in evs:
             flush.zero_()
             e0.record(stream)
-            ctrl.command(x_dev)
+            a_last = ctrl.command(x_dev)
             e1.record(stream)
         torch.cuda.synchronize()
         step_ms += [e0.elapsed_time(e1) for e0, e1 in evs]
         done += n
     barrier()
     t_end = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, a_last, ctrl)
     stats = trimmed_stats(step_ms)
     # max over ranks of the per-rank figures (every rank times the same K steps)
     agg = torch.tensor([stats["trimmed_mean"], stats["mean"], stats["median"], stats["min"]], dtype=torch.float64, device=dev)
@@ -406,7 +400,7 @@ def run_engine(args, wl):
 
     # ---- back-to-back launches (no flush): the steady-state command rate ---------------------------
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    nb2b = max(min(args.steps, 2000), 200)
+    nb2b = args.steps
     barrier()
     e0.record(stream)
     for _ in range(nb2b):
@@ -423,7 +417,7 @@ def run_engine(args, wl):
     for _ in range(20):
         ctrl.command_host(x_host)
     barrier()
-    n_e2e = max(args.steps, 2000) if K_gpu * T < 4_000_000 else max(min(args.steps, 2000), 300)
+    n_e2e = args.steps
     t0 = time.perf_counter()
     for _ in range(n_e2e):
         a_host = ctrl.command_host(x_host)
@@ -480,26 +474,26 @@ def run_engine(args, wl):
         t_s = ms_per_step * 1e-3
         hbm_achieved = b_full / t_s / 1e9
         lane_ops = wl["lane_ops"] * K_loc * T / t_s
-        lane_peak = info.sm_count * 128 * (clocks["sm_max_mhz"] or 1965.0) * 1e6
+        lane_peak = info.sm_count * 128 * (clocks["sm_max_mhz"] or 1980.0) * 1e6
         if wl["model"] == "mlp":
             tf = wl["flop_per_step"] * K_loc * T / t_s / 1e12
             roofline = {"bound": "tensor", "achieved": tf, "peak": peaks["tf_sustained"], "unit": "TFLOP/s",
-                        "frac": tf / peaks["tf_sustained"], "traffic": load_traffic(args.workload),
+                        "frac": tf / peaks["tf_sustained"],
                         "peak_source": peaks["src"] + " bf16_tflops_sustained (kernel timed inside a long step)",
                         "algorithmic_flop_per_launch": wl["flop_per_step"] * K_loc * T,
-                        "note": "useful MLP math only (2,368 flop per rollout-step, SURVEY 8a); bf16x3 issues 7 MMAs per "
-                                "layer-triple for fp32-grade layer outputs, N=32 tiles: the step is bound by the "
-                                "tanh/convert epilogue and the MMA round trips, not by tensor throughput",
+                        "note": "useful MLP math only (2,368 flop per rollout-step, SURVEY 8a); bf16x3 issues 3 MMAs per "
+                                "K step for fp32-grade layer outputs, N=32 tiles: the step is bound by the tanh/convert "
+                                "epilogue and the MMA round trips, not by tensor throughput",
                         "hbm_achieved_GBps": hbm_achieved, "hbm_frac": hbm_achieved / peaks["hbm"], "lane_ops_frac": lane_ops / lane_peak}
         else:
             roofline = {"bound": "latency/issue", "achieved": lane_ops / 1e12, "peak": lane_peak / 1e12, "unit": "Tlane-op/s",
-                        "frac": lane_ops / lane_peak, "traffic": load_traffic(args.workload),
+                        "frac": lane_ops / lane_peak,
                         "peak_source": "SMs x 128 FP32 lanes x max SM clock (nvidia-smi); HBM peak: " + peaks["src"] + " hbm_gbs",
                         "lane_ops_per_rollout_step": wl["lane_ops"],
                         "hbm": {"achieved": hbm_achieved, "peak": peaks["hbm"], "unit": "GB/s", "frac": hbm_achieved / peaks["hbm"],
                                 "algorithmic_bytes_per_launch": b_full, "algorithmic_bytes_min_per_launch": b_min,
                                 "frac_min_bytes": b_min / t_s / 1e9 / peaks["hbm"]},
-                        "note": "the fused analytic rollout moves ~B_min bytes per launch (traffic) and is bound by FP32/SFU "
+                        "note": "the fused analytic rollout moves ~B_min bytes per launch and is bound by FP32/SFU "
                                 "issue and dependent-issue latency, not HBM (SURVEY 8d); frac = lane-op fraction"}
         line = {
             "metric": "K*T rollout-steps/s through command()", "value": value, "unit": "rollout-steps/s",
@@ -556,10 +550,21 @@ def run_engine(args, wl):
         dist.destroy_process_group()
 
 
+def dump_outputs(out_dir, action, ctrl):
+    """What a caller of command() receives from the last timed step, as float32/float64 .npy files (a few hundred KB at
+    the largest workload)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in (("action", action), ("U", ctrl.U), ("cost_total", ctrl.cost_total)):
+        a = t.detach().cpu()
+        a = a.double() if a.dtype == torch.float64 else a.float()
+        np.save(os.path.join(out_dir, name + ".npy"), a.numpy())
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=10000)
+    ap.add_argument("--steps", type=int, default=10000, help="timed command() calls (each timing loop runs this many)")
     ap.add_argument("--warmup", type=int, default=50)
     ap.add_argument("--impl", default="engine", choices=["engine", "reference"])
     ap.add_argument("--workload", default="pendulum_c2", choices=sorted(WORKLOADS))
@@ -569,15 +574,21 @@ def main():
                     help="mlp_c4 operand precision on the tensor cores: hi/lo-split bf16 (fp32-grade layer outputs, the parity "
                          "route) or plain bf16")
     ap.add_argument("--cpu-seconds", type=float, default=10.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed command() as DIR/<name>.npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-shard-check", action="store_true")
     ap.add_argument("--no-resident", action="store_true",
                     help="e2e on the launch route only (default at N=1: also time the host loop on a resident grid, "
                          "csrc/mppi_resident.cuh, and report the faster one as e2e)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the engine's outputs; it does not apply to --impl reference")
     wl = WORKLOADS[args.workload]
     if args.impl == "reference":
-        run_reference(args, wl)      # bounds its own step count
+        run_reference(args, wl)
     else:
         run_engine(args, wl)
 

@@ -1,5 +1,5 @@
 /*
- * mppi_b200.h — C ABI of the B200-native MPPI rollout-and-reweight engine.
+ * mppi_b200.h — C ABI of the H100-native MPPI rollout-and-reweight engine.
  *
  * The reference (UM-ARM-Lab/pytorch_mppi) is pure Python and has no FFI; the drop-in boundary is
  * its Python class API (SURVEY.md §8b).  This header is the boundary *below* that API: the Python
@@ -11,7 +11,7 @@
  *   - is not re-entrant per controller (one controller <-> one stream, as the reference).
  *
  * Each entry point cites the reference code it replaces (file:line into
- * /root/reference/src/pytorch_mppi/mppi.py).
+ * reference src/pytorch_mppi/mppi.py).
  */
 #ifndef MPPI_B200_H
 #define MPPI_B200_H
@@ -47,7 +47,7 @@ typedef enum MppiDType { MPPI_F32 = 0, MPPI_F64 = 1 } MppiDType;
  * (The reference takes arbitrary Python callables, mppi.py:147-157; arbitrary callables use the
  * per-step entry points further down.) */
 typedef enum MppiModel {
-    MPPI_MODEL_PENDULUM = 1,      /* /root/reference/tests/pendulum.py:30-60                      */
+    MPPI_MODEL_PENDULUM = 1,      /* reference tests/pendulum.py:30-60                      */
     MPPI_MODEL_LINEAR_POINT = 2,  /* tests/test_mppi.py:24-51 and tests/smooth_mppi.py:29-142    */
     MPPI_MODEL_PENDULUM_MLP = 3,  /* tests/pendulum_approximate.py:47-67 (3-32-32-2 tanh residual MLP) */
     MPPI_MODEL_USER = 100         /* a user-written model compiled into a variant of this library (build with
@@ -62,7 +62,7 @@ typedef enum MppiModel {
  *                 [15]=terminal_scale [16]=n_hills(<=3) then per hill h at 17+7h:
  *                 Qh(4) centre(2) height(1)
  *  PENDULUM_MLP : [0]=max_torque [1]=w_thdot [2]=tanh_mode(0 exp-based, 1 MUFU.TANH) [3]=tensor_cores (0 = FFMA kernel;
- *                 tcgen05/TMEM kernel, fp32 accumulate: 1 = hi/lo-split bf16 operands, 2 = plain bf16; 3 = automatic:
+ *                 wgmma kernel, fp32 accumulate: 1 = hi/lo-split bf16 operands, 2 = plain bf16; 3 = automatic:
  *                 mode 1 wherever that kernel exists — fp32, one environment — else the FFMA kernel); the 1,250 weights go in
  *                 model_params_ext: W1 (32x3 row-major), b1 (32), W2 (32x32), b2 (32), W3 (2x32), b3 (2)
  */

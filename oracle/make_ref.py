@@ -8,7 +8,7 @@ It copies the reference's pure-Python package files where they lie (`/root/refer
 and its own test-suite (`/root/reference/tests/test_mppi.py`, used by tests/test_gpu_ref_suite.py) into `oracle/_ref/`,
 and writes the `arm_pytorch_utilities` stand-in next to them (tests/golden/_shim; the real dependency is not
 vendored with the reference and there is no network).  `oracle/_ref/` is git-ignored — reference sources never enter
-the history — but NOT gpurun-ignored, so it travels to the GPU box with the snapshot, where `bench.py --impl reference`
+the history — but it travels with a copy of the working tree to a GPU machine, where `bench.py --impl reference`
 and the `cpu_baseline` leg time it (kind "reference") and the reference's own tests run against the engine.
 Nothing in the product imports it.
 """

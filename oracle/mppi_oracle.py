@@ -8,7 +8,7 @@ missing instead of falling back to this).
 
 It is a functional restatement (torch-CPU tensor ops, explicit state in / state
 out, no classes with hidden RNG) of the algorithm in the reference
-``/root/reference/src/pytorch_mppi/mppi.py``.  Torch CPU ops are used (rather
+``reference src/pytorch_mppi/mppi.py``.  Torch CPU ops are used (rather
 than numpy) because every flop of the reference runs in torch: using the same
 ATen kernels makes the oracle *bit-identical* to the reference in fp32 and fp64
 when both consume the same standard-normal draws ``z`` — see
@@ -33,7 +33,7 @@ import torch
 # Workload definitions (the analytic models BASELINE.json's configs are quoted on)
 # --------------------------------------------------------------------------------------
 class PendulumModel:
-    """Gym pendulum, restating /root/reference/tests/pendulum.py:30-60.
+    """Gym pendulum, restating reference tests/pendulum.py:30-60.
 
     dynamics : u <- clamp(u, +-max_torque); thdot' = clip(thdot + (3g/(2l) sin th + 3/(m l^2) u) dt, +-max_speed)
                th' = th + thdot' dt                         (velocity clipped BEFORE integrating th)
@@ -79,10 +79,10 @@ class LinearPointModel:
     optional Gaussian 'hill' costs and an optional terminal cost.
 
     With B=diag(1,-1), Q=I, R=0, no hills it is the fixture environment of the reference's
-    unit tests (/root/reference/tests/test_mppi.py:24-51).  With B=diag(.5,-.5), R=0.01 I,
+    unit tests (reference tests/test_mppi.py:24-51).  With B=diag(.5,-.5), R=0.01 I,
     one hill (Q_h=2.5*[[.1,.05],[.05,.1]], centre (-.5,-1), height 200), goal (2,2) and
     terminal_scale=10 it is the Toy2D navigation environment of
-    /root/reference/tests/smooth_mppi.py:29-36,50-76,102-111,131-142 (BASELINE config 3).
+    reference tests/smooth_mppi.py:29-36,50-76,102-111,131-142 (BASELINE config 3).
     Quadratic forms are evaluated as sum_i sum_j d_i Q_ij d_j per row (the reference delegates
     to arm_pytorch_utilities.linalg.batch_quadratic_product, which is not vendored).
     """
@@ -130,7 +130,7 @@ class LinearPointModel:
 
 class MlpPendulumModel:
     """Learned pendulum dynamics of BASELINE config 4, restating the plugins of
-    /root/reference/tests/pendulum_approximate.py:54-66, 100-110 around a given 3-32-32-2 tanh network:
+    reference tests/pendulum_approximate.py:54-66, 100-110 around a given 3-32-32-2 tanh network:
     x' = x + net([x, clamp(u, +-2)]), theta' wrapped to [-pi, pi); cost as the analytic pendulum."""
     nx, nu = 2, 1
     has_terminal = False

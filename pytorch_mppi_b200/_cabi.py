@@ -1,6 +1,6 @@
 """ctypes binding of the C-ABI library (include/mppi_b200.h -> csrc/libmppi_b200.so).
 
-The library is built in-tree by ``pytorch_mppi_b200.build`` (nvcc, sm_100a).  There is NO fallback:
+The library is built in-tree by ``pytorch_mppi_b200.build`` (nvcc, sm_90a).  There is NO fallback:
 if the shared object is missing or a symbol is absent, importing the controllers raises.
 """
 from __future__ import annotations
@@ -188,7 +188,7 @@ def load(path=None):
     if not os.path.exists(path):
         raise MppiLibraryError(
             f"{path} not found: build it with `python -m pytorch_mppi_b200.build` "
-            "(nvcc, sm_100a). pytorch_mppi_b200 has no CPU or eager-PyTorch fallback.")
+            "(nvcc, sm_90a). pytorch_mppi_b200 has no CPU or eager-PyTorch fallback.")
     lib = C.CDLL(path)
     for name, restype, argtypes in SYMBOLS:
         try:

@@ -1,8 +1,8 @@
-"""In-tree build of the C-ABI CUDA library for sm_100a:  python -m pytorch_mppi_b200.build [--force] [-v]
+"""In-tree build of the C-ABI CUDA library for sm_90a:  python -m pytorch_mppi_b200.build [--force] [-v]
 
 nvcc cross-compiles without a GPU.  The library is several translation units compiled in parallel (one per
 registered model x dtype plus the C-ABI / model-independent unit) and linked into ONE shared object, which stays
-in-tree (git-ignored, but shipped to the GPU box by gpurun) so the driver sees which native code the tests loaded.
+in-tree (git-ignored) so that a copy of the built tree carries the native code its tests load.
 Objects are cached under csrc/_obj/ keyed by the hash of everything they are compiled from, so touching one
 kernel header rebuilds only the units that include it.
 """
@@ -30,7 +30,7 @@ COMMON_HEADERS = _h("mppi_host.cuh", "mppi_fused.cuh", "mppi_math.cuh", "mppi_re
 MODEL_HEADERS = COMMON_HEADERS + _h("mppi_mlp_tc.cuh")
 CABI_HEADERS = COMMON_HEADERS + _h("mppi_fused_host.cuh")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC"]
 
 # name -> (source, extra defines, headers it depends on)
 UNITS = {"cabi": ("mppi_b200.cu", [], CABI_HEADERS)}
@@ -50,7 +50,7 @@ def _unit_hash(src, defines, headers, extra_text=""):
 
 def source_hash() -> str:
     """Hash of everything the library is compiled from (sources, headers, flags).  File times are not used: the
-    snapshot that ships the tree to a GPU box does not promise to keep them, and a spurious rebuild there costs
+    copy that ships a built tree to a GPU machine need not keep them, and a spurious rebuild there costs
     GPU minutes."""
     h = hashlib.sha1()
     for name in sorted(UNITS):
@@ -87,7 +87,7 @@ def _compile_unit(name, src, defines, headers, verbose=False, extra_text="", obj
 
 def _link(objs, out):
     nvcc = os.environ.get("NVCC", "nvcc")
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-o", out, *objs]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-o", out, *objs]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{' '.join(cmd)}\n{r.stdout}\n{r.stderr}")

@@ -1,5 +1,5 @@
 // mppi_b200.cu — C-ABI entry points (include/mppi_b200.h) and kernel dispatch.
-// Built with: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -shared -Xcompiler -fPIC
+// Built with: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -shared -Xcompiler -fPIC
 // No torch types cross this boundary; the Python side binds it with ctypes.
 //
 // Translation units of the library (built in parallel by pytorch_mppi_b200/build.py):

@@ -7,14 +7,13 @@
 namespace {
 
 // ---- fused command ----------------------------------------------------------------------------
-// PENDULUM_MLP in fp32 with model_params[3] != 0: the tcgen05/TMEM kernel (mppi_mlp_tc.cuh).  One CTA = 256 threads = 128
-// samples (two threads per sample) = the 128 lanes of an M=128 accumulator tile; it does not take part in PDL.
+// PENDULUM_MLP in fp32 with model_params[3] != 0: the wgmma kernel (mppi_mlp_tc.cuh).  One CTA = 256 threads = 128
+// samples (two threads per sample) = two warpgroups of 64 accumulator rows; it does not take part in PDL.
 inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedParams* p, MppiFusedParams& p_tc, const void*& kernel) {
     if (mk->is_mlp && !mk->is_double) {
         int mode = (int)p->model_params[3];            // 1: hi/lo-split bf16 operands ("3 x bf16"), 2: plain bf16, 3: automatic
         // automatic (the Python default): the tensor-core kernel with split operands — the parity route — wherever it
-        // exists (fp32, one environment); it is faster than the FFMA kernel at every K from 1024 to 131072
-        // (profiles/r02_c4_routes.txt: 78 against 113 us at K = 1024, 102 against 141 at 32768, 320 against 337 at 131072)
+        // exists (fp32, one environment)
         if (mode == 3) mode = 1;
         const int fast = p->model_params[2] != 0.0 ? 1 : 0;
         if ((mode == 1 || mode == 2) && p->n_env <= 1 && mk->tc[p->variant][mode - 1][fast] != nullptr) {
@@ -23,8 +22,6 @@ inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedPara
             p_tc.threads_per_sample = 2;
             p_tc.flags &= ~(uint32_t)MPPI_FLAG_PDL;
             kernel = mk->tc[p->variant][mode - 1][fast];
-            g_tc_kernel = 1;
-            g_tc_cols = 64;                             // tc::TMEM_COLS (mppi_mlp_tc.cuh)
             // co-residency is bounded by shared memory: ask for the largest carve-out
             cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
             return true;
@@ -35,7 +32,7 @@ inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedPara
 
 // ---- kernel + launch geometry of one fused command -------------------------------------------------------------------
 // What is decided here, once per plan (or per mppi_fused_command call):
-//   kernel     fused_command_kernel<Model, real, V, batched, split>  (or the tcgen05 kernel, select_tensor_core_route)
+//   kernel     fused_command_kernel<Model, real, V, batched, split>  (or the wgmma kernel, select_tensor_core_route)
 //   geometry   tile size / helper threads / grid (plan_geometry), planned for K_geom samples on sharded controllers so
 //              that every rank launches the same grid
 //   split      MPPI_FLAG_SPLIT_COST honoured: problems small enough to run with helper threads (threads_per_sample > 1)
@@ -71,7 +68,6 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     int rc;
     if (tc_route) {
         rc = plan_geometry(kernel, &pg, es, 0, false, g, layout_fn<real>);
-        g_tc_kernel = 0;
         if (rc) return rc;
         c = FusedChoice{kernel, g, 0, 0, 1};
         return MPPI_OK;

@@ -318,8 +318,6 @@ struct GeomKey {
 
 // Launch geometry for (kernel, dimensions).  The occupancy / attribute queries cost microseconds, so
 // the last few results are cached per thread: a steady-state command() pays only the lookup.
-static thread_local int g_tc_kernel = 0;   // set around plan_geometry() for the tcgen05 kernels (see below)
-static thread_local int g_tc_cols = 64;    // TMEM columns one CTA of that kernel allocates
 template <typename KernelT>
 int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_rows2, bool single_partial_grid, Geometry& g,
                   SmemLayout (*layout)(int, int, int, int, int, int, int, int, int)) {
@@ -345,8 +343,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_row
     // the reduction order must not depend on scheduling), so the finish time follows the most
     // loaded SM.  Enumerate BS in steps of a warp and j = resident CTAs per SM, size the grid as
     // min(n_tiles, SMs*j), and keep the candidate with the smallest worst-case samples per SM
-    // (ties: fewer passes, then more threads).  Measured on B200 (scripts/geom_sweep.py) this picks
-    // the winners of an exhaustive sweep within ~3 %: e.g. K=131072 -> BS=448, 293 CTAs, one pass.
+    // (ties: fewer passes, then more threads).
     int BS = p->block_threads;
     int tps = p->threads_per_sample;
     int grid_hint = 0;
@@ -415,20 +412,6 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_row
         if (L.total > dyn_limit) return UNSUPPORTED("shared-memory tile does not fit");
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, BD, L.total));
         if (occ < 1) return UNSUPPORTED("kernel does not fit on an SM with this block size");
-        if (g_tc_kernel) {
-            // The occupancy API answers 1 CTA/SM for kernels that allocate tensor memory; measured on B200 the
-            // 128-thread tcgen05 CTAs do co-reside (K=131072, T=30: 585 us at 1 CTA/SM, 379 at 2, 311 at 3), so
-            // size the grid from the real limits: shared memory, registers, and the CTA's share of the 512 TMEM columns.
-            int smem_sm = 0;
-            CK(cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
-            const int by_smem = smem_sm / ((int)fa.sharedSizeBytes + L.total + 1024);
-            const int by_regs = 65536 / (((fa.numRegs + 7) / 8 * 8) * BD);
-            int o = by_smem < by_regs ? by_smem : by_regs;
-            if (o > 512 / g_tc_cols) o = 512 / g_tc_cols;
-            const char* e = getenv("MPPI_TC_OCC");
-            if (e != nullptr && atoi(e) > 0) o = atoi(e);
-            if (o > occ) occ = o;
-        }
         int nb2 = n_tiles < di.sm_count * occ ? n_tiles : di.sm_count * occ;
         if (nb2 > cap) nb2 = cap;
         if (p->grid_blocks > 0 && p->grid_blocks < nb2) nb2 = p->grid_blocks;

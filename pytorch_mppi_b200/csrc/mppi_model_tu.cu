@@ -1,6 +1,6 @@
 // mppi_model_tu.cu — one translation unit per (registered model, dtype): the fused command kernels
 // (fused_command_kernel<Model, real, V, ...>, all variants and instantiations), the resident command kernels and the
-// states kernel of that model — and, for the fp32 MLP, the tcgen05 kernels.  The unit contains no launch logic: it
+// states kernel of that model — and, for the fp32 MLP, the wgmma kernels.  The unit contains no launch logic: it
 // exports ONE symbol, mppi_host::model_kernels_<model>_<dtype>(), a table of kernel handles plus the parameter packer,
 // which the generic host code in mppi_b200.cu (mppi_fused_host.cuh) works on.
 //

@@ -5,7 +5,7 @@ The reference's plugin surface is a pair of Python callables ``dynamics(state, a
 inlined into CUDA, so the fused path recognises callables that are *bound methods of a registered
 model object*: pass ``model.dynamics`` / ``model.running_cost`` (and optionally
 ``model.terminal_cost``) to the controller exactly as you would pass your own functions, and the
-controller launches the fused sm_100a kernel.  The same bound methods are ordinary torch functions
+controller launches the fused sm_90a kernel.  The same bound methods are ordinary torch functions
 (any device, any dtype), so they also serve as the simulator you step your real system with and as
 the callables of the per-step path.
 
@@ -49,7 +49,7 @@ class AnalyticModel:
 
 class Pendulum(AnalyticModel):
     """Gym pendulum swing-up, the model of BASELINE configs 1/2/5
-    (/root/reference/tests/pendulum.py:30-60): state (theta, theta_dot), one torque input.
+    (reference tests/pendulum.py:30-60): state (theta, theta_dot), one torque input.
 
         u      <- clamp(u, +-max_torque)
         thdot' =  clip(thdot + (3g/(2l) sin(theta) + 3/(m l^2) u) dt, +-max_speed)
@@ -89,8 +89,8 @@ class LinearPoint(AnalyticModel):
     ``h exp(-(c-x)^T Q_h (c-x))`` and an optional terminal cost ``terminal_scale * state_cost(x_T)``.
 
     `LinearPoint.unit_test_env()` is the fixture of the reference's test-suite
-    (/root/reference/tests/test_mppi.py:24-51); `LinearPoint.toy2d_nav()` is the Toy2D navigation
-    environment of /root/reference/tests/smooth_mppi.py:79-142 (BASELINE config 3).
+    (reference tests/test_mppi.py:24-51); `LinearPoint.toy2d_nav()` is the Toy2D navigation
+    environment of reference tests/smooth_mppi.py:79-142 (BASELINE config 3).
     """
     model_id = _cabi.MODEL_LINEAR_POINT
     nx, nu = 2, 2
@@ -166,7 +166,7 @@ class LinearPoint(AnalyticModel):
 
 
 class PendulumMLP(AnalyticModel):
-    """Learned pendulum dynamics of BASELINE config 4 (/root/reference/tests/pendulum_approximate.py:47-67):
+    """Learned pendulum dynamics of BASELINE config 4 (reference tests/pendulum_approximate.py:47-67):
     ``x' = x + net([x, clamp(u)])`` with ``net = Linear(3,32)-Tanh-Linear(32,32)-Tanh-Linear(32,2)``, then the
     angle is wrapped to [-pi, pi); running cost as the analytic pendulum.
 
@@ -187,7 +187,7 @@ class PendulumMLP(AnalyticModel):
             raise ValueError("PendulumMLP expects Linear(3,32)-Tanh-Linear(32,32)-Tanh-Linear(32,2); got " + str(shapes))
         self.net = net
         self.max_torque, self.w_thdot, self.fast_tanh = float(max_torque), float(w_thdot), bool(fast_tanh)
-        # tensor_cores (fp32 controllers only): the three layers run as tcgen05 MMAs with TMEM accumulators
+        # tensor_cores (fp32 controllers only): the hidden and output layers run as wgmma MMAs with fp32 accumulators
         # (csrc/mppi_mlp_tc.cuh).  True / "bf16x3": operands are hi/lo-split bf16, layer outputs agree with the
         # fp32 FFMA kernel to ~1e-5 relative.  "bf16": plain bf16 operands for the two hidden-layer products
         # (~2^-8 relative; the state inputs stay split), the fastest route.

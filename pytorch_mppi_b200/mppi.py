@@ -1,5 +1,5 @@
 """MPPI / SMPPI / KMPPI controllers with the reference's constructor + ``command()`` API
-(/root/reference/src/pytorch_mppi/mppi.py:35-688), executing on hand-written sm_100a kernels.
+(reference src/pytorch_mppi/mppi.py:35-688), executing on hand-written sm_90a kernels.
 
 Two execution routes, chosen at construction:
 
@@ -71,7 +71,7 @@ def _pad16(n_elems, es):
 
 
 class MPPI:
-    """Model Predictive Path Integral control (Williams et al. 2017, alg. 2), B200 engine.
+    """Model Predictive Path Integral control (Williams et al. 2017, alg. 2), CUDA engine.
     Constructor and methods mirror the reference (mppi.py:45-61, 208-290, 425-448)."""
 
     _VARIANT = _cabi.VARIANT_MPPI
@@ -461,7 +461,7 @@ class MPPI:
             self.launch_info = info
             need = int(info.workspace_bytes)
         else:
-            need = 32 + 148 * 16 * (4 + self._noise_rows()) * 8 + 256 + 2 * 12288 * 8
+            need = 32 + self._max_grid() * (4 + self._noise_rows()) * 8 + 256 + 2 * 12288 * 8
         if self._workspace is None or self._workspace.numel() < need:
             self._workspace = torch.zeros(need, device=self.d, dtype=torch.uint8)
         p.workspace = self._workspace.data_ptr()
@@ -475,6 +475,10 @@ class MPPI:
         self._dirty = False
         if self._model is not None:
             self._make_plan(p)
+
+    def _max_grid(self):
+        """Largest grid the planner launches on this device: 16 CTAs per SM (mppi_host.cuh, plan_geometry)."""
+        return torch.cuda.get_device_properties(self.d).multi_processor_count * 16
 
     def _make_plan(self, p):
         """Freeze the launch state in the C library (`mppi_plan_create`): per command only the state,
@@ -1515,7 +1519,7 @@ class MPPI_Batched(MPPI):
     def _variant_pack(self, p):
         es = _ES[self.dtype]
         rows = self.T * self.nu
-        nb_max = min((self.K + 31) // 32 + 1, 148 * 16)
+        nb_max = min((self.K + 31) // 32 + 1, self._max_grid())
         stride = (max(16 + 2 * ((nb_max * es + 15) // 16 * 16) + ((nb_max * rows * es + 15) // 16 * 16),
                       16 + nb_max * (rows + 2) * 8) + 255) // 256 * 256 + 2 * 12288 * 8   # ws_bytes: partials / records + local mailbox
         self._env_ws_stride = (stride + 255) // 256 * 256

@@ -1,7 +1,7 @@
 """Run-time compilation of user-written analytic models with NVRTC (in process; no nvcc, no toolkit at run time).
 
 `CudaModel` (models.py) turns the user's `step` / `cost` / `terminal` bodies into a `struct mppi::UserModel`; this module
-compiles `csrc/mppi_fused.cuh + csrc/mppi_resident.cuh + that struct` for sm_100a — the SAME kernel templates the
+compiles `csrc/mppi_fused.cuh + csrc/mppi_resident.cuh + that struct` for sm_90a — the SAME kernel templates the
 registry models are built from — and returns the cubin with the lowered names of the instantiated kernels, which the
 C library loads (`mppi_user_model_register`: cudaLibraryLoadData + cudaLibraryGetKernel).  Compiled modules are cached
 on disk under csrc/_user/ keyed by the hash of everything they are built from, so a model compiles once (a few
@@ -21,7 +21,7 @@ import os
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 CACHE = os.path.join(CSRC, "_user")
-ARCH = "sm_100a"
+ARCH = "sm_90a"
 _KERNEL_HEADERS = ("mppi_fused.cuh", "mppi_math.cuh", "mppi_resident.cuh")
 
 _nvrtc = None

@@ -1,4 +1,4 @@
-"""GPU diagnostic: per-case parity table + quick command() timing.  Writes gpurun_out/diag.txt"""
+"""GPU diagnostic: per-case parity table + quick command() timing.  usage: gpu_diag.py [out.txt] (default: stdout only)"""
 import math
 import os
 import sys
@@ -14,14 +14,15 @@ from tests.golden.cases import CASES  # noqa: E402
 from tests.golden.replay import OracleRunner, load  # noqa: E402
 from tests.golden.engine import make_engine  # noqa: E402
 
-out = open(os.path.join(ROOT, "gpurun_out", "diag.txt"), "w")
+out = open(sys.argv[1], "w") if len(sys.argv) > 1 else None
 
 
 def P(*a):
     s = " ".join(str(x) for x in a)
     print(s, flush=True)
-    out.write(s + "\n")
-    out.flush()
+    if out is not None:
+        out.write(s + "\n")
+        out.flush()
 
 
 P(torch.cuda.get_device_name(0), torch.__version__)

@@ -1,4 +1,4 @@
-"""Summarise `ncu --set full` reports (read here, no GPU needed) into one JSON for profiles/.
+"""Summarise `ncu --set full` reports (read here, no GPU needed) into one JSON.
 usage: ncu_summary.py out.json name=report.ncu-rep [name=report.ncu-rep ...]"""
 import csv
 import io

@@ -1,5 +1,5 @@
 """BASELINE config 3 (2-D navigation, KMPPI, RBF(sigma=2), 5 support points, K=8192, T=40, fp32; SURVEY 8d /
-/root/reference/tests/smooth_mppi.py:539-560): device time per command for the three controllers on the same model,
+reference tests/smooth_mppi.py:539-560): device time per command for the three controllers on the same model,
 fused route (both rollouts) and stepped route.  Not under ncu."""
 import os
 import sys

@@ -28,7 +28,7 @@ for fast in (False, True):
 for mode in ("bf16x3", "bf16"):
     for fast in (False, True):
         m = eng.PendulumMLP(net, fast_tanh=fast, tensor_cores=mode)
-        run(f"fused   tcgen05 {mode} fast_tanh={fast}", m.dynamics, m.running_cost, 50)
+        run(f"fused   wgmma {mode} fast_tanh={fast}", m.dynamics, m.running_cost, 50)
 m = eng.PendulumMLP(net)
 run("stepped fp32 (torch MLP, Python T-loop)", lambda s, a: m.dynamics(s, a), lambda s, a: m.running_cost(s, a), 10)
 c = eng.MPPI(lambda s, a: m.dynamics(s, a), lambda s, a: m.running_cost(s, a), 2, torch.tensor(1.0), num_samples=K, horizon=T,

@@ -1,4 +1,4 @@
-"""Learned-dynamics rollout (BASELINE config 4 network), fp32: FFMA kernel vs tcgen05 kernel over K — picks the
+"""Learned-dynamics rollout (BASELINE config 4 network), fp32: FFMA kernel vs wgmma kernel over K — picks the
 crossover of the automatic route (PendulumMLP(tensor_cores="auto")).  Device time per command, back to back."""
 import os
 import sys

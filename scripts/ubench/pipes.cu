@@ -1,7 +1,7 @@
 // Issue-rate microbenchmark for the instruction mix of the tensor-core MLP epilogue (csrc/mppi_mlp_tc.cuh): how many
-// lanes per clock per SM do MUFU.EX2 / MUFU.RCP / MUFU.TANH / F2FP (cvt.rn.bf16x2.f32) / FFMA sustain on B200, alone and
+// lanes per clock per SM do MUFU.EX2 / MUFU.RCP / MUFU.TANH / F2FP (cvt.rn.bf16x2.f32) / FFMA sustain, alone and
 // mixed?  Decides how the tanh of that epilogue is built (2 MUFU vs 1 MUFU + FMA-pipe work).
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o gpurun_out/ubench_pipes scripts/ubench/pipes.cu && gpurun_out/ubench_pipes
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o /tmp/ubench_pipes scripts/ubench/pipes.cu && /tmp/ubench_pipes
 #include <cstdio>
 #include <cuda_runtime.h>
 
@@ -66,13 +66,14 @@ template <int OP> __global__ void bench(float* out, long long* clk) {
 template <int OP> void run(const char* name, int warps_per_sm) {
     float* out;
     long long* clk;
-    int nb = 148;
+    int nb = 0;
+    cudaDeviceGetAttribute(&nb, cudaDevAttrMultiProcessorCount, 0);     // one CTA per SM
     cudaMalloc(&out, nb * 1024 * 4);
     cudaMalloc(&clk, nb * 8);
     bench<OP><<<nb, warps_per_sm * 32>>>(out, clk);
     bench<OP><<<nb, warps_per_sm * 32>>>(out, clk);
     cudaDeviceSynchronize();
-    long long h[148];
+    long long h[1024];
     cudaMemcpy(h, clk, nb * 8, cudaMemcpyDeviceToHost);
     double c = 0;
     for (int i = 0; i < nb; ++i) c += (double)h[i];

@@ -1,6 +1,6 @@
 """Minimal stand-in for the un-vendored `arm_pytorch_utilities` dependency of the reference
 (pyproject.toml:57), used ONLY by tests/golden/make_golden.py to import the live reference in
-the build container.  Behaviour pinned by /root/reference/tests/test_batch_wrapper.py:19-47:
+the build container.  Behaviour pinned by reference tests/test_batch_wrapper.py:19-47:
 `handle_batch_input(n)` flattens extra leading batch dimensions so tensor arguments are n-D,
 calls the function and restores the leading dimensions on the outputs."""
 import functools

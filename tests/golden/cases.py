@@ -13,16 +13,16 @@ from oracle import mppi_oracle as orc
 _DT = {"f32": torch.float32, "f64": torch.float64}
 
 PENDULUM = {"kind": "pendulum"}
-# test-suite fixture environment (/root/reference/tests/test_mppi.py:24-51)
+# test-suite fixture environment (reference tests/test_mppi.py:24-51)
 LINEAR2D = {"kind": "linear_point", "B": [[1.0, 0.0], [0.0, -1.0]], "goal": [2.0, 2.0]}
 LINEAR2D_TERM = dict(LINEAR2D, terminal_scale=1.0)
-# Toy2D navigation (/root/reference/tests/smooth_mppi.py:79-142, main() :539-560)
+# Toy2D navigation (reference tests/smooth_mppi.py:79-142, main() :539-560)
 NAV2D = {"kind": "linear_point", "B": [[0.5, 0.0], [0.0, -0.5]], "goal": [2.0, 2.0],
          "R": [[0.01, 0.0], [0.0, 0.01]],
          "hills": [[[[0.25, 0.125], [0.125, 0.25]], [-0.5, -1.0], 200.0]],
          "terminal_scale": 10.0}
 
-# learned pendulum dynamics of BASELINE config 4 (/root/reference/tests/pendulum_approximate.py:31, 47-67):
+# learned pendulum dynamics of BASELINE config 4 (reference tests/pendulum_approximate.py:31, 47-67):
 # the 3-32-32-2 tanh network as torch initialises it right after torch.manual_seed(25) (the reference then trains it
 # against gym, which is not available here; the fixture stores the weights it was generated with)
 MLP_C4 = {"kind": "pendulum_mlp", "seed": 25}

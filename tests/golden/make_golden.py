@@ -1,7 +1,7 @@
 """Generate tests/golden/*.npz by running the LIVE reference (read-only at /root/reference) with
 injected standard-normal draws, and pin the oracle (oracle/mppi_oracle.py) bit-for-bit against it.
 
-Run in the build container only (the GPU box has no /root/reference):
+Run only where the reference sources are available:
 
     python tests/golden/make_golden.py
 
@@ -33,7 +33,7 @@ from tests.golden.cases import (BATCHED_CASES, CASES, build_problem, draw_z, mlp
 
 def ref_plugins(case, prob, model):
     """Plugins handed to the reference controller.  The pendulum is written with the same
-    np.sin / np.clip-on-tensor calls as /root/reference/tests/pendulum.py:30-60 so the fixture
+    np.sin / np.clip-on-tensor calls as reference tests/pendulum.py:30-60 so the fixture
     also pins that those equal the oracle's torch.sin / torch.clamp.  Every other model hands the reference the
     callables of the oracle's problem (the MLP network and the per-copy offset dynamics are torch callables)."""
     if case["model"]["kind"] == "pendulum":

@@ -1,5 +1,5 @@
 """GPU: API conformance with the reference's class surface.  Each test restates, for the CUDA engine,
-a behaviour the reference's own suite pins (/root/reference/tests/test_mppi.py — cited per test); both
+a behaviour the reference's own suite pins (reference tests/test_mppi.py — cited per test); both
 execution routes are exercised: `fused` (registered LinearPoint model) and `stepped` (plain callables)."""
 import numpy as np
 import pytest

@@ -1,8 +1,8 @@
-"""Multi-GPU (K sharded over ranks, SURVEY.md §8e): needs >= 2 CUDA devices (gpurun --gpus 2).
+"""Multi-GPU (K sharded over ranks, SURVEY.md §8e): needs >= 2 CUDA devices (run on a machine with two GPUs).
 Each rank rolls out its slice; the (beta, eta, V) records are exchanged (a) inside the kernel over
 NVLink peer mailboxes — the cluster records of every rank straight to every peer (direct mode) or one
 combined record per rank —, (b) with an NCCL all-gather + mppi_apply_partials; all must reproduce the
-unsharded update, identically on every rank.  The log of a 2-GPU run is kept under profiles/."""
+unsharded update, identically on every rank."""
 import os
 
 import pytest

@@ -1,12 +1,12 @@
-"""GPU: the reference's OWN test-suite (/root/reference/tests/test_mppi.py, 73 tests; its CI gate is
+"""GPU: the reference's OWN test-suite (its tests/test_mppi.py, 73 tests; its CI gate is
 .github/workflows/tests.yml:28-29) run against the engine.
 
-`oracle/make_ref.py` (build container, where /root/reference exists) writes an engine-pointed copy of that file into
+`oracle/make_ref.py` (run by build() where the reference sources are available) writes an engine-pointed copy of that file into
 the git-ignored `oracle/_ref/tests/test_mppi_engine.py` — identical except for the one-line `DEVICE = "cpu"` ->
 `"cuda"` (the engine has no CPU path) — and an alias package so that `from pytorch_mppi import MPPI, ...` resolves to
 `pytorch_mppi_b200`.  This test runs it in a subprocess and checks the outcome test by test: everything must pass except
 the entries of EXPECTED_FAIL, each with the reason it cannot hold for a CUDA-only engine.  The per-test report is
-written to gpurun_out/ref_suite_report.txt (copied to profiles/ by hand when it changes).
+written to tests/_reports/ref_suite_report.txt (tests/reports.py).
 """
 import os
 import re
@@ -15,20 +15,22 @@ import sys
 
 import pytest
 
+from tests import reports
+
 pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SUITE = os.path.join(ROOT, "oracle", "_ref", "tests", "test_mppi_engine.py")
 ALIAS = os.path.join(ROOT, "oracle", "_ref", "engine_alias")
 
-# test id (Class::name) -> why it cannot pass against this engine.  Filled from the first B200 run.
+# test id (Class::name) -> why it cannot pass against this engine.
 EXPECTED_FAIL = {
 }
 
 
 def test_reference_suite_against_the_engine():
     if not os.path.exists(SUITE):
-        pytest.skip("oracle/_ref not built (python oracle/make_ref.py in the build container)")
+        pytest.skip("oracle/_ref not built (python oracle/make_ref.py where the reference sources are available)")
     env = dict(os.environ)
     env["PYTHONPATH"] = os.pathsep.join([ALIAS, ROOT, env.get("PYTHONPATH", "")])
     r = subprocess.run([sys.executable, "-m", "pytest", SUITE, "-q", "-rA", "--no-header", "-p", "no:cacheprovider",
@@ -38,15 +40,14 @@ def test_reference_suite_against_the_engine():
     results = {}
     for m in re.finditer(r"^(PASSED|FAILED|ERROR|SKIPPED|XFAIL|XPASS)\s+\S*test_mppi_engine\.py::(\S+)", out, re.M):
         results[m.group(2)] = m.group(1)
-    os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-    with open(os.path.join(ROOT, "gpurun_out", "ref_suite_report.txt"), "w") as f:
+    try:
+        assert len(results) >= 70, f"suite did not run: {out[-3000:]}"
+        bad = {k: v for k, v in results.items() if v not in ("PASSED", "SKIPPED") and k not in EXPECTED_FAIL}
+        stale = [k for k in EXPECTED_FAIL if results.get(k) == "PASSED"]
+        assert not bad, f"unexpected failures against the engine: {bad}\n{out[-4000:]}"
+        assert not stale, f"listed as expected failures but passing: {stale}"
+    finally:
         n_pass = sum(v == "PASSED" for v in results.values())
-        f.write(f"reference suite against pytorch_mppi_b200: {n_pass} passed of {len(results)}\n")
-        for k in sorted(results):
-            f.write(f"{results[k]:8s} {k}" + (f"    # expected: {EXPECTED_FAIL[k]}" if k in EXPECTED_FAIL else "") + "\n")
-        f.write("\n---- raw tail ----\n" + out[-6000:])
-    assert len(results) >= 70, f"suite did not run: {out[-3000:]}"
-    bad = {k: v for k, v in results.items() if v not in ("PASSED", "SKIPPED") and k not in EXPECTED_FAIL}
-    stale = [k for k in EXPECTED_FAIL if results.get(k) == "PASSED"]
-    assert not bad, f"unexpected failures against the engine: {bad}\n{out[-4000:]}"
-    assert not stale, f"listed as expected failures but passing: {stale}"
+        lines = [f"reference suite against pytorch_mppi_b200: {n_pass} passed of {len(results)}"]
+        lines += [f"{results[k]:8s} {k}" + (f"    # expected: {EXPECTED_FAIL[k]}" if k in EXPECTED_FAIL else "") for k in sorted(results)]
+        reports.write("ref_suite_report.txt", "\n".join(lines) + "\n\n---- raw tail ----\n" + out[-6000:])

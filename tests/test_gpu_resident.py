@@ -3,17 +3,17 @@
 The contract is bit-identity with the launch route: the resident kernel runs the same stage functions on the same
 (state, seed, Philox counter, flags), so every action, the nominal sequence and cost_total must be EQUAL, not close.
 
-Validated on B200 in round 1 (profiles/r01_pytest_gpu_resident.txt).  A resident kernel is a spin-waiting kernel, so
+A resident kernel is a spin-waiting kernel, so
 every test carries a timeout, the host side gives up after 10 s, and the kernel itself leaves after `idle_us` without a
 command.
 """
-import os
 import time
 
 import pytest
 import torch
 
 import pytorch_mppi_b200 as eng
+from tests import reports
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(120)]
 
@@ -120,7 +120,7 @@ def test_resident_refuses_what_it_cannot_run():
 
 def test_resident_latency_report():
     """Not an assertion about speed — writes the host-loop time per command of both routes (C2 shape) to
-    gpurun_out/resident_latency.txt for the profiles/ record."""
+    tests/_reports/resident_latency.txt."""
     lines = []
     for K, T in ((16384, 30), (4096, 30)):
         res = {}
@@ -143,7 +143,5 @@ def test_resident_latency_report():
                 c.stop_resident()
         lines.append(f"K={K} T={T} command_host: launch route {res['launch']:.2f} us, resident {res['resident']:.2f} us per command "
                      f"(Python host loop, pendulum stepped on the host)")
-    os.makedirs("gpurun_out", exist_ok=True)
-    with open("gpurun_out/resident_latency.txt", "w") as f:
-        f.write("\n".join(lines) + "\n")
+    reports.write("resident_latency.txt", "\n".join(lines) + "\n")
     print("\n".join(lines))

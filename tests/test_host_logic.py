@@ -293,7 +293,7 @@ def test_bf16_split_contraction_precision_model():
 
 def test_build_is_keyed_by_source_hash_not_file_times(tmp_path, monkeypatch):
     """The in-tree library is rebuilt when (and only when) the sources it was compiled from change: the stamp next to
-    the .so holds their hash, so a snapshot copy that scrambles file times does not trigger a rebuild on the GPU box."""
+    the .so holds their hash, so a snapshot copy that scrambles file times does not trigger a rebuild on the GPU machine."""
     from pytorch_mppi_b200 import build
     build.build()
     assert not build.needs_build()

@@ -80,7 +80,7 @@ def test_fp32_noise_floor_documented():
 
 
 def test_rbf_closed_form():
-    # /root/reference/tests/test_mppi.py:560-570 pins exp(-0.5) for unit-distance points at sigma=1
+    # reference tests/test_mppi.py:560-570 pins exp(-0.5) for unit-distance points at sigma=1
     from oracle.mppi_oracle import rbf_kernel
     t = torch.tensor([[0.0], [1.0]], dtype=torch.double)
     k = rbf_kernel(t, t, 1.0)

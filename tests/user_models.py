@@ -1,5 +1,5 @@
 """User-written CUDA models used by the tests (built into variant libraries by `__graft_entry__.build()` so the
-GPU box does not spend GPU time running nvcc)."""
+GPU machine does not spend GPU time running nvcc)."""
 import torch
 
 import pytorch_mppi_b200 as eng
