@@ -50,10 +50,10 @@ typedef enum MppiModel {
     MPPI_MODEL_PENDULUM = 1,      /* reference tests/pendulum.py:30-60                      */
     MPPI_MODEL_LINEAR_POINT = 2,  /* tests/test_mppi.py:24-51 and tests/smooth_mppi.py:29-142    */
     MPPI_MODEL_PENDULUM_MLP = 3,  /* tests/pendulum_approximate.py:47-67 (3-32-32-2 tanh residual MLP) */
-    MPPI_MODEL_USER = 100         /* a user-written model compiled into a variant of this library (build with
-                                     -DMPPI_USER_MODEL_HEADER=\"file\"; see pytorch_mppi_b200.models.CudaModel): the
+    MPPI_MODEL_USER = 100         /* a user-written model compiled at run time and registered with
+                                     mppi_user_model_register (see pytorch_mppi_b200.models.CudaModel): the
                                      reference accepts arbitrary Python callables (mppi.py:63-64) — this is the
-                                     compiled-in equivalent for analytic dynamics/costs                        */
+                                     compiled equivalent for analytic dynamics/costs                           */
 } MppiModel;
 
 /* model_params layouts (doubles):
@@ -178,14 +178,15 @@ typedef struct MppiFusedParams {
     void* xchg_status_host;      /* optional pinned HOST int64: the kernel stores MPPI_ERR_TIMEOUT there when a peer
                                     exchange timed out (the caller checks it before the next command)      */
     void* user_model;            /* model == MPPI_MODEL_USER: handle from mppi_user_model_register (a model compiled at
-                                    run time), or NULL for a model linked into a variant library            */
+                                    run time); required                                                     */
 } MppiFusedParams;
 
 typedef struct MppiLaunchInfo {
     int32_t block_threads, grid_blocks;
     int32_t smem_bytes, regs_per_thread;
     int32_t max_blocks_per_sm, sm_count;
-    uint64_t workspace_bytes;    /* minimum workspace for these dimensions                               */
+    uint64_t workspace_bytes;    /* workspace for these dimensions, per environment: enough for any grid they can be
+                                    planned with, so one allocation serves every route and geometry         */
     int32_t tma_staging;         /* 1 if the nominal sequence is staged with cp.async.bulk (TMA)         */
     int32_t threads_per_sample;
     int32_t split_cost;          /* 1 if MPPI_FLAG_SPLIT_COST was honoured for these dimensions          */
@@ -203,14 +204,17 @@ uint64_t mppi_abi_layout(int which);
 const char* mppi_status_string(int status);
 const char* mppi_last_cuda_error(void);
 
-/* Launch geometry / scratch needs for these parameters (no launch). */
+/* Launch geometry / scratch needs for these parameters (no launch).  With model == 0 (no fused model: the per-step
+ * entry points further down) only sm_count and workspace_bytes are filled in. */
 int mppi_fused_query(const MppiFusedParams* p, MppiLaunchInfo* out);
-/* The fused command (see struct comment).  `stream` is a cudaStream_t. */
+/* The fused command (see struct comment) as a one-shot plan: mppi_plan_create, one command with the struct's state /
+ * state_dev / flags / seed / offset / z / action_out / host_mailbox, mppi_plan_destroy.  `stream` is a cudaStream_t. */
 int mppi_fused_command(const MppiFusedParams* p, void* stream);
 
 /* ---- Plans: the steady-state fast path ----------------------------------------------------------
- * A plan freezes everything `mppi_fused_command` derives from an MppiFusedParams (kernel selection,
- * launch geometry, the pre-cast kernel argument block) so that one command costs one short call.
+ * A plan freezes everything a fused command derives from an MppiFusedParams (kernel selection, launch
+ * geometry, the pre-cast kernel argument block, the checks of its buffers, workspace and strides) so
+ * that one command costs one short call.
  * Per command only the start state, the RNG counter / injected-noise pointer, the flags that vary
  * (SHIFT, STATE_DEVICE, STATE_PER_SAMPLE) and the action destination change.  The multi-GPU epoch is
  * advanced inside the plan (every rank issues the same sequence of commands). */
@@ -234,10 +238,8 @@ int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint
  * itself after `idle_us` without a command (the next command relaunches it), so a device-wide synchronise is
  * never blocked for longer than that.  Results are bit-identical to mppi_plan_command_host with the same
  * (state, flags, seed, offset).  Available for plans that run the split-cost rollout (one tile per SM;
- * MPPI_FLAG_SPLIT_COST honoured — MppiLaunchInfo.split_cost) of the analytic registry models; others: MPPI_ERR_UNSUPPORTED.
- * A plan that is one shard of a multi-GPU controller with the in-kernel exchange (peer_slots set) runs the instantiation
- * whose records also carry the exchange epoch: every rank's host posts its own record, the finishers exchange over
- * NVLink inside the resident grids (validated on one GPU in round 1; the sharded instantiation is to be run on two).
+ * MPPI_FLAG_SPLIT_COST honoured — MppiLaunchInfo.split_cost) of single-GPU controllers (one environment, no peers, no
+ * EXPORT_PARTIAL); others: MPPI_ERR_UNSUPPORTED.
  *
  *   host_box      pinned host memory, zero-initialised, 64 + u_per_command*nu (x2 for f64) 8-byte words:
  *                 [0,32) command record | [32] sequence number of the last finished command | [33] exit word |

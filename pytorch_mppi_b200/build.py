@@ -40,8 +40,8 @@ for _mid, _mname in ((1, "pendulum"), (2, "linear_point"), (3, "pendulum_mlp")):
             "mppi_model_tu.cu", [f"-DMPPI_TU_MODEL={_mid}", f"-DMPPI_TU_F64={_f64}"], MODEL_HEADERS)
 
 
-def _unit_hash(src, defines, headers, extra_text=""):
-    h = hashlib.sha1((" ".join(NVCC_FLAGS + defines) + extra_text).encode())
+def _unit_hash(src, defines, headers):
+    h = hashlib.sha1(" ".join(NVCC_FLAGS + defines).encode())
     for d in [os.path.join(CSRC, src), *headers]:
         with open(d, "rb") as f:
             h.update(f.read())
@@ -65,12 +65,12 @@ def needs_build() -> bool:
         return f.read().strip() != source_hash()
 
 
-def _compile_unit(name, src, defines, headers, verbose=False, extra_text="", obj_dir=OBJ):
-    """Compile one unit into obj_dir/<name>.o unless an object with the same input hash is already there."""
-    os.makedirs(obj_dir, exist_ok=True)
-    obj = os.path.join(obj_dir, name + ".o")
+def _compile_unit(name, src, defines, headers, verbose=False):
+    """Compile one unit into csrc/_obj/<name>.o unless an object with the same input hash is already there."""
+    os.makedirs(OBJ, exist_ok=True)
+    obj = os.path.join(OBJ, name + ".o")
     stamp = obj + ".stamp"
-    want = _unit_hash(src, defines, headers, extra_text)
+    want = _unit_hash(src, defines, headers)
     if os.path.exists(obj) and os.path.exists(stamp) and open(stamp).read().strip() == want:
         return obj, ""
     nvcc = os.environ.get("NVCC", "nvcc")
@@ -158,40 +158,6 @@ def _build_locked(force: bool, verbose: bool) -> str:
             except OSError:
                 pass
     return OUT
-
-
-def build_user_model(header_text: str, verbose: bool = False) -> str:
-    """JIT-build a variant of the library with a user model in the registry: only the two user-model units (fp32, fp64)
-    are compiled (the generated header + the fused-kernel templates) and linked with the C-ABI unit from csrc/_obj/ —
-    the variant serves that model (and the model-independent stepped-route kernels), not the stock registry.
-    Cached by the hash of the header text and the kernel sources under csrc/_user/."""
-    tag = hashlib.sha1((header_text + source_hash()).encode()).hexdigest()[:16]
-    udir = os.path.join(CSRC, "_user")
-    os.makedirs(udir, exist_ok=True)
-    hdr = os.path.join(udir, f"user_model_{tag}.cuh")
-    out = os.path.join(udir, f"libmppi_b200_user_{tag}.so")
-    if os.path.exists(out):
-        return out
-    with _BuildLock():
-        if os.path.exists(out):
-            return out
-        return _build_user_model_locked(header_text, tag, udir, hdr, out, verbose)
-
-
-def _build_user_model_locked(header_text, tag, udir, hdr, out, verbose):
-    with open(hdr, "w") as f:
-        f.write(header_text)
-    base = _compile_all({"cabi": UNITS["cabi"]}, verbose)          # normally cached
-    units = {f"user_{tag}_{'f64' if f64 else 'f32'}": ("mppi_model_tu.cu", ["-DMPPI_TU_MODEL=100", f"-DMPPI_TU_F64={f64}",
-                                                                              f'-DMPPI_USER_MODEL_HEADER="{hdr}"'], MODEL_HEADERS)
-             for f64 in (0, 1)}
-    with concurrent.futures.ThreadPoolExecutor(max_workers=2) as ex:
-        futs = [ex.submit(_compile_unit, name, *spec, verbose, header_text, udir) for name, spec in units.items()]
-        uobjs = [f.result()[0] for f in futs]
-    tmp = out + f".{os.getpid()}.tmp"
-    _link(base + uobjs, tmp)
-    os.replace(tmp, out)
-    return out
 
 
 if __name__ == "__main__":

@@ -11,17 +11,13 @@
 namespace mppi_host {
 thread_local char g_cuda_err[512] = "";
 
-// one getter per (model, dtype) translation unit, all weak: the stock library links the six registry units, an
-// nvcc-built user-model variant library links this unit and the two units of that model only
-#define MPPI_KERNELS_DECL(name) const ModelKernels* name() __attribute__((weak))
-MPPI_KERNELS_DECL(model_kernels_pendulum_f32);
-MPPI_KERNELS_DECL(model_kernels_pendulum_f64);
-MPPI_KERNELS_DECL(model_kernels_linear_point_f32);
-MPPI_KERNELS_DECL(model_kernels_linear_point_f64);
-MPPI_KERNELS_DECL(model_kernels_pendulum_mlp_f32);
-MPPI_KERNELS_DECL(model_kernels_pendulum_mlp_f64);
-MPPI_KERNELS_DECL(model_kernels_user_f32);
-MPPI_KERNELS_DECL(model_kernels_user_f64);
+// one getter per (model, dtype) translation unit (mppi_model_tu.cu)
+const ModelKernels* model_kernels_pendulum_f32();
+const ModelKernels* model_kernels_pendulum_f64();
+const ModelKernels* model_kernels_linear_point_f32();
+const ModelKernels* model_kernels_linear_point_f64();
+const ModelKernels* model_kernels_pendulum_mlp_f32();
+const ModelKernels* model_kernels_pendulum_mlp_f64();
 }  // namespace mppi_host
 
 namespace {
@@ -49,19 +45,16 @@ const ModelKernels* find_kernels(const MppiFusedParams* p, int* rc) {
             }
             get = f32 ? model_kernels_pendulum_mlp_f32 : model_kernels_pendulum_mlp_f64;
             break;
-        case MPPI_MODEL_USER:
-            if (p->user_model != nullptr) {
-                const UserModelHandle* h = reinterpret_cast<const UserModelHandle*>(p->user_model);
-                if (h->magic != kUserMagic || h->mk.is_double != (f32 ? 0 : 1)) {
-                    *rc = MPPI_ERR_BAD_ARG;
-                    return nullptr;
-                }
-                return &h->mk;
+        case MPPI_MODEL_USER: {
+            const UserModelHandle* h = reinterpret_cast<const UserModelHandle*>(p->user_model);
+            if (h == nullptr || h->magic != kUserMagic || h->mk.is_double != (f32 ? 0 : 1)) {
+                *rc = MPPI_ERR_BAD_ARG;
+                return nullptr;
             }
-            get = f32 ? model_kernels_user_f32 : model_kernels_user_f64;
-            break;
+            return &h->mk;
+        }
     }
-    return get != nullptr ? get() : nullptr;      // nullptr: this library was linked without that unit
+    return get != nullptr ? get() : nullptr;
 }
 
 template <typename real>
@@ -96,6 +89,17 @@ inline int plan_launch(Plan* pl, cudaStream_t stream) {
         return MPPI_ERR_CUDA;
     }
     return MPPI_OK;
+}
+
+// one command on a plan: the per-command checks, the argument update and the launch
+int plan_command(Plan* pl, const double* state, const void* state_dev, uint32_t flags, uint64_t seed, uint64_t offset, const void* z,
+                 void* action_out, void* host_mailbox, cudaStream_t stream) {
+    if (pl == nullptr || action_out == nullptr) return MPPI_ERR_BAD_ARG;
+    if (state == nullptr && !(flags & MPPI_FLAG_STATE_DEVICE)) return MPPI_ERR_BAD_ARG;
+    if (pl->p.n_env > 1 && !(flags & MPPI_FLAG_STATE_DEVICE)) return MPPI_ERR_BAD_ARG;   // states are (n_env, nx) on the device
+    if (pl->is_double) plan_update<double>(pl, state, state_dev, flags, seed, offset, z, action_out, host_mailbox);
+    else plan_update<float>(pl, state, state_dev, flags, seed, offset, z, action_out, host_mailbox);
+    return plan_launch(pl, stream);
 }
 
 // ---- resident mode: the device backend of csrc/mppi_resident_host.h ---------------------------------
@@ -174,20 +178,12 @@ int resident_be_health(void* ctx) {
 static_assert(MPPI_RES_CMD_SHIFT == (unsigned)RES_CMD_SHIFT && MPPI_RES_CMD_STOP == (unsigned)RES_CMD_STOP, "record flags: host and device disagree");
 static_assert((int)RES_ERR_BAD_ARG == (int)MPPI_ERR_BAD_ARG && (int)RES_ERR_TIMEOUT == (int)MPPI_ERR_TIMEOUT, "status codes of the protocol header");
 
-int dispatch_fused(const MppiFusedParams* p, cudaStream_t s, MppiLaunchInfo* info) {
-    int rc = validate(p, true);
-    if (rc) return rc;
-    const ModelKernels* mk = find_kernels(p, &rc);
-    if (mk == nullptr) return rc;
-    return mk->is_double ? run_fused<double>(mk, p, s, info) : run_fused<float>(mk, p, s, info);
-}
-
 // ---- generic path: sample / softmin -------------------------------------------------------------
 template <typename real, int V, int NU>
 int run_sample(const MppiFusedParams* p, KArgs<real>& a_extra, cudaStream_t stream) {
     auto kernel = sample_kernel<real, V, NU>;
     Geometry g;
-    int rc = plan_geometry(kernel, p, (int)sizeof(real), V == V_KMPPI, true, g, layout_fn<real>);
+    int rc = plan_geometry<real>(kernel, p, V == V_KMPPI, true, g);
     if (rc) return rc;
     KArgs<real> a;
     fill_kargs<real>(p, a, g.BS, g.nb, g.tps);
@@ -244,7 +240,7 @@ template <typename real, int V, int NU>
 int run_softmin(const MppiFusedParams* p, const void* cost, const void* eps, cudaStream_t stream) {
     auto kernel = softmin_update_kernel<real, V, NU>;
     Geometry g;
-    int rc = plan_geometry(kernel, p, (int)sizeof(real), 0, false, g, layout_fn<real>);
+    int rc = plan_geometry<real>(kernel, p, 0, false, g);
     if (rc) return rc;
     const uint64_t need_ws = ws_bytes(g.nb, rows_of(p), (int)sizeof(real));
     if (p->workspace == nullptr || p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
@@ -324,10 +320,36 @@ const char* mppi_last_cuda_error(void) { return g_cuda_err; }
 int mppi_fused_query(const MppiFusedParams* p, MppiLaunchInfo* out) {
     if (out == nullptr) return MPPI_ERR_BAD_ARG;
     memset(out, 0, sizeof(*out));
-    return dispatch_fused(p, nullptr, out);
+    int rc = validate(p);
+    if (rc) return rc;
+    if (p->model == 0) {      // the per-step entry points: only the workspace mppi_softmin_update needs
+        DevInfo di;
+        if ((rc = get_dev_info(di)) != MPPI_OK) return rc;
+        out->sm_count = di.sm_count;
+        out->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p), p->dtype == MPPI_F64 ? 8 : 4);
+        return MPPI_OK;
+    }
+    if ((rc = validate(p, true)) != MPPI_OK) return rc;
+    const ModelKernels* mk = find_kernels(p, &rc);
+    if (mk == nullptr) return rc;
+    return mk->is_double ? query_fused<double>(mk, p, out) : query_fused<float>(mk, p, out);
 }
 
-int mppi_fused_command(const MppiFusedParams* p, void* stream) { return dispatch_fused(p, (cudaStream_t)stream, nullptr); }
+// a one-shot plan, with the record tags of a plan-less command: one process-wide counter on a single GPU (or with
+// EXPORT_PARTIAL), the caller's epoch on an in-kernel sharded controller (every rank issues the same sequence)
+int mppi_fused_command(const MppiFusedParams* p, void* stream) {
+    void* plan = nullptr;
+    int rc = mppi_plan_create(p, &plan);
+    if (rc) return rc;
+    Plan* pl = reinterpret_cast<Plan*>(plan);
+    static unsigned long long s_epoch = 0;
+    // plan_update pre-increments both tags
+    pl->epoch = sharded_in_kernel(p) ? p->epoch - 1 : __atomic_add_fetch(&s_epoch, 1ull, __ATOMIC_RELAXED) - 1;
+    pl->host_epoch = p->host_epoch - 1;
+    rc = plan_command(pl, p->state, p->state_dev, p->flags, p->seed, p->offset, p->z, p->action_out, p->host_mailbox, (cudaStream_t)stream);
+    delete pl;
+    return rc;
+}
 
 int mppi_plan_create(const MppiFusedParams* p, void** plan_out) {
     if (plan_out == nullptr) return MPPI_ERR_BAD_ARG;
@@ -355,12 +377,7 @@ int mppi_plan_destroy(void* plan) {
 
 int mppi_plan_command(void* plan, const double* state, const void* state_dev, uint32_t flags, uint64_t seed, uint64_t offset,
                       const void* z, void* action_out, void* stream) {
-    Plan* pl = reinterpret_cast<Plan*>(plan);
-    if (pl == nullptr || action_out == nullptr) return MPPI_ERR_BAD_ARG;
-    if (state == nullptr && !(flags & MPPI_FLAG_STATE_DEVICE)) return MPPI_ERR_BAD_ARG;
-    if (pl->is_double) plan_update<double>(pl, state, state_dev, flags, seed, offset, z, action_out, nullptr);
-    else plan_update<float>(pl, state, state_dev, flags, seed, offset, z, action_out, nullptr);
-    return plan_launch(pl, (cudaStream_t)stream);
+    return plan_command(reinterpret_cast<Plan*>(plan), state, state_dev, flags, seed, offset, z, action_out, nullptr, (cudaStream_t)stream);
 }
 
 int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint64_t seed, uint64_t offset, const void* z,
@@ -368,9 +385,7 @@ int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint
     Plan* pl = reinterpret_cast<Plan*>(plan);
     if (pl == nullptr || state == nullptr || host_mailbox == nullptr || action_host_out == nullptr || action_out_dev == nullptr)
         return MPPI_ERR_BAD_ARG;
-    if (pl->is_double) plan_update<double>(pl, state, nullptr, flags, seed, offset, z, action_out_dev, host_mailbox);
-    else plan_update<float>(pl, state, nullptr, flags, seed, offset, z, action_out_dev, host_mailbox);
-    int rc = plan_launch(pl, (cudaStream_t)stream);
+    int rc = plan_command(pl, state, nullptr, flags, seed, offset, z, action_out_dev, host_mailbox, (cudaStream_t)stream);
     if (rc) return rc;
     // every action value arrives as self-validating 8-byte word(s): payload32 | (epoch & 0xffffffff) << 32
     volatile unsigned long long* box = reinterpret_cast<volatile unsigned long long*>(host_mailbox);
@@ -405,7 +420,7 @@ int mppi_resident_start(void* plan, void* host_box, void* board_dev, void* actio
     if (pl == nullptr || host_box == nullptr || board_dev == nullptr || action_out_dev == nullptr || idle_us == 0)
         return MPPI_ERR_BAD_ARG;
     if (pl->res_kernel == nullptr)
-        return UNSUPPORTED("resident mode needs a plan on the split-cost rollout (one tile per SM, registered analytic model, in-kernel exchange if sharded)");
+        return UNSUPPORTED("resident mode needs a plan on the split-cost rollout (one tile per SM, one environment, single GPU)");
     if (pl->p.z_out != nullptr) return UNSUPPORTED("resident mode does not record the noise it draws (z_out)");
     if (pl->res.launched) {                 // re-arming: the old grid leaves first (it polls the box that is about to be cleared)
         int rc = res_halt(pl->res);
@@ -443,8 +458,8 @@ int mppi_resident_stop(void* plan) {
 // ---- user models compiled at run time ----------------------------------------------------------------------------------
 // The Python side compiles `mppi_fused.cuh + mppi_resident.cuh + the user's model header` with NVRTC (in process, no
 // toolkit) into a cubin and hands it over with the lowered names of the kernels; they are loaded as a cudaLibrary_t and
-// wrapped in a ModelKernels table exactly like a registry unit's.  `names`: 6 entries, nullptr = not built:
-//   [0] fused (this variant)  [1] split-cost  [2] batched (MPPI variant only)  [3] resident  [4] states  [5] unused
+// wrapped in a ModelKernels table exactly like a registry unit's.  `names`: 5 entries, nullptr = not built:
+//   [0] fused (this variant)  [1] split-cost  [2] batched (MPPI variant only)  [3] resident  [4] states
 namespace {
 void user_load(const ModelKernels* mk, void* dst, const double* blob, const double* ext, int n_ext) {
     for (int i = 0; i < mk->np; ++i) {

@@ -1,4 +1,4 @@
-// mppi_fused_host.cuh — kernel selection, launch geometry, plans and launches of the fused command, for ANY model: the
+// mppi_fused_host.cuh — kernel selection, launch geometry and plans of the fused command, for ANY model: the
 // model enters through a ModelKernels descriptor (kernel handles + parameter packing), so this is compiled once, in
 // mppi_b200.cu, and serves the registry models and NVRTC-compiled user models alike.
 #pragma once
@@ -31,7 +31,7 @@ inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedPara
 }
 
 // ---- kernel + launch geometry of one fused command -------------------------------------------------------------------
-// What is decided here, once per plan (or per mppi_fused_command call):
+// What is decided here, once per plan:
 //   kernel     fused_command_kernel<Model, real, V, batched, split>  (or the wgmma kernel, select_tensor_core_route)
 //   geometry   tile size / helper threads / grid (plan_geometry), planned for K_geom samples on sharded controllers so
 //              that every rank launches the same grid
@@ -44,8 +44,15 @@ inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedPara
 struct FusedChoice {
     const void* kernel;
     Geometry g;
-    int split, wide, tc;
+    int split, tc;
 };
+
+// the rank records of a command are exchanged with peers inside the kernel (else they stay in this GPU's own mailbox)
+inline bool sharded_in_kernel(const MppiFusedParams* p) {
+    bool any_peer = false;
+    for (int g = 0; g < MPPI_MAX_RANKS; ++g) any_peer = any_peer || p->peer_slots[g] != nullptr;
+    return p->world > 1 && any_peer && !(p->flags & MPPI_FLAG_EXPORT_PARTIAL);
+}
 
 template <typename real>
 int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedParams& p_tc, FusedChoice& c) {
@@ -57,24 +64,22 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     if (kernel == nullptr) return UNSUPPORTED("this model was built without the kernel of this controller variant");
     const bool tc_route = select_tensor_core_route(mk, p, p_tc, kernel);
     if (tc_route) p = &p_tc;
-    const int R = rows_of(p), es = (int)sizeof(real);
+    const int R = rows_of(p);
     const int world = p->world <= 0 ? 1 : p->world;
-    bool any_peer = false;
-    for (int g = 0; g < MPPI_MAX_RANKS; ++g) any_peer = any_peer || p->peer_slots[g] != nullptr;
-    const bool sharded = world > 1 && any_peer && !(p->flags & MPPI_FLAG_EXPORT_PARTIAL);
+    const bool sharded = sharded_in_kernel(p);
     MppiFusedParams pg = *p;
     if (p->K_geom > p->K) pg.K = p->K_geom;
     Geometry g;
     int rc;
     if (tc_route) {
-        rc = plan_geometry(kernel, &pg, es, 0, false, g, layout_fn<real>);
+        rc = plan_geometry<real>(kernel, &pg, 0, false, g);
         if (rc) return rc;
-        c = FusedChoice{kernel, g, 0, 0, 1};
+        c = FusedChoice{kernel, g, 0, 1};
         return MPPI_OK;
     }
     const int xst1 = sharded ? world * (R + 2) : 0;          // staging of the rank-record exchange
     const int tile2 = V != V_MPPI;                          // SMPPI: effective-noise tile, KMPPI: interpolated-trajectory tile
-    rc = plan_geometry(kernel, &pg, es, layout_extra(tile2, 0, 1, xst1), true, g, layout_fn<real>);
+    rc = plan_geometry<real>(kernel, &pg, layout_extra(tile2, 0, 1, xst1), true, g);
     if (rc) return rc;
     int split = 0;
     if (mk->split[V] != nullptr) {      // (the MLP has none: its step is the network, the cost is nothing)
@@ -85,7 +90,7 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
             p2.threads_per_sample = g.tps;
             p2.grid_blocks = g.nb;
             Geometry g2;
-            if (plan_geometry(k2, &p2, es, layout_extra(tile2, mk->nx, 1, xst1), true, g2, layout_fn<real>) == MPPI_OK &&
+            if (plan_geometry<real>(k2, &p2, layout_extra(tile2, mk->nx, 1, xst1), true, g2) == MPPI_OK &&
                 g2.BS == g.BS && g2.tps == g.tps) {
                 kernel = k2;
                 g = g2;
@@ -141,7 +146,7 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
         break;
     }
     if (g.cluster == 0) return UNSUPPORTED("shared-memory tile does not fit");
-    c = FusedChoice{kernel, g, split, 0, 0};
+    c = FusedChoice{kernel, g, split, 0};
     return MPPI_OK;
 }
 
@@ -150,60 +155,33 @@ template <typename real> void finish_kargs(const MppiFusedParams* p, const Fused
     a.xchg_npub = c.g.npub > 0 ? c.g.npub : 1;
 }
 
-template <typename real>
-int run_fused(const ModelKernels* mk, const MppiFusedParams* p, cudaStream_t stream, MppiLaunchInfo* info) {
-    const bool batched = p->n_env > 1;
-    if (batched && info == nullptr && !(p->flags & MPPI_FLAG_STATE_DEVICE)) return MPPI_ERR_BAD_ARG;   // states are (n_env, nx) on the device
+// MppiLaunchInfo of the plan these parameters would make (no launch)
+template <typename real> int query_fused(const ModelKernels* mk, const MppiFusedParams* p, MppiLaunchInfo* info) {
     MppiFusedParams p_tc;
     FusedChoice c;
     int rc = choose_fused<real>(mk, p, p_tc, c);
     if (rc) return rc;
-    const Geometry& g = c.g;
-    const uint64_t need_ws = ws_bytes(g.nb, rows_of(p), (int)sizeof(real));
+    DevInfo di;
+    if ((rc = get_dev_info(di)) != MPPI_OK) return rc;
     KArgs<real> a;
     finish_kargs<real>(p, c, a);
-    if (info != nullptr) {
-        DevInfo di;
-        get_dev_info(di);
-        info->block_threads = g.BD;
-        info->threads_per_sample = g.tps;
-        info->grid_blocks = g.nb;
-        info->smem_bytes = g.smem;
-        info->regs_per_thread = g.regs;
-        info->max_blocks_per_sm = g.occ;
-        info->sm_count = di.sm_count;
-        // report the worst case so one allocation serves any later geometry for these dimensions
-        info->workspace_bytes = ws_bytes(di.sm_count * 16, rows_of(p), (int)sizeof(real));
-        info->tma_staging = a.tma_ok;
-        info->split_cost = c.split;
-        info->wide_regs = c.wide;
-        info->cluster_size = g.cluster;
-        info->xchg_records = g.npub;
-        return MPPI_OK;
-    }
-    if (p->U == nullptr || p->cost_total == nullptr || p->action_out == nullptr || p->nominal_used == nullptr ||
-        p->stats == nullptr || p->workspace == nullptr)
-        return MPPI_ERR_BAD_ARG;
-    if (p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
-    if (batched && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env ||
-                    p->env_u_stride < p->T * p->nu))
-        return MPPI_ERR_WORKSPACE;
-    if (a.world > 1 && rows_of(p) > MPPI_XCHG_MAX_R) return UNSUPPORTED("T*nu exceeds the peer mailbox record size");
-    if (a.export_partial && p->partial_out == nullptr) return MPPI_ERR_BAD_ARG;
-    alignas(16) unsigned char mp[MPPI_MODEL_BLOCK_BYTES];
-    if (mk->param_bytes > (int)sizeof(mp)) return UNSUPPORTED("model parameter block too large");
-    mk->load(mk, mp, p->model_params, p->model_params_ext, p->n_model_params_ext);
-    if ((rc = refuse_capture(stream, g)) != MPPI_OK) return rc;
-    if (a.world == 1 || a.export_partial) {       // plan-less single-GPU launches draw their record tags from one process-wide counter
-        static unsigned long long s_epoch = 0;
-        a.epoch = __atomic_add_fetch(&s_epoch, 1ull, __ATOMIC_RELAXED);
-    }
-    void* argv2[2] = {(void*)&a, (void*)mp};
-    cudaError_t e = launch_raw(c.kernel, g.nb, g.BD, g.smem, stream, argv2, a.pdl != 0, a.n_env, g.cluster);
-    if (e != cudaSuccess) return cuda_fail(e, "fused launch");
+    const Geometry& g = c.g;
+    info->block_threads = g.BD;
+    info->threads_per_sample = g.tps;
+    info->grid_blocks = g.nb;
+    info->smem_bytes = g.smem;
+    info->regs_per_thread = g.regs;
+    info->max_blocks_per_sm = g.occ;
+    info->sm_count = di.sm_count;
+    info->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p), (int)sizeof(real));
+    info->tma_staging = a.tma_ok;
+    info->split_cost = c.split;
+    info->cluster_size = g.cluster;
+    info->xchg_records = g.npub;
     return MPPI_OK;
 }
 
+// Every check of the buffers and strides a command uses happens here, once per plan.
 template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedParams* p, Plan* pl) {
     const bool batched = p->n_env > 1;
     const int V = p->variant;
@@ -214,15 +192,19 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
     pl->g = c.g;
     if (p->U == nullptr || p->cost_total == nullptr || p->nominal_used == nullptr || p->stats == nullptr || p->workspace == nullptr)
         return MPPI_ERR_BAD_ARG;
-    if (p->workspace_bytes < ws_bytes(pl->g.nb, rows_of(p), (int)sizeof(real))) return MPPI_ERR_WORKSPACE;
+    const uint64_t need_ws = ws_bytes(pl->g.nb, rows_of(p), (int)sizeof(real));
+    if (p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
+    if (batched && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env ||
+                    p->env_u_stride < p->T * p->nu))
+        return MPPI_ERR_WORKSPACE;
     if (mk->param_bytes > (int)sizeof(pl->mparams)) return UNSUPPORTED("model parameter block too large");
     KArgs<real>* a = reinterpret_cast<KArgs<real>*>(pl->kargs);
     finish_kargs<real>(p, c, *a);
     if (a->world > 1 && rows_of(p) > MPPI_XCHG_MAX_R) return UNSUPPORTED("T*nu exceeds the peer mailbox record size");
+    if (a->export_partial && p->partial_out == nullptr) return MPPI_ERR_BAD_ARG;
     mk->load(mk, pl->mparams, p->model_params, p->model_params_ext, p->n_model_params_ext);
     pl->kernel = c.kernel;
     pl->res_kernel = nullptr;
-    pl->res_xchg = 0;
     // resident mode runs the split-cost rollout with one tile per CTA: exactly the single-GPU plans that took it, with
     // the launch route's grid and cluster size (mppi_resident.cuh)
     if (c.split && !batched && !a->export_partial && a->world == 1 && a->n_tiles <= pl->g.nb && pl->g.nb <= a->n_tiles + pl->g.cluster - 1) {

@@ -44,8 +44,7 @@ struct ResidentDevice {
 struct Plan {
     MppiFusedParams p;
     const void* kernel;
-    const void* res_kernel;            // resident_command_kernel<Model, real, V, sharded>, or nullptr when this plan cannot run resident
-    int res_xchg;                      // always 0 (resident mode serves single-GPU controllers)
+    const void* res_kernel;            // resident_command_kernel<Model, real, V>, or nullptr when this plan cannot run resident
     Resident res;
     ResidentDevice resdev;
     Geometry g;
@@ -166,6 +165,17 @@ inline uint64_t ws_partials_bytes(int nb, int R, int es) {
     return ((per_cta > per_cluster ? per_cta : per_cluster) + 255) / 256 * 256;
 }
 inline uint64_t ws_bytes(int nb, int R, int es) { return ws_partials_bytes(nb, R, es) + 2ull * MPPI_LL_LOCAL_WORDS * 8; }
+
+#define MPPI_MAX_CTAS_PER_SM 16                            // plan_geometry's grid cap
+// The largest grid any kernel of these dimensions can be planned with, on any route: tiles hold at least 32 samples, the
+// planner caps grids at MPPI_MAX_CTAS_PER_SM CTAs per SM, and the fused command pads its grid to a multiple of its
+// cluster size (8 at most).  A workspace of ws_bytes of this grid (MppiLaunchInfo.workspace_bytes) serves every geometry.
+inline int max_planned_grid(const MppiFusedParams* p, int sm_count) {
+    const long long K = p->K_geom > p->K ? p->K_geom : p->K;
+    const long long tiles = (K + 31) / 32, cap = (long long)sm_count * MPPI_MAX_CTAS_PER_SM;
+    const long long nb = tiles < cap ? tiles : cap;
+    return (int)((nb + 7) / 8 * 8);
+}
 
 inline unsigned long long xchg_timeout_ns() {
     // how long a shard waits for its peers' records before giving up (rank skew: a GC pause, a JIT build, a lazy module
@@ -318,9 +328,8 @@ struct GeomKey {
 
 // Launch geometry for (kernel, dimensions).  The occupancy / attribute queries cost microseconds, so
 // the last few results are cached per thread: a steady-state command() pays only the lookup.
-template <typename KernelT>
-int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_rows2, bool single_partial_grid, Geometry& g,
-                  SmemLayout (*layout)(int, int, int, int, int, int, int, int, int)) {
+template <typename real, typename KernelT>
+int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool single_partial_grid, Geometry& g) {
     static thread_local GeomKey keys[8];
     static thread_local Geometry vals[8];
     static thread_local int n_cached = 0, next_slot = 0;
@@ -358,7 +367,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_row
         const long long per_sm = ((long long)p->K + di.sm_count - 1) / di.sm_count;
         const long long want_threads = per_sm < 768 ? per_sm : 768;
         for (int bs = 64; bs <= 512; bs += (bs < 128 ? 64 : 32)) {     // 64-sample tiles let K < 128 x SMs reach every SM
-            SmemLayout Lc = layout(p->variant, p->T, p->nu, p->S, R, bs, bs, single_partial_grid ? 1 : di.sm_count * 4, need_rows2);
+            SmemLayout Lc = make_layout<real>(p->variant, p->T, p->nu, p->S, R, bs, bs, single_partial_grid ? 1 : di.sm_count * 4, need_rows2);
             if (Lc.total > dyn0) continue;
             int occ_c = 0;
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, kernel, bs, Lc.total));
@@ -395,7 +404,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_row
     while (tps > 1 && BS * tps > 512) tps >>= 1;
     if (tps != 1 && tps != 2 && tps != 4 && tps != 8) return MPPI_ERR_BAD_ARG;
     const int BD = BS * tps;
-    const int cap = di.sm_count * 16;
+    const int cap = di.sm_count * MPPI_MAX_CTAS_PER_SM;     // workspaces are sized for it: max_planned_grid
     cudaFuncAttributes fa;
     CK(cudaFuncGetAttributes(&fa, kernel));
     const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;   // static + dynamic <= opt-in maximum
@@ -408,7 +417,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_row
     int occ = 0;
     SmemLayout L;
     for (int it = 0; it < 4; ++it) {
-        L = layout(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
+        L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
         if (L.total > dyn_limit) return UNSUPPORTED("shared-memory tile does not fit");
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, BD, L.total));
         if (occ < 1) return UNSUPPORTED("kernel does not fit on an SM with this block size");
@@ -419,7 +428,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_row
         if (nb2 == nb) break;
         nb = nb2;
     }
-    L = layout(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
+    L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
     g.BS = BS;
     g.tps = tps;
     g.BD = BD;
@@ -429,18 +438,12 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int es, int need_row
     g.regs = fa.numRegs;
     g.cluster = 1;
     g.npub = 0;
-    (void)es;
     keys[next_slot] = key;
     vals[next_slot] = g;
     next_slot = (next_slot + 1) % 8;
     if (n_cached < 8) ++n_cached;
     return MPPI_OK;
 }
-
-template <typename real> SmemLayout layout_fn(int v, int T, int nu, int S, int R, int BD, int BS, int nb, int r2) {
-    return make_layout<real>(v, T, nu, S, R, BD, BS, nb, r2);
-}
-
 
 }  // namespace
 

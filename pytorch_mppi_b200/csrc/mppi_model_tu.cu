@@ -5,9 +5,8 @@
 // which the generic host code in mppi_b200.cu (mppi_fused_host.cuh) works on.
 //
 // Compiled several times by pytorch_mppi_b200/build.py:
-//     nvcc ... -DMPPI_TU_MODEL=<1 pendulum | 2 linear point | 3 pendulum MLP | 100 user> -DMPPI_TU_F64=<0|1> -c
-// (user model built with nvcc: additionally -DMPPI_USER_MODEL_HEADER="<generated header>"; the default route for user
-// models is NVRTC at run time, mppi_user_model_register — same kernels, same table).
+//     nvcc ... -DMPPI_TU_MODEL=<1 pendulum | 2 linear point | 3 pendulum MLP> -DMPPI_TU_F64=<0|1> -c
+// (user models are compiled at run time with NVRTC and registered with mppi_user_model_register — same kernels, same table).
 #include "mppi_host.cuh"
 #include "mppi_mlp_tc.cuh"
 
@@ -35,12 +34,6 @@ typedef mppi::LinearPointModel TuModel;
 #elif MPPI_TU_MODEL == 3
 typedef mppi::PendulumMLPModel TuModel;
 #define MPPI_TU_NAME pendulum_mlp
-#elif MPPI_TU_MODEL == 100
-#ifndef MPPI_USER_MODEL_HEADER
-#error "the user-model unit needs -DMPPI_USER_MODEL_HEADER"
-#endif
-typedef mppi::UserModel TuModel;
-#define MPPI_TU_NAME user
 #else
 #error "unknown MPPI_TU_MODEL"
 #endif

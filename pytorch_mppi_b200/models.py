@@ -251,7 +251,6 @@ class CudaModel(AnalyticModel):
         self.params = [float(v) for v in params]
         self._step_code, self._cost_code, self._terminal_code = step_code, cost_code, terminal_code
         self._dyn, self._cost, self._term = dynamics, running_cost, terminal_cost
-        self._lib_path = None
         self._rtc_handles = {}
 
     @property
@@ -320,14 +319,6 @@ struct UserModel {{
             _cabi.check(rc, "mppi_user_model_register")
             self._rtc_handles[key] = handle
         return self._rtc_handles[key]
-
-    def library_path(self):
-        """The nvcc route (MPPI_B200_USER_MODEL_BUILD=nvcc): path of a (cached) variant library with this model linked in;
-        builds it on first use.  Needs the CUDA toolkit."""
-        if self._lib_path is None:
-            from . import build
-            self._lib_path = build.build_user_model(self.header_text())
-        return self._lib_path
 
     def dynamics(self, state, action):
         if self._dyn is None:

@@ -173,11 +173,6 @@ class MPPI:
             m = resolve_fused_model(dynamics, running_cost, terminal_state_cost)
             if m is not None and m.nx == self.nx and m.nu == self.nu:
                 self._model = m
-                # user model: its kernels are compiled at run time with NVRTC and registered with the stock library
-                # (_pack); MPPI_B200_USER_MODEL_BUILD=nvcc builds a variant library with the toolkit instead
-                self._user_model_nvcc = hasattr(m, "library_path") and os.environ.get("MPPI_B200_USER_MODEL_BUILD", "rtc") == "nvcc"
-                if self._user_model_nvcc:
-                    self._lib = _cabi.load(m.library_path())
         if rng not in ("philox", "torch"):
             raise ValueError("rng must be 'philox' (one subsequence per sample) or 'torch' (the stream torch.randn draws on CUDA)")
         self._rng_mode = rng
@@ -361,7 +356,8 @@ class MPPI:
         p.variant = self._VARIANT
         p.model = self._model.model_id if self._model is not None else 0
         p.user_model = None
-        if self._model is not None and hasattr(self._model, "rtc_handle") and not getattr(self, "_user_model_nvcc", False):
+        # user model: its kernels are compiled at run time with NVRTC and registered with the library
+        if self._model is not None and hasattr(self._model, "rtc_handle"):
             with torch.cuda.device(self.d):
                 p.user_model = self._model.rtc_handle(self._lib, self.dtype, self._VARIANT)
         p.dtype = _DT[self.dtype]
@@ -453,15 +449,14 @@ class MPPI:
                 self._xchg_status_word = C.c_longlong.from_address(self._xchg_status.data_ptr())
             p.xchg_status_host = self._xchg_status.data_ptr()
         self._variant_pack(p)
-        # workspace sized for the worst-case geometry of these dimensions
-        if self._model is not None:
-            info = _cabi.MppiLaunchInfo()
-            p.flags = self._base_flags
-            _cabi.check(self._lib.mppi_fused_query(C.byref(p), C.byref(info)), "mppi_fused_query")
-            self.launch_info = info
-            need = int(info.workspace_bytes)
-        else:
-            need = 32 + self._max_grid() * (4 + self._noise_rows()) * 8 + 256 + 2 * 12288 * 8
+        # the library sizes the workspace for any geometry of these dimensions, per environment
+        info = _cabi.MppiLaunchInfo()
+        p.flags = self._base_flags
+        _cabi.check(self._lib.mppi_fused_query(C.byref(p), C.byref(info)), "mppi_fused_query")
+        self.launch_info = info
+        if p.n_env > 1:
+            p.env_ws_stride = info.workspace_bytes
+        need = int(info.workspace_bytes) * max(p.n_env, 1)
         if self._workspace is None or self._workspace.numel() < need:
             self._workspace = torch.zeros(need, device=self.d, dtype=torch.uint8)
         p.workspace = self._workspace.data_ptr()
@@ -475,10 +470,6 @@ class MPPI:
         self._dirty = False
         if self._model is not None:
             self._make_plan(p)
-
-    def _max_grid(self):
-        """Largest grid the planner launches on this device: 16 CTAs per SM (mppi_host.cuh, plan_geometry)."""
-        return torch.cuda.get_device_properties(self.d).multi_processor_count * 16
 
     def _make_plan(self, p):
         """Freeze the launch state in the C library (`mppi_plan_create`): per command only the state,
@@ -1517,24 +1508,8 @@ class MPPI_Batched(MPPI):
         self._Ubuf[:, : self.T * self.nu].copy_(value)
 
     def _variant_pack(self, p):
-        es = _ES[self.dtype]
-        rows = self.T * self.nu
-        nb_max = min((self.K + 31) // 32 + 1, self._max_grid())
-        stride = (max(16 + 2 * ((nb_max * es + 15) // 16 * 16) + ((nb_max * rows * es + 15) // 16 * 16),
-                      16 + nb_max * (rows + 2) * 8) + 255) // 256 * 256 + 2 * 12288 * 8   # ws_bytes: partials / records + local mailbox
-        self._env_ws_stride = (stride + 255) // 256 * 256
-        need = self._env_ws_stride * self.N
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = torch.zeros(need, device=self.d, dtype=torch.uint8)
         p.n_env = self.N
         p.env_u_stride = self._u_stride
-        p.env_ws_stride = self._env_ws_stride
-
-    def _pack(self):
-        super()._pack()
-        # super() sized the workspace for one problem; restore the per-environment slices
-        p = self._p
-        assert p.workspace == self._workspace.data_ptr() and p.workspace_bytes >= self._env_ws_stride * self.N
 
     def reset(self):
         """mppi.py:819-820"""

@@ -59,6 +59,9 @@ def test_bad_arguments_return_status_not_crash(lib):
     assert lib.mppi_resident_sync(None) == -1
     assert lib.mppi_resident_stop(None) == -1
     assert lib.mppi_resident_launches(None) == 0
+    # a run-time user model without its handle
+    u = _cabi.MppiFusedParams(struct_size=C.sizeof(p), model=_cabi.MODEL_USER, K=1, T=1, nx=1, nu=1, u_per_command=1, lambda_=1.0)
+    assert lib.mppi_plan_create(C.byref(u), C.byref(C.c_void_p())) == -1
 
 
 def test_missing_library_fails_loudly(monkeypatch, tmp_path):

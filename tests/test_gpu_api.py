@@ -452,6 +452,54 @@ def test_command_host_after_replan_returns_the_new_action():
     assert torch.equal(a.command_host(x), b.command(x).cpu())
 
 
+def test_fused_command_equals_plan_command():
+    """mppi_fused_command is a one-shot plan: on a C2-shaped fp32 controller (K=16384, T=30) it returns the same action,
+    U and cost_total, bit for bit, as mppi_plan_command on an identically seeded twin."""
+    import ctypes as C
+    from pytorch_mppi_b200 import _cabi
+    pend = eng.Pendulum()
+
+    def make():
+        torch.manual_seed(0)
+        U0 = torch.randn(30, 1) * 2
+        return eng.MPPI(pend.dynamics, pend.running_cost, 2, torch.tensor(4.0), num_samples=16384, horizon=30, U_init=U0,
+                        u_min=torch.tensor(-2.0), u_max=torch.tensor(2.0), device="cuda", rng_seed=5)
+    planned, oneshot = make(), make()
+    assert oneshot.dtype == torch.float32
+    oneshot._pack()
+    p = oneshot._p
+    stream = torch._C._cuda_getCurrentRawStream(oneshot.d.index)
+    for x in ([3.0, 0.4], [2.5, -1.0], [0.1, 0.2]):
+        want = planned.command(x)
+        p.flags = oneshot._base_flags | _cabi.FLAG_SHIFT
+        p.seed, p.offset = oneshot._next_rng()
+        p.z, p.state_dev, p.host_mailbox = None, None, None
+        for i, v in enumerate(x):
+            p.state[i] = v
+        action = torch.empty((1, 1), device="cuda", dtype=oneshot.dtype)
+        p.action_out = action.data_ptr()
+        _cabi.check(oneshot._lib.mppi_fused_command(C.byref(p), stream), "mppi_fused_command")
+        torch.cuda.synchronize()
+        assert torch.equal(action[0], want), x
+        assert torch.equal(oneshot.U, planned.U) and torch.equal(oneshot._cost_buf, planned._cost_buf), x
+
+
+def test_plan_rejects_a_batched_workspace_stride_too_small():
+    """A plan checks the per-environment workspace stride before any launch: 256 bytes is less than the local record
+    mailbox alone."""
+    import ctypes as C
+    m = eng.LinearPoint.unit_test_env()
+    c = eng.MPPI_Batched(m.dynamics, m.running_cost, 2, torch.eye(2, dtype=DT), num_envs=4, num_samples=100, horizon=10,
+                         device=DEV)
+    c._pack()
+    p = c._p
+    assert p.env_ws_stride == c.launch_info.workspace_bytes and p.workspace_bytes >= 4 * p.env_ws_stride
+    p.env_ws_stride = 256
+    plan = C.c_void_p()
+    assert c._lib.mppi_plan_create(C.byref(p), C.byref(plan)) == -3          # MPPI_ERR_WORKSPACE
+    assert plan.value is None
+
+
 def test_kmppi_change_horizon_rebuilds_interpolation():
     """ADVICE r1: KMPPI.change_horizon must rebuild W / Wshift / Tk / Hs for the new horizon (growing T used to read
     the old (T_old x S) matrix out of bounds)."""

@@ -192,28 +192,18 @@ def test_kernel_matrices_identities():
     assert len(idx) >= 2
 
 
-def test_cuda_model_builds_a_variant_library():
-    """A user-written model is JIT-built (nvcc, no GPU needed) into a variant library that exports the
-    whole C ABI; the controller-side resolution treats its bound methods like any registered model."""
-    from pytorch_mppi_b200 import _cabi
+def test_cuda_model_compiles_with_nvrtc_in_process():
+    """User models: NVRTC compiles the fused / split-cost / batched / resident / states kernels of the model from the
+    engine's own kernel headers — no nvcc, no GPU — and returns a cubin plus the lowered names the C library resolves
+    (`mppi_user_model_register`); the result is cached on disk.  The controller-side resolution treats the model's bound
+    methods like any registered model's."""
     from tests.user_models import pendulum_user_model
     ref = eng.Pendulum()
     m = pendulum_user_model()
     assert "struct UserModel" in m.header_text() and "NX = 2, NU = 1" in m.header_text()
     assert resolve_fused_model(m.dynamics, m.running_cost, None) is m
-    lib = _cabi.load(m.library_path())
-    assert lib.mppi_b200_abi_version() == _cabi.ABI_VERSION
-    assert m.library_path() == m.library_path()                 # cached
     s = torch.randn(8, 2)
     assert torch.equal(m.dynamics(s, torch.zeros(8, 1)), ref.dynamics(s, torch.zeros(8, 1)))
-
-
-def test_cuda_model_compiles_with_nvrtc_in_process():
-    """The default route for user models: NVRTC compiles the fused / split-cost / batched / resident / states kernels of
-    the model from the engine's own kernel headers — no nvcc, no GPU — and returns a cubin plus the lowered names the C
-    library resolves (`mppi_user_model_register`); the result is cached on disk."""
-    from tests.user_models import pendulum_user_model
-    m = pendulum_user_model()
     cubin, names = m.compile_rtc(torch.float32, 0)
     assert cubin[:4] == b"\x7fELF" and len(cubin) > 100000
     assert len(names) == 5 and all(n is not None for n in names)

@@ -1,5 +1,5 @@
-"""User-written CUDA models used by the tests (built into variant libraries by `__graft_entry__.build()` so the
-GPU machine does not spend GPU time running nvcc)."""
+"""User-written CUDA models used by the tests (compiled with NVRTC by `__graft_entry__.build()`, cubins cached in-tree,
+so the GPU tests load them without compiling)."""
 import torch
 
 import pytorch_mppi_b200 as eng
