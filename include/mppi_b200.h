@@ -229,6 +229,16 @@ int mppi_plan_command(void* plan, const double* state, const void* state_dev, ui
  * `host_mailbox`: u_per_command*nu*8 bytes (x2 for f64) of zero-initialised pinned host memory. */
 int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint64_t seed, uint64_t offset,
                            const void* z, void* action_out_dev, void* host_mailbox, void* action_host_out, void* stream);
+/* New model parameters for the plan's following commands, without re-planning: `model_params`
+ * (MPPI_MODEL_PARAM_DOUBLES doubles, the layout of MppiFusedParams.model_params) and `ext` / `n_ext` (host doubles, as
+ * model_params_ext) are packed with the model's loader exactly as at plan creation, and the plan's copy of the
+ * parameters is updated.  Nothing else changes: no kernel selection, geometry, allocation or CUDA call.  Commands
+ * already launched keep the values they were launched with (kernel arguments are copied at launch).  This is how a
+ * time-varying problem (a moving target, a reference trajectory) follows its data from one control step to the next.
+ * PENDULUM_MLP: [2] and [3] selected the plan's kernel and must stay as they are, and the weights are required.
+ * MPPI_ERR_BAD_ARG: null plan or model_params, n_ext < 0, ext NULL with n_ext > 0.  MPPI_ERR_UNSUPPORTED while a
+ * resident grid is armed (its parameters are frozen; mppi_resident_stop first). */
+int mppi_plan_set_model_params(void* plan, const double* model_params, const double* ext, int32_t n_ext);
 
 /* ---- Resident mode: command() without a kernel launch ---------------------------------------------
  * For a host control loop (mppi.py:240-252 called once per control step).  One cooperative launch leaves the

@@ -142,6 +142,7 @@ SYMBOLS = [
                                     C.c_void_p, C.c_void_p]),
     ("mppi_plan_command_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
+    ("mppi_plan_set_model_params", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),
     ("mppi_resident_start", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     ("mppi_resident_command", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]),
     ("mppi_resident_sync", C.c_int, [C.c_void_p]),

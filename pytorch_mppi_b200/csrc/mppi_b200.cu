@@ -380,6 +380,22 @@ int mppi_plan_command(void* plan, const double* state, const void* state_dev, ui
     return plan_command(reinterpret_cast<Plan*>(plan), state, state_dev, flags, seed, offset, z, action_out, nullptr, (cudaStream_t)stream);
 }
 
+// the plan's parameter block is a kernel argument: it is copied at every launch, so a launch already enqueued keeps the
+// values it was launched with; a resident grid holds the block of its own launch for as long as it stays
+int mppi_plan_set_model_params(void* plan, const double* model_params, const double* ext, int32_t n_ext) {
+    Plan* pl = reinterpret_cast<Plan*>(plan);
+    if (pl == nullptr || model_params == nullptr || n_ext < 0 || (n_ext > 0 && ext == nullptr)) return MPPI_ERR_BAD_ARG;
+    if (pl->mk->is_mlp && (n_ext < PendulumMLPModel::N_EXT || model_params[2] != pl->p.model_params[2] ||
+                           model_params[3] != pl->p.model_params[3]))
+        return MPPI_ERR_BAD_ARG;      // the weights are required, and [2] / [3] selected the plan's kernel
+    if (pl->res.armed) return UNSUPPORTED("the resident grid holds the parameters it was launched with: stop it first");
+    memcpy(pl->p.model_params, model_params, sizeof(pl->p.model_params));
+    pl->p.model_params_ext = ext;
+    pl->p.n_model_params_ext = n_ext;
+    pl->mk->load(pl->mk, pl->mparams, pl->p.model_params, ext, n_ext);
+    return MPPI_OK;
+}
+
 int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint64_t seed, uint64_t offset, const void* z,
                            void* action_out_dev, void* host_mailbox, void* action_host_out, void* stream) {
     Plan* pl = reinterpret_cast<Plan*>(plan);
@@ -415,6 +431,12 @@ int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint
     return MPPI_OK;
 }
 
+// The record epochs a resident session used (res_epoch_off + seq, stop records included) become the plan's own: the
+// workspace still holds records with those tags, so neither the next session nor a launch-route command may reuse them.
+inline void fold_resident_epochs(Plan* pl) {
+    if (pl->res_epoch_off + pl->res.seq > pl->epoch) pl->epoch = pl->res_epoch_off + pl->res.seq;
+}
+
 int mppi_resident_start(void* plan, void* host_box, void* board_dev, void* action_out_dev, uint64_t idle_us, void* stream) {
     Plan* pl = reinterpret_cast<Plan*>(plan);
     if (pl == nullptr || host_box == nullptr || board_dev == nullptr || action_out_dev == nullptr || idle_us == 0)
@@ -426,6 +448,7 @@ int mppi_resident_start(void* plan, void* host_box, void* board_dev, void* actio
         int rc = res_halt(pl->res);
         if (rc) return rc;
     }
+    fold_resident_epochs(pl);
     ResidentDevice& d = pl->resdev;
     d.host_box = reinterpret_cast<unsigned long long*>(host_box);
     d.board = reinterpret_cast<unsigned long long*>(board_dev);
@@ -452,7 +475,10 @@ int mppi_resident_sync(void* plan) {
 
 int mppi_resident_stop(void* plan) {
     Plan* pl = reinterpret_cast<Plan*>(plan);
-    return pl == nullptr ? (int)MPPI_ERR_BAD_ARG : res_stop(pl->res);
+    if (pl == nullptr) return MPPI_ERR_BAD_ARG;
+    const int rc = res_stop(pl->res);
+    fold_resident_epochs(pl);
+    return rc;
 }
 
 // ---- user models compiled at run time ----------------------------------------------------------------------------------

@@ -1438,7 +1438,7 @@ MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
             noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
 #pragma unroll
             for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
-            Model::template step<real>(mp, x, u);                                     // mppi.py:314
+            model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
 #pragma unroll
             for (int i = 0; i < NX; ++i) xcol[(t * NX + i) * BS] = x[i];
             pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
@@ -1465,7 +1465,7 @@ MPPI_UNROLL_N(2)
             for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);
 #pragma unroll
             for (int i = 0; i < NX; ++i) xt[i] = xcol[(t * NX + i) * BS];
-            xcol[(t * NX) * BS] = Model::template cost<real>(mp, xt, u);              // mppi.py:318
+            xcol[(t * NX) * BS] = model_cost<Model, real>(mp, xt, u, t);              // mppi.py:318
         }
     }
     __syncthreads();
@@ -1594,11 +1594,11 @@ MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
 #pragma unroll
                 for (int i = 0; i < NX; ++i) xs[i] = x[i];
 #if MPPI_ROLLOUT_PIPELINED
-                Model::template step<real>(mp, x, u);                                     // mppi.py:314
-                if (t > 0) roll = O::add(roll, Model::template cost<real>(mp, xs, uprev));   // mppi.py:318-319 (step t-1)
+                model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
+                if (t > 0) roll = O::add(roll, model_cost<Model, real>(mp, xs, uprev, t - 1));   // mppi.py:318-319 (step t-1)
 #else
-                Model::template step<real>(mp, x, u);                                     // mppi.py:314
-                roll = O::add(roll, Model::template cost<real>(mp, x, u));                // mppi.py:318-319
+                model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
+                roll = O::add(roll, model_cost<Model, real>(mp, x, u, t));                // mppi.py:318-319
 #endif
                 pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
                 if (VARIANT == V_SMPPI) {
@@ -1616,7 +1616,7 @@ MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
                 for (int n = 0; n < NU; ++n) uprev[n] = u[n];
             }
 #if MPPI_ROLLOUT_PIPELINED
-            roll = O::add(roll, Model::template cost<real>(mp, x, uprev));                // step T-1
+            roll = O::add(roll, model_cost<Model, real>(mp, x, uprev, T - 1));            // step T-1
 #endif
             if (Model::template has_terminal<real>(mp)) roll = O::add(roll, Model::template terminal<real>(mp, x));
             c_tot = O::add(roll, pert);                                                   // mppi.py:416
@@ -1755,7 +1755,7 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
     for (int t = 0; t < a.T; ++t) {
         real u[NU];
         for (int n = 0; n < NU; ++n) u[n] = O::mul(a.nm.u_scale, pa[t * NU + n]);                 // mppi.py:313 / :445
-        Model::template step<real>(mp, x, u);
+        model_step<Model, real>(mp, x, u, t);
         for (int i = 0; i < NX; ++i) states[((size_t)k * a.T + t) * NX + i] = x[i];
     }
 }

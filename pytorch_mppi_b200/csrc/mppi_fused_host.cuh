@@ -203,6 +203,7 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
     if (a->world > 1 && rows_of(p) > MPPI_XCHG_MAX_R) return UNSUPPORTED("T*nu exceeds the peer mailbox record size");
     if (a->export_partial && p->partial_out == nullptr) return MPPI_ERR_BAD_ARG;
     mk->load(mk, pl->mparams, p->model_params, p->model_params_ext, p->n_model_params_ext);
+    pl->mk = mk;
     pl->kernel = c.kernel;
     pl->res_kernel = nullptr;
     // resident mode runs the split-cost rollout with one tile per CTA: exactly the single-GPU plans that took it, with

@@ -41,8 +41,11 @@ struct ResidentDevice {
     unsigned long long idle_ns = 0;
 };
 
+struct ModelKernels;
+
 struct Plan {
     MppiFusedParams p;
+    const ModelKernels* mk;            // the model's kernels and parameter packer (mppi_plan_set_model_params re-packs)
     const void* kernel;
     const void* res_kernel;            // resident_command_kernel<Model, real, V>, or nullptr when this plan cannot run resident
     Resident res;

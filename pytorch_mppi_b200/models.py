@@ -9,8 +9,9 @@ controller launches the fused sm_90a kernel.  The same bound methods are ordinar
 (any device, any dtype), so they also serve as the simulator you step your real system with and as
 the callables of the per-step path.
 
-Anything else (a torch MLP, a lambda, a step-dependent function) takes the per-step path:
-the T-loop stays in Python with sampling / accumulation / softmin in CUDA kernels.
+Anything else (a torch MLP, a lambda, a plain step-dependent function) takes the per-step path:
+the T-loop stays in Python with sampling / accumulation / softmin in CUDA kernels.  A `CudaModel` declared
+``step_dependent=True`` is the compiled form of a step-dependent pair (``step_dependent_dynamics=True``).
 """
 from __future__ import annotations
 
@@ -27,6 +28,8 @@ class AnalyticModel:
     model_id: int = 0
     nx: int = 0
     nu: int = 0
+    step_dependent: bool = False     # dynamics / running_cost take the horizon index t (CudaModel(step_dependent=True))
+    _param_version: int = 0          # bumped by CudaModel.set_params; controllers compare it at command time
 
     def param_blob(self) -> list:
         """The `model_params` doubles of MppiFusedParams for this instance."""
@@ -233,6 +236,8 @@ class CudaModel(AnalyticModel):
         x[NX]      state (read/write in `step_code`, read-only in `cost_code` / `terminal_code`)
         u[NU]      action, already multiplied by u_scale
         p[...]     your `params` (cast to the controller dtype)
+        t          step_dependent=True only: the horizon index 0..T-1 of this step (`const int`), in `step_code` and
+                   `cost_code` (not in `terminal_code`, as the reference's terminal cost)
         real       the controller dtype; O::add/sub/mul/div are individually rounded ops (use them if you want
                    bit-level agreement with an eager fp32 torch implementation), sinf/exp/... via O::sin_, O::exp_
 
@@ -240,15 +245,28 @@ class CudaModel(AnalyticModel):
     are the torch callables of the same model (used by the stepped route and as your simulator;
     `get_rollouts` runs the compiled `step_code`); pass ``model.dynamics`` / ``model.running_cost`` to the
     controller as usual.
+
+    Step-dependent models (time-varying problems: a moving target, a reference trajectory to track, a forcing
+    schedule): with ``step_dependent=True`` the torch callables are called as ``dynamics(state, action, t)`` and
+    ``running_cost(state, action, t)``, and the controller must be built with ``step_dependent_dynamics=True``, exactly as
+    the reference calls such plugins (mppi.py:147-157).  MPPI / SMPPI / KMPPI / MPPI_Batched with
+    ``rollout_samples=1`` and no SpecificActionSampler then run the fused kernel.
+
+    `set_params(values)` replaces the parameter values (same count as at construction).  Every controller using the
+    model takes them at its next command, without re-planning; a resident grid leaves and the next `command_host()`
+    brings it back.  Intermediates of earlier commands (`states`, `noise`, ...) keep the values they were computed
+    with, `get_rollouts` uses the current ones.  Your torch callables see the change only if they read `model.params`.
+    A sharded (multi-GPU) controller needs the same values on every rank before the same command.
     """
     model_id = _cabi.MODEL_USER
 
     def __init__(self, nx, nu, step_code, cost_code, params=(), terminal_code=None, dynamics=None, running_cost=None,
-                 terminal_cost=None):
+                 terminal_cost=None, step_dependent=False):
         if not (1 <= nx <= _cabi.MPPI_MAX_NX and 1 <= nu <= _cabi.MPPI_MAX_NU):
             raise ValueError(f"nx <= {_cabi.MPPI_MAX_NX} and nu <= {_cabi.MPPI_MAX_NU} required")
         self.nx, self.nu = int(nx), int(nu)
         self.params = [float(v) for v in params]
+        self.step_dependent = bool(step_dependent)
         self._step_code, self._cost_code, self._terminal_code = step_code, cost_code, terminal_code
         self._dyn, self._cost, self._term = dynamics, running_cost, terminal_cost
         self._rtc_handles = {}
@@ -263,28 +281,41 @@ class CudaModel(AnalyticModel):
     def param_blob_ext(self):
         return self.params[_cabi.MPPI_MODEL_PARAM_DOUBLES:]
 
+    def set_params(self, values):
+        """New values of `params` for the following commands of every controller using this model (see the class
+        docstring).  The number of parameters is compiled into the kernels: it must not change."""
+        values = [float(v) for v in values]
+        if len(values) != len(self.params):
+            raise ValueError(f"this model was compiled with {len(self.params)} parameters, got {len(values)}")
+        self.params = values
+        self._param_version += 1
+
     def header_text(self):
         n = max(len(self.params), 1)
         term = self._terminal_code if self._terminal_code is not None else "return (real)0;"
+        sd = self.step_dependent
+        decl = "\n    static const bool STEP_DEPENDENT = true;" if sd else ""
+        targ = ", const int t" if sd else ""
+        tvoid = " (void)t;" if sd else ""
         return f"""// generated by pytorch_mppi_b200.models.CudaModel
 namespace mppi {{
 struct UserModel {{
-    static const int NX = {self.nx}, NU = {self.nu}, NP = {n};
+    static const int NX = {self.nx}, NU = {self.nu}, NP = {n};{decl}
     template <typename real> struct P {{ real v[NP]; }};
     template <typename real> static void load(P<real>& P_, const double* b, const double* ext = nullptr, int n_ext = 0) {{
         for (int i = 0; i < NP; ++i)
             P_.v[i] = (real)(i < {_cabi.MPPI_MODEL_PARAM_DOUBLES} ? b[i] : (ext != nullptr && i - {_cabi.MPPI_MODEL_PARAM_DOUBLES} < n_ext ? ext[i - {_cabi.MPPI_MODEL_PARAM_DOUBLES}] : 0.0));
     }}
-    template <typename real> static MPPI_HD void step(const P<real>& P_, real* x, const real* u) {{
+    template <typename real> static MPPI_HD void step(const P<real>& P_, real* x, const real* u{targ}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p;
+        (void)p;{tvoid}
         {self._step_code}
     }}
-    template <typename real> static MPPI_HD real cost(const P<real>& P_, const real* x, const real* u) {{
+    template <typename real> static MPPI_HD real cost(const P<real>& P_, const real* x, const real* u{targ}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p; (void)u;
+        (void)p; (void)u;{tvoid}
         {self._cost_code}
     }}
     template <typename real> static MPPI_HD bool has_terminal(const P<real>&) {{ return {"true" if self.has_terminal else "false"}; }}
@@ -320,15 +351,20 @@ struct UserModel {{
             self._rtc_handles[key] = handle
         return self._rtc_handles[key]
 
-    def dynamics(self, state, action):
-        if self._dyn is None:
-            raise NotImplementedError("this CudaModel was created without a torch `dynamics` callable")
-        return self._dyn(state, action)
+    def _with_t(self, fn, what, args, t):
+        if fn is None:
+            raise NotImplementedError(f"this CudaModel was created without a torch `{what}` callable")
+        if not self.step_dependent:
+            return fn(*args)
+        if t is None:
+            raise TypeError(f"this CudaModel is step-dependent: call {what}(state, action, t)")
+        return fn(*args, t)
 
-    def running_cost(self, state, action):
-        if self._cost is None:
-            raise NotImplementedError("this CudaModel was created without a torch `running_cost` callable")
-        return self._cost(state, action)
+    def dynamics(self, state, action, t=None):
+        return self._with_t(self._dyn, "dynamics", (state, action), t)
+
+    def running_cost(self, state, action, t=None):
+        return self._with_t(self._cost, "running_cost", (state, action), t)
 
     def terminal_cost(self, states, actions):
         if self._term is None:

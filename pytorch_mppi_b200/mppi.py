@@ -6,7 +6,8 @@ Two execution routes, chosen at construction:
 * fused  — dynamics / running_cost (/ terminal cost) are bound methods of one registered analytic
            model (pytorch_mppi_b200.models): ONE kernel launch per ``command()`` does sampling,
            rollout, softmin and the nominal update (csrc/mppi_fused.cuh `fused_command_kernel`).
-* stepped — arbitrary Python callables (a torch MLP, step-dependent functions, M>1 rollouts, a
+           A step-dependent CudaModel takes this route with ``step_dependent_dynamics=True``.
+* stepped — arbitrary Python callables (a torch MLP, plain step-dependent functions, M>1 rollouts, a
            SpecificActionSampler): the T-loop stays in Python exactly like mppi.py:312-322, with the
            sampling (`mppi_sample_perturb`), cost accumulation (`mppi_cost_accumulate`) and softmin
            update (`mppi_softmin_update`) as kernels.
@@ -70,11 +71,30 @@ def _pad16(n_elems, es):
     return (n_elems * es + 15) // 16 * 16 // es
 
 
+def fused_route_model(dynamics, running_cost, terminal_state_cost, nx, nu, rollout_samples, specific_action_sampler,
+                      step_dependent_dynamics) -> typing.Optional[AnalyticModel]:
+    """The registered model a controller with these arguments runs on the fused route, or None (stepped route).
+    A model's compiled bodies take the horizon index t exactly when the reference would pass it (mppi.py:147-157): a
+    step-dependent CudaModel needs step_dependent_dynamics=True, and a model without t takes the fused route only
+    without it."""
+    owner = AnalyticModel.owner_of(dynamics) or AnalyticModel.owner_of(running_cost)
+    if owner is not None and owner.step_dependent and not step_dependent_dynamics:
+        raise ValueError("this model is step-dependent (its dynamics / running_cost take the horizon index t): "
+                         "pass step_dependent_dynamics=True")
+    if rollout_samples != 1 or specific_action_sampler is not None:
+        return None
+    m = resolve_fused_model(dynamics, running_cost, terminal_state_cost)
+    if m is None or m.nx != nx or m.nu != nu or m.step_dependent != bool(step_dependent_dynamics):
+        return None
+    return m
+
+
 class MPPI:
     """Model Predictive Path Integral control (Williams et al. 2017, alg. 2), CUDA engine.
     Constructor and methods mirror the reference (mppi.py:45-61, 208-290, 425-448)."""
 
     _VARIANT = _cabi.VARIANT_MPPI
+    _model_version = 0                  # the model's `_param_version` the plan was last given
 
     def __init__(self, dynamics, running_cost, nx, noise_sigma, num_samples=100, horizon=15, device="cuda",
                  terminal_state_cost=None,
@@ -167,12 +187,9 @@ class MPPI:
         self.rollout_var_cost = rollout_var_cost
         self.rollout_var_discount = rollout_var_discount
 
-        # route selection
-        self._model: typing.Optional[AnalyticModel] = None
-        if (self.M == 1 and specific_action_sampler is None and not step_dependent_dynamics):
-            m = resolve_fused_model(dynamics, running_cost, terminal_state_cost)
-            if m is not None and m.nx == self.nx and m.nu == self.nu:
-                self._model = m
+        self._model: typing.Optional[AnalyticModel] = fused_route_model(
+            dynamics, running_cost, terminal_state_cost, self.nx, self.nu, self.M, specific_action_sampler,
+            step_dependent_dynamics)
         if rng not in ("philox", "torch"):
             raise ValueError("rng must be 'philox' (one subsequence per sample) or 'torch' (the stream torch.randn draws on CUDA)")
         self._rng_mode = rng
@@ -392,17 +409,8 @@ class MPPI:
                 p.sigma_inv[i * _cabi.MPPI_MAX_NU + j] = float(Si[i, j]) if inside else 0.0
         p.w_action_seq_cost = 0.0
         p.delta_t = 1.0
-        blob = self._model.param_blob() if self._model is not None else []
-        for i in range(_cabi.MPPI_MODEL_PARAM_DOUBLES):
-            p.model_params[i] = float(blob[i]) if i < len(blob) else 0.0
-        ext = self._model.param_blob_ext() if self._model is not None else []
-        if ext:
-            self._ext_arr = (C.c_double * len(ext))(*ext)      # host memory, read by the library at plan creation / launch
-            p.model_params_ext = C.cast(self._ext_arr, C.c_void_p)
-            p.n_model_params_ext = len(ext)
-        else:
-            p.model_params_ext = None
-            p.n_model_params_ext = 0
+        self._ext_arr = self._fill_model_params(p)
+        self._model_version = self._model._param_version if self._model is not None else 0
         self._base_flags = ((_cabi.FLAG_NULL_ACTION if self.sample_null_action else 0)
                             | (_cabi.FLAG_ABS_COST if self.noise_abs_cost else 0)
                             | (_cabi.FLAG_DIAG_SIGMA if self._diagonal_sigma else 0)
@@ -470,6 +478,30 @@ class MPPI:
         self._dirty = False
         if self._model is not None:
             self._make_plan(p)
+
+    def _fill_model_params(self, p):
+        """The model's current parameters into `p`; returns the host array `p.model_params_ext` points to (the caller
+        keeps it alive: the library reads it at plan creation / launch)."""
+        m = self._model
+        blob = m.param_blob() if m is not None else []
+        for i in range(_cabi.MPPI_MODEL_PARAM_DOUBLES):
+            p.model_params[i] = float(blob[i]) if i < len(blob) else 0.0
+        ext = m.param_blob_ext() if m is not None else []
+        arr = (C.c_double * len(ext))(*ext) if ext else None
+        p.model_params_ext = None if arr is None else C.cast(arr, C.c_void_p)
+        p.n_model_params_ext = len(ext)
+        return arr
+
+    def _take_model_params(self):
+        """`CudaModel.set_params` since this controller's last command: its plan takes the new values (no re-plan).
+        The struct is updated here, at command time, so that the intermediates of the previous command are still
+        materialised with the values they were computed with."""
+        self._leave_resident()          # a resident grid holds the parameters it was launched with
+        self._ext_arr = self._fill_model_params(self._p)
+        self._model_version = self._model._param_version
+        p = self._p
+        _cabi.check(self._lib.mppi_plan_set_model_params(self._plan, p.model_params, p.model_params_ext, p.n_model_params_ext),
+                    "mppi_plan_set_model_params")
 
     def _make_plan(self, p):
         """Freeze the launch state in the C library (`mppi_plan_create`): per command only the state,
@@ -600,6 +632,8 @@ class MPPI:
             self._pack()
         if self._model is None or self._plan is None:
             raise _cabi.MppiLibraryError("resident mode needs a registered model (the fused route)")
+        if getattr(self._model, "_param_version", 0) != self._model_version:
+            self._take_model_params()
         if self._z_out is not None:
             raise _cabi.MppiLibraryError("resident mode does not record noise; call record_noise(False) first")
         words = 64 + self.u_per_command * self.nu * (2 if self.dtype == torch.float64 else 1)
@@ -866,6 +900,8 @@ class MPPI:
         return None, seed, off
 
     def _command_fused(self, state, shift):
+        if getattr(self._model, "_param_version", 0) != self._model_version:
+            self._take_model_params()
         if self._world > 1:
             self._check_exchange_status()
         sflags, sdev = self._host_state(state)
@@ -957,6 +993,8 @@ class MPPI:
         sflags, sdev = self._host_state(state)
         if sdev is not None:
             return self.command(state, shift_nominal_trajectory, info).cpu()
+        if getattr(self._model, "_param_version", 0) != self._model_version:
+            self._take_model_params()       # a resident grid leaves; the branch below brings it back
         if self._resident or self._resident_wanted:
             if self._z_inject is None and getattr(self, "_offset_dev", None) is None:
                 if not self._resident:
@@ -1218,11 +1256,17 @@ class MPPI:
                 raise ValueError(f"state has {state.size(0)} rows, expected 1 or num_rollouts={num_rollouts}")
             if self._dirty:
                 self._pack()
+            p, ext = self._p, None          # ext: keeps the host array p.model_params_ext points to alive
+            if getattr(self._model, "_param_version", 0) != self._model_version:
+                # the model's current parameters, as a reference closure would use; the controller's own copy stays with
+                # the last command (its intermediates are materialised from it) until the next command takes them
+                p = _cabi.MppiFusedParams.from_buffer_copy(self._p)
+                ext = self._fill_model_params(p)
             x0 = state.contiguous()
             seq = U.to(self.d, self.dtype).contiguous()
             out = torch.empty((num_rollouts, T, self.nx), dtype=self.dtype, device=self.d)
             stream = torch.cuda.current_stream(self.d).cuda_stream
-            _cabi.check(self._lib.mppi_rollout_states(C.byref(self._p), x0.data_ptr(), seq.data_ptr(), 0, num_rollouts, T,
+            _cabi.check(self._lib.mppi_rollout_states(C.byref(p), x0.data_ptr(), seq.data_ptr(), 0, num_rollouts, T,
                                                       out.data_ptr(), stream), "mppi_rollout_states")
             return out
         states = torch.zeros((num_rollouts, T + 1, self.nx), dtype=U.dtype, device=U.device)
@@ -1541,6 +1585,8 @@ class MPPI_Batched(MPPI):
         zptr, seed, off = self._noise_source()
         self._cmd_count += 1
         if self._model is not None:
+            if getattr(self._model, "_param_version", 0) != self._model_version:
+                self._take_model_params()
             self._last = (flags, seed, off, zptr, states.data_ptr())
             _cabi.check(self._lib.mppi_plan_command(self._plan, None, states.data_ptr(), flags, seed, off, zptr,
                                                     action.data_ptr(), stream), "mppi_plan_command")

@@ -1,0 +1,123 @@
+"""Golden cases of step-dependent dynamics and cost (step_dependent_dynamics=True, reference mppi.py:147-157): the model
+of tests/step_models.py under MPPI, KMPPI and MPPI_Batched.  Fixtures tests/golden/stepint_*.npz, produced by the live
+reference (tests/golden/make_golden_step.py); kept apart from cases.CASES so that the tests parametrised over those do
+not see them.
+
+The oracle (oracle/mppi_oracle.py) calls its plugins as `dynamics(state, u)` / `running_cost(state, u)`.  Its rollouts,
+like the reference's (mppi.py:312-319, 849-853), call dynamics and then running_cost exactly once per horizon step,
+t = 0, ..., T-1, in order, once per command; `HorizonClock` relies on that order to hand the step-dependent callables
+their t, and refuses any other call sequence."""
+import functools
+
+import numpy as np
+import torch
+
+from oracle import mppi_oracle as orc
+from tests import step_models as sm
+from tests.golden.cases import _DT, draw_z
+from tests.golden.replay import Stream
+
+STEPINT = {"kind": "step_integrator", "params": list(sm.SD_PARAMS), "terminal": True}
+STEP_CASES = {
+    "stepint_mppi_f64": dict(variant="mppi", model=STEPINT, dtype="f64", K=512, T=20, lambda_=1.0, noise_sigma=1.0,
+                             u_max=3.0, x0=[0.0, 0.0], steps=3, seed=801),
+    "stepint_kmppi_f32": dict(variant="kmppi", model=STEPINT, dtype="f32", K=2048, T=24, lambda_=1.0, noise_sigma=2.0,
+                              u_max=3.0, x0=[0.2, -0.1], kernel=dict(S=6, sigma=2.0), steps=3, seed=802),
+}
+STEP_BATCHED_CASES = {
+    "stepint_batched_f64": dict(model=dict(STEPINT, terminal=False), dtype="f64", N=3, K=384, T=15, lambda_=0.8,
+                                noise_sigma=1.0, u_max=3.0, x0=[[0.0, 0.0], [1.0, -0.5], [-1.0, 0.5]], steps=3, seed=803),
+}
+
+
+class HorizonClock:
+    """dynamics(state, u) / running_cost(state, u) for the oracle, calling f(state, u, t) / c(state, u, t) with the
+    horizon index of the step the rollout is at (see the module docstring)."""
+
+    def __init__(self, f, c, T):
+        self.f, self.c, self.T = f, c, T
+        self.t, self.stepped = 0, False
+
+    def dynamics(self, state, u):
+        assert not self.stepped, "dynamics called twice without the running cost of the step in between"
+        self.stepped = True
+        return self.f(state, u, self.t)
+
+    def running_cost(self, state, u):
+        assert self.stepped, "running cost called before the dynamics of its step"
+        self.stepped = False
+        cost = self.c(state, u, self.t)
+        self.t = (self.t + 1) % self.T
+        return cost
+
+
+def callables(case):
+    """The step-dependent (dynamics, running_cost, terminal cost or None) of a case: f(state, u, t) etc."""
+    m = case["model"]
+    p = m["params"]
+    term = functools.partial(sm.sd_term, p=p) if m["terminal"] else None
+    return functools.partial(sm.sd_dyn, p=p), functools.partial(sm.sd_cost, p=p), term
+
+
+def step_problem(case, dynamics=None, running_cost=None):
+    """The oracle's Problem of a case; `dynamics` / `running_cost` (f(state, u, t)) replace the case's own."""
+    dt = _DT[case["dtype"]]
+    f, c, term = callables(case)
+    clock = HorizonClock(dynamics or f, running_cost or c, case["T"])
+    return orc.Problem(clock.dynamics, clock.running_cost, 2, torch.tensor(case["noise_sigma"], dtype=dt), K=case["K"],
+                       T=case["T"], lambda_=case["lambda_"], u_max=torch.tensor(case["u_max"], dtype=dt),
+                       terminal_state_cost=term)
+
+
+def plant_step(case, x, u):
+    """The closed loop's simulated system: the model at t = 0, the horizon index of the step being applied."""
+    return sm.sd_dyn(x, u, 0, case["model"]["params"])
+
+
+class StepOracleRunner:
+    """Steps the oracle through an MPPI / KMPPI step case on the fixture's injected draws."""
+
+    def __init__(self, case, dynamics=None, running_cost=None):
+        self.case = case
+        self.prob = step_problem(case, dynamics, running_cost)
+        self.stream = Stream(case, self.prob)
+        self.U = self.stream.U0.clone()
+        if case["variant"] == "kmppi":
+            S, sig = case["kernel"]["S"], case["kernel"]["sigma"]
+            self.theta = torch.zeros(S, self.prob.nu, dtype=self.prob.dtype)
+            self.W, self.Wshift = orc.kernel_matrices(case["T"], S, lambda a, b: orc.rbf_kernel(a, b, sig), self.prob.dtype)
+
+    def step(self, x, z):
+        if self.case["variant"] == "kmppi":
+            r = orc.kmppi_command(self.prob, self.U, self.theta, x, z, self.W, self.Wshift)
+            self.theta = r["theta"]
+        else:
+            r = orc.mppi_command(self.prob, self.U, x, z)
+        self.U = r["U"]
+        return r
+
+    def advance(self, x, action):
+        return plant_step(self.case, x.view(1, -1), (self.prob.u_scale * action).view(1, -1)).view(-1)
+
+
+class StepBatchedOracleRunner:
+    """MPPI_Batched step case: shared (K,T,nu) draws, (N,T,nu) nominal, (N,nx) states."""
+
+    def __init__(self, case):
+        self.case = case
+        self.prob = step_problem(case)
+        self.gen = np.random.Generator(np.random.Philox(key=case["seed"]))
+        self.U0 = torch.from_numpy(self.gen.standard_normal((case["N"], case["T"], 1), dtype=np.float32)).to(self.prob.dtype)
+        self.U = self.U0.clone()
+
+    def next_z(self):
+        c = self.case
+        return draw_z(self.gen, (c["K"], c["T"], 1), self.prob.dtype, c.get("z_dtype"))
+
+    def step(self, x, z):
+        r = orc.mppi_batched_command(self.prob, self.U, x, z)
+        self.U = r["U"]
+        return r
+
+    def advance(self, x, action):
+        return plant_step(self.case, x, self.prob.u_scale * action)
