@@ -29,6 +29,7 @@ extern "C" {
 #define MPPI_MAX_NX 8            /* state dimension supported by the fused registry              */
 #define MPPI_MODEL_PARAM_DOUBLES 48
 #define MPPI_MAX_RANKS 8         /* GPUs of one NVSwitch box                                     */
+#define MPPI_MAX_COPIES 8        /* rollout_samples of a user model compiled with copies (registers) */
 
 typedef enum MppiStatus {
     MPPI_OK = 0,
@@ -179,6 +180,13 @@ typedef struct MppiFusedParams {
                                     exchange timed out (the caller checks it before the next command)      */
     void* user_model;            /* model == MPPI_MODEL_USER: handle from mppi_user_model_register (a model compiled at
                                     run time); required                                                     */
+    /* ---- rollout_samples M > 1 (mppi.py:334-373): each sample's actions are rolled out through M copies of the
+     * dynamics; cost = mean over copies + rollout_var_cost * sum_t var_discount[t] * var_m(c_{m,t}).  Fused route: user
+     * models compiled with M copies only (mppi_user_model_set_copies); registered models: MPPI_ERR_UNSUPPORTED. */
+    int32_t rollout_samples;     /* 0 or 1: one rollout per sample                                                  */
+    double rollout_var_cost;
+    const void* var_discount;    /* (T) device buffer of the controller dtype: rollout_var_discount ** arange(T)
+                                    (mppi.py:174-175); required when rollout_samples > 1                        */
 } MppiFusedParams;
 
 typedef struct MppiLaunchInfo {
@@ -288,6 +296,11 @@ int mppi_apply_partials(const MppiFusedParams* p, const void* partials, void* st
 int mppi_user_model_register(const void* cubin, uint64_t cubin_bytes, int32_t nx, int32_t nu, int32_t n_params, int32_t dtype,
                              int32_t variant, const char* const* names, void** handle_out);
 int mppi_user_model_release(void* handle);
+/* The copy count a user model's kernels were compiled with (CudaModel(copies=M): its bodies take the copy index m; 1 by
+ * default).  Plans of the model require rollout_samples == copies.  A model with copies > 1 has no split-cost, batched
+ * or resident kernels (names[1..3] NULL), so its commands run the single-loop rollout and resident mode is refused.
+ * MPPI_ERR_BAD_ARG: bad handle, copies outside 1..MPPI_MAX_COPIES, or copies > 1 with any of those kernels. */
+int mppi_user_model_set_copies(void* handle, int32_t copies);
 /* Highest command epoch this plan has used (the tag of its reduction records, shared by the launch and resident routes);
  * pass it as MppiFusedParams.epoch when re-creating the plan so that stale records can never match. */
 uint64_t mppi_plan_epoch(void* plan);
@@ -302,12 +315,13 @@ uint64_t mppi_xchg_bytes(void);
  * states / actions (mppi.py:307-322) on every command.  The fused kernel keeps them in shared
  * memory only; these entry points regenerate them from (seed, offset | z) and nominal_used. */
 int mppi_materialize(const MppiFusedParams* p, void* perturbed_action /*(K,T,nu)*/, void* noise /*(K,T,nu)*/,
-                     void* noise_theta /*KMPPI (K,S,nu) or NULL*/, void* states /*(K,T,nx) or NULL*/, void* stream);
+                     void* noise_theta /*KMPPI (K,S,nu) or NULL*/,
+                     void* states /*(K,T,nx), (M,K,T,nx) with rollout_samples = M > 1, or NULL*/, void* stream);
 
 /* get_rollouts (mppi.py:425-448) for a registered model: `n_rollouts` start states (n_rollouts,nx) on the device, each
  * rolled T steps through u_scale * actions[t] — one (T,nu) sequence replayed by every rollout (actions_stride = 0) or a
  * sequence per rollout (actions_stride = elements between them, e.g. T*nu) — into states_out (n_rollouts,T,nx).
- * Only model, dtype, nx, nu, u_scale and the model parameters of `p` are read. */
+ * Only model, dtype, nx, nu, u_scale and the model parameters of `p` are read; a model with copies rolls out copy 0. */
 int mppi_rollout_states(const MppiFusedParams* p, const void* start_states, const void* actions, int64_t actions_stride,
                         int32_t n_rollouts, int32_t T, void* states_out, void* stream);
 

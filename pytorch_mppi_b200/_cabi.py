@@ -15,6 +15,7 @@ MPPI_MAX_NU = 4
 MPPI_MAX_NX = 8
 MPPI_MODEL_PARAM_DOUBLES = 48
 MPPI_MAX_RANKS = 8
+MPPI_MAX_COPIES = 8
 ABI_VERSION = 1
 
 # enums
@@ -106,6 +107,9 @@ class MppiFusedParams(C.Structure):
         ("debug_clocks", C.c_void_p),
         ("xchg_status_host", C.c_void_p),
         ("user_model", C.c_void_p),
+        ("rollout_samples", C.c_int32),
+        ("rollout_var_cost", C.c_double),
+        ("var_discount", C.c_void_p),
     ]
 
 
@@ -152,6 +156,7 @@ SYMBOLS = [
     ("mppi_user_model_register", C.c_int, [C.c_void_p, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                            C.POINTER(C.c_char_p), C.POINTER(C.c_void_p)]),
     ("mppi_user_model_release", C.c_int, [C.c_void_p]),
+    ("mppi_user_model_set_copies", C.c_int, [C.c_void_p, C.c_int32]),
     ("mppi_apply_partials", C.c_int, [_P, C.c_void_p, C.c_void_p]),
     ("mppi_xchg_create", C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
     ("mppi_xchg_open", C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),

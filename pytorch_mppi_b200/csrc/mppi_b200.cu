@@ -57,6 +57,18 @@ const ModelKernels* find_kernels(const MppiFusedParams* p, int* rc) {
     return get != nullptr ? get() : nullptr;
 }
 
+// rollout_samples M > 1 (mppi.py:334-373) on the fused route: only a user model compiled with M copies makes its copies
+// differ (a registered model's M rollouts would be identical).  No CUDA call.
+int check_rollout_samples(const MppiFusedParams* p, const ModelKernels* mk) {
+    if (p->rollout_samples < 0) return MPPI_ERR_BAD_ARG;
+    const int M = p->rollout_samples > 1 ? p->rollout_samples : 1;
+    if (M > 1 && p->model != MPPI_MODEL_USER)
+        return UNSUPPORTED("rollout_samples > 1 on the fused route needs a user model compiled with that many copies");
+    const int copies = mk->copies > 1 ? mk->copies : 1;
+    if (M != copies || (M > 1 && p->var_discount == nullptr)) return MPPI_ERR_BAD_ARG;
+    return MPPI_OK;
+}
+
 template <typename real>
 inline void plan_update(Plan* pl, const double* state, const void* state_dev, uint32_t flags, uint64_t seed, uint64_t offset,
                         const void* z, void* action_out, void* host_mailbox) {
@@ -332,6 +344,7 @@ int mppi_fused_query(const MppiFusedParams* p, MppiLaunchInfo* out) {
     if ((rc = validate(p, true)) != MPPI_OK) return rc;
     const ModelKernels* mk = find_kernels(p, &rc);
     if (mk == nullptr) return rc;
+    if ((rc = check_rollout_samples(p, mk)) != MPPI_OK) return rc;
     return mk->is_double ? query_fused<double>(mk, p, out) : query_fused<float>(mk, p, out);
 }
 
@@ -358,7 +371,8 @@ int mppi_plan_create(const MppiFusedParams* p, void** plan_out) {
     Plan* pl = new (std::nothrow) Plan();
     if (pl == nullptr) return MPPI_ERR_BAD_ARG;
     const ModelKernels* mk = find_kernels(p, &rc);
-    if (mk != nullptr) rc = mk->is_double ? build_plan<double>(mk, p, pl) : build_plan<float>(mk, p, pl);
+    if (mk != nullptr) rc = check_rollout_samples(p, mk);
+    if (mk != nullptr && rc == MPPI_OK) rc = mk->is_double ? build_plan<double>(mk, p, pl) : build_plan<float>(mk, p, pl);
     if (rc) {
         delete pl;
         return rc;
@@ -547,6 +561,17 @@ int mppi_user_model_release(void* handle) {
     return MPPI_OK;
 }
 
+int mppi_user_model_set_copies(void* handle, int32_t copies) {
+    UserModelHandle* h = reinterpret_cast<UserModelHandle*>(handle);
+    if (h == nullptr || h->magic != kUserMagic || copies < 1 || copies > MPPI_MAX_COPIES) return MPPI_ERR_BAD_ARG;
+    const ModelKernels& mk = h->mk;
+    bool others = mk.batched != nullptr;
+    for (int v = 0; v < 3; ++v) others = others || mk.split[v] != nullptr || mk.resident[v] != nullptr;
+    if (copies > 1 && others) return MPPI_ERR_BAD_ARG;     // those kernels roll out one copy per sample
+    h->mk.copies = copies;
+    return MPPI_OK;
+}
+
 uint64_t mppi_plan_epoch(void* plan) {
     Plan* pl = reinterpret_cast<Plan*>(plan);
     if (pl == nullptr) return 0;
@@ -635,6 +660,7 @@ int mppi_materialize(const MppiFusedParams* p, void* perturbed_action, void* noi
     if (rc || states == nullptr) return rc;
     const ModelKernels* mk = find_kernels(p, &rc);
     if (mk == nullptr) return rc;
+    if ((rc = check_rollout_samples(p, mk)) != MPPI_OK) return rc;
     return mk->is_double ? run_states<double>(mk, p, perturbed_action, states, s) : run_states<float>(mk, p, perturbed_action, states, s);
 }
 

@@ -101,8 +101,13 @@ template <typename real> struct KArgs {
     const real* override_rows;
     int n_override, override_start;
     const real* in_cost;
-    const real* in_eps;
-    real* out_omega;
+    // The fused kernel of a model with COPIES > 1 (rollout_samples, mppi.py:334-373) reads none of the generic-path
+    // extras: its two constants share their space, so that KArgs keeps its size and every other kernel its code.
+    union {
+        const real* in_eps;       // softmin_update_kernel
+        real var_cost;            // COPIES > 1: rollout_var_cost (mppi.py:372)
+    };
+    const real* var_disc;         // COPIES > 1: (T) rollout_var_discount^t (mppi.py:174-175, 364)
 };
 
 // ---- shared-memory carve, computed identically on host and device -------------------------------
@@ -1411,6 +1416,7 @@ __device__ void make_env_args(const KArgs<real>& in, KArgs<real>* out) {
 template <class Model, typename real, int VARIANT>
 __device__ __forceinline__ real split_cost_rollout(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
                                                    int k, unsigned long long kg, bool in_range, bool active) {
+    static_assert(ModelCopies<Model>::value == 1, "models with COPIES > 1 run the single-loop rollout (copies_rollout)");
     typedef Ops<real> O;
     constexpr int NX = Model::NX, NU = Model::NU;
     const NoiseModel<real>& nm = a.nm;
@@ -1480,6 +1486,120 @@ MPPI_UNROLL_N(2)
     return c_tot;
 }
 
+// one step's costs c[0..M-1] of the M copies (mppi.py:362-364): cs[m] += c[m], and var += var_m(c) * disc with the
+// two-pass unbiased variance of cost_accumulate_kernel (mean = sum_m c / M, then sum_m (c - mean)^2 / (M - 1))
+template <typename real, int M>
+__device__ __forceinline__ void copies_fold(real* cs, real& var, const real* c, real disc) {
+    typedef Ops<real> O;
+    real mean = c[0];
+#pragma unroll
+    for (int m = 1; m < M; ++m) mean = O::add(mean, c[m]);
+    mean = O::div(mean, (real)M);
+    real ss = (real)0;
+#pragma unroll
+    for (int m = 0; m < M; ++m) {
+        const real d = O::sub(c[m], mean);
+        ss = O::add(ss, O::mul(d, d));
+    }
+    var = O::add(var, O::mul(O::div(ss, (real)(M - 1)), disc));
+#pragma unroll
+    for (int m = 0; m < M; ++m) cs[m] = O::add(cs[m], c[m]);
+}
+
+// ---- stage C'', rollout of a model with COPIES = M > 1 (rollout_samples, mppi.py:334-373), on the sample's rollout
+// thread.  The M copies share the sample's action sequence, noise and action cost; their recurrences are M independent
+// chains, interleaved in registers.  Per copy the running costs are summed t = 0..T-1, the discounted variance over the
+// copies is accumulated per step, then cost = (mean_m(cost_m + terminal_m) + var * rollout_var_cost) + perturbation
+// (+ SMPPI smoothness), in the reference's order (mppi.py:369-372, 415-416).  Stores cost_total[k] and returns it.
+template <class Model, typename real, int VARIANT>
+__device__ __forceinline__ real copies_rollout(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
+                                               int k, unsigned long long kg) {
+    typedef Ops<real> O;
+    constexpr int NX = Model::NX, NU = Model::NU, M = ModelCopies<Model>::value;
+    const NoiseModel<real>& nm = a.nm;
+    const int T = a.T;
+    real x[M][NX];
+    if (a.state_dev != nullptr) {
+        const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
+#pragma unroll
+        for (int i = 0; i < NX; ++i) x[0][i] = sp[i];
+    } else {
+#pragma unroll
+        for (int i = 0; i < NX; ++i) x[0][i] = a.x0[i];
+    }
+    real cs[M];
+#pragma unroll
+    for (int m = 0; m < M; ++m) {
+        cs[m] = (real)0;
+#pragma unroll
+        for (int i = 0; i < NX; ++i) x[m][i] = x[0][i];
+    }
+    real var = (real)0, pert = (real)0, smooth = (real)0;
+    real vprev[NU], uprev[NU];
+#pragma unroll
+    for (int n = 0; n < NU; ++n) { vprev[n] = (real)0; uprev[n] = (real)0; }
+    for (int t = 0; t < T; ++t) {
+        real v[NU], u[NU], eps[NU], c[M];
+        action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
+        noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
+#pragma unroll
+        for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);                // mppi.py:355
+#if MPPI_ROLLOUT_PIPELINED
+        // step t-1's costs in iteration t, as the single loop of one copy: its variance takes disc[t-1]
+#pragma unroll
+        for (int m = 0; m < M; ++m) {
+            real xs[NX];
+#pragma unroll
+            for (int i = 0; i < NX; ++i) xs[i] = x[m][i];
+            model_step<Model, real>(mp, x[m], u, t, m);                                 // mppi.py:357
+            if (t > 0) c[m] = model_cost<Model, real>(mp, xs, uprev, t - 1, m);         // mppi.py:362 (step t-1)
+        }
+        if (t > 0) copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t - 1));         // mppi.py:363-364
+#else
+#pragma unroll
+        for (int m = 0; m < M; ++m) {
+            model_step<Model, real>(mp, x[m], u, t, m);                                 // mppi.py:357
+            c[m] = model_cost<Model, real>(mp, x[m], u, t, m);                          // mppi.py:362
+        }
+        copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t));                         // mppi.py:363-364
+#endif
+        pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
+        if (VARIANT == V_SMPPI) {
+            if (t > 0) {
+#pragma unroll
+                for (int n = 0; n < NU; ++n) {
+                    const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));          // mppi.py:559
+                    smooth = O::add(smooth, O::mul(d, d));
+                }
+            }
+#pragma unroll
+            for (int n = 0; n < NU; ++n) vprev[n] = v[n];
+        }
+#pragma unroll
+        for (int n = 0; n < NU; ++n) uprev[n] = u[n];
+    }
+#if MPPI_ROLLOUT_PIPELINED
+    {
+        real c[M];
+#pragma unroll
+        for (int m = 0; m < M; ++m) c[m] = model_cost<Model, real>(mp, x[m], uprev, T - 1, m);   // step T-1
+        copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + T - 1));
+    }
+#endif
+    if (Model::template has_terminal<real>(mp)) {
+#pragma unroll
+        for (int m = 0; m < M; ++m) cs[m] = O::add(cs[m], model_terminal<Model, real>(mp, x[m], m));   // mppi.py:369-370
+    }
+    real mean = cs[0];
+#pragma unroll
+    for (int m = 1; m < M; ++m) mean = O::add(mean, cs[m]);
+    mean = O::div(mean, (real)M);                                                         // mppi.py:371
+    real c_tot = O::add(O::add(mean, O::mul(var, a.var_cost)), pert);                     // mppi.py:372, 416
+    if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));           // mppi.py:562,569
+    a.cost_total[k] = c_tot;
+    return c_tot;
+}
+
 // =================================================================================================
 // The fused command kernel
 // =================================================================================================
@@ -1495,8 +1615,13 @@ MPPI_UNROLL_N(2)
 // whole register file.  The single-loop kernels of the analytic models get 2 = a 64-register cap (20 B of spill): the
 // two-CTA-per-SM geometry of large K needs it, and without the promise the out-of-line tail functions push ptxas to 128
 // registers and one CTA per SM (measured at K = 131072: 42 -> 53 us).  The MLP's step keeps 64 activations live: it gets
-// the whole register file (one CTA per SM) — under the cap it spilled 340 B per thread.
-template <class Model> struct FusedMinBlocks { static constexpr int value = MPPI_FUSED_MIN_BLOCKS; };
+// the whole register file (one CTA per SM) — under the cap it spilled 340 B per thread.  So do models with COPIES > 1:
+// at M = 8 (the test models of tests/ensemble_models.py) the M states, costs and cost sums of copies_rollout spilled
+// 42-62 B (fp32) and 458-578 B (fp64) of stores per thread under the cap; without it fp32 takes 122-124 registers and
+// does not spill, fp64 takes 128 and spills 4-62 B.
+template <class Model> struct FusedMinBlocks {
+    static constexpr int value = ModelCopies<Model>::value > 1 ? 1 : MPPI_FUSED_MIN_BLOCKS;
+};
 template <> struct FusedMinBlocks<PendulumMLPModel> { static constexpr int value = 1; };
 
 template <class Model, typename real, int VARIANT, bool BATCHED, bool SPLIT = false, int MINB = (SPLIT ? 1 : FusedMinBlocks<Model>::value)>
@@ -1564,6 +1689,9 @@ __global__ void __launch_bounds__(512, MINB) fused_command_kernel(const __grid_c
         if constexpr (SPLIT) {
             // C'. split rollout: recurrence (rollout thread) | running costs (all tps threads) | ordered sum
             c_tot = split_cost_rollout<Model, real, VARIANT>(a, mp, sm, k, kg, in_range, active);
+        } else if constexpr (ModelCopies<Model>::value > 1) {
+            // C''. M copies of the sample's rollout, interleaved in registers
+            if (active) c_tot = copies_rollout<Model, real, VARIANT>(a, mp, sm, k, kg);
         } else if (active) {
 
             // C. rollout (mppi.py:297-332) + action cost (mppi.py:409,415) [+ smoothness :559-562]
@@ -1737,6 +1865,7 @@ __global__ void __launch_bounds__(512) sample_kernel(const __grid_constant__ KAr
 // states along the rollout of given perturbed actions (mppi.py:307-322), for registered models.
 // pa_stride = elements between consecutive samples' action sequences: T*nu for a (K,T,nu) tensor, 0 when every
 // sample replays the SAME (T,nu) sequence (get_rollouts, mppi.py:425-448).
+// Models with COPIES > 1: blockIdx.y is the copy, states are (gridDim.y, K, T, nx) (mppi.py:345, 366).
 template <class Model, typename real>
 __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ states, const KArgs<real> a,
                               const typename Model::template P<real> mp, long long pa_stride) {
@@ -1744,6 +1873,11 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
     constexpr int NX = Model::NX, NU = Model::NU;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.K) return;
+    int m = 0;
+    if constexpr (ModelCopies<Model>::value > 1) {
+        m = blockIdx.y;
+        states += (size_t)m * a.K * a.T * NX;
+    }
     pa += (size_t)k * (size_t)pa_stride;
     real x[NX];
     if (a.state_dev != nullptr) {
@@ -1755,7 +1889,7 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
     for (int t = 0; t < a.T; ++t) {
         real u[NU];
         for (int n = 0; n < NU; ++n) u[n] = O::mul(a.nm.u_scale, pa[t * NU + n]);                 // mppi.py:313 / :445
-        model_step<Model, real>(mp, x, u, t);
+        model_step<Model, real>(mp, x, u, t, m);
         for (int i = 0; i < NX; ++i) states[((size_t)k * a.T + t) * NX + i] = x[i];
     }
 }

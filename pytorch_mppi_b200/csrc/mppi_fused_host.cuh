@@ -227,25 +227,27 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
 
 template <typename real>
 int launch_states(const ModelKernels* mk, const MppiFusedParams* p, KArgs<real>& a, int n, const void* actions, void* states,
-                  long long stride, cudaStream_t stream) {
+                  long long stride, cudaStream_t stream, int copies = 1) {
     alignas(16) unsigned char mp[MPPI_MODEL_BLOCK_BYTES];
     if (mk->param_bytes > (int)sizeof(mp)) return UNSUPPORTED("model parameter block too large");
     mk->load(mk, mp, p->model_params, p->model_params_ext, p->n_model_params_ext);
     const real* pa = (const real*)actions;
     real* st = (real*)states;
     void* argv[5] = {(void*)&pa, (void*)&st, (void*)&a, (void*)mp, (void*)&stride};
-    cudaError_t e = cudaLaunchKernel(mk->states, dim3((n + 127) / 128), dim3(128), argv, 0, stream);
+    cudaError_t e = cudaLaunchKernel(mk->states, dim3((n + 127) / 128, copies), dim3(128), argv, 0, stream);
     if (e != cudaSuccess) return cuda_fail(e, "states launch");
     return MPPI_OK;
 }
 
-// states along the rollouts of the last command's perturbed actions (mppi.py:307-322)
+// states along the rollouts of the last command's perturbed actions (mppi.py:307-322); every copy's with
+// rollout_samples = M > 1 (mppi.py:366): (M,K,T,nx)
 template <typename real>
 int run_states(const ModelKernels* mk, const MppiFusedParams* p, const void* pa, void* states, cudaStream_t stream) {
     if (p->nx != mk->nx || p->nu != mk->nu) return MPPI_ERR_BAD_ARG;
     KArgs<real> a;
     fill_kargs<real>(p, a, 128, 1);
-    return launch_states<real>(mk, p, a, p->K, pa, states, (long long)p->T * p->nu, stream);
+    return launch_states<real>(mk, p, a, p->K, pa, states, (long long)p->T * p->nu, stream,
+                               p->rollout_samples > 1 ? p->rollout_samples : 1);
 }
 
 // get_rollouts (mppi.py:425-448): n start states, each rolled through an action sequence

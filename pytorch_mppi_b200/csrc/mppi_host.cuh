@@ -77,6 +77,7 @@ struct ModelKernels {
     const void* states;              // states_kernel<Model, real>
     const void* tc[3][2][2];         // mlp_tc_command_kernel<V, SPLIT = 2 - mode, FAST>, [V][mode - 1][fast]; fp32 MLP only
     void* library;                   // run-time user models: the cudaLibrary_t that owns the kernels
+    int copies;                      // run-time user models: the COPIES their kernels were compiled with (0 or 1: none)
 };
 }  // namespace mppi_host
 
@@ -254,6 +255,10 @@ template <typename real> int fill_kargs(const MppiFusedParams* p, KArgs<real>& a
     for (int g = 0; g < MPPI_MAX_RANKS; ++g) {
         a.peers[g] = (unsigned long long*)p->peer_slots[g];
         any_peer = any_peer || p->peer_slots[g] != nullptr;
+    }
+    if (p->rollout_samples > 1) {
+        a.var_disc = (const real*)p->var_discount;
+        a.var_cost = (real)p->rollout_var_cost;
     }
     if (!any_peer || a.export_partial) a.world = a.export_partial ? a.world : 1;
     if (p->workspace != nullptr && (a.world == 1 || a.export_partial)) {

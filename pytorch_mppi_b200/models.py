@@ -29,6 +29,7 @@ class AnalyticModel:
     nx: int = 0
     nu: int = 0
     step_dependent: bool = False     # dynamics / running_cost take the horizon index t (CudaModel(step_dependent=True))
+    copies: int = 1                  # compiled rollout copies per sample (CudaModel(copies=M)): runs with rollout_samples=M
     _param_version: int = 0          # bumped by CudaModel.set_params; controllers compare it at command time
 
     def param_blob(self) -> list:
@@ -238,6 +239,8 @@ class CudaModel(AnalyticModel):
         p[...]     your `params` (cast to the controller dtype)
         t          step_dependent=True only: the horizon index 0..T-1 of this step (`const int`), in `step_code` and
                    `cost_code` (not in `terminal_code`, as the reference's terminal cost)
+        m          copies=M > 1 only: the copy index 0..M-1 (`const int`), in `step_code`, `cost_code` and
+                   `terminal_code`; `COPIES` is M
         real       the controller dtype; O::add/sub/mul/div are individually rounded ops (use them if you want
                    bit-level agreement with an eager fp32 torch implementation), sinf/exp/... via O::sin_, O::exp_
 
@@ -257,13 +260,29 @@ class CudaModel(AnalyticModel):
     brings it back.  Intermediates of earlier commands (`states`, `noise`, ...) keep the values they were computed
     with, `get_rollouts` uses the current ones.  Your torch callables see the change only if they read `model.params`.
     A sharded (multi-GPU) controller needs the same values on every rank before the same command.
+
+    Ensembles (robust control under model uncertainty: domain randomisation over masses and lengths, disturbance
+    scenarios): with ``copies=M`` (2 <= M <= MPPI_MAX_COPIES) every sample's action sequence is rolled out through M
+    copies of the model, and the bodies tell the copies apart by `m` (e.g. ``p[2 + m]`` a per-copy mass, or a scenario
+    table ``p[m * T + t]`` with ``step_dependent=True``; long tables go in `params`, past the first
+    MPPI_MODEL_PARAM_DOUBLES values).  The controller must be built with ``rollout_samples=M``: the cost of a sample is
+    the mean over its copies plus ``rollout_var_cost * sum_t rollout_var_discount**t * var_m(c_{m,t})``, as the
+    reference computes it (mppi.py:334-373).  MPPI / SMPPI / KMPPI (also sharded) without a SpecificActionSampler then
+    run the fused kernel, which keeps the M states in registers; resident mode and MPPI_Batched are not available.
+    The torch callables are called exactly as the reference calls an M-copy rollout: with M*K rows, copy-major, so row r
+    belongs to copy ``r // K``.  Your twins therefore have to know K (the controller's num_samples; on a sharded
+    controller, its shard's sample count).  `get_rollouts` runs copy 0, which is what such a twin computes for
+    ``num_rollouts <= K`` rows.
     """
     model_id = _cabi.MODEL_USER
 
     def __init__(self, nx, nu, step_code, cost_code, params=(), terminal_code=None, dynamics=None, running_cost=None,
-                 terminal_cost=None, step_dependent=False):
+                 terminal_cost=None, step_dependent=False, copies=1):
         if not (1 <= nx <= _cabi.MPPI_MAX_NX and 1 <= nu <= _cabi.MPPI_MAX_NU):
             raise ValueError(f"nx <= {_cabi.MPPI_MAX_NX} and nu <= {_cabi.MPPI_MAX_NU} required")
+        if isinstance(copies, bool) or not isinstance(copies, int) or not 1 <= copies <= _cabi.MPPI_MAX_COPIES:
+            raise ValueError(f"copies must be an integer 1..{_cabi.MPPI_MAX_COPIES}, got {copies!r}")
+        self.copies = copies
         self.nx, self.nu = int(nx), int(nu)
         self.params = [float(v) for v in params]
         self.step_dependent = bool(step_dependent)
@@ -297,6 +316,10 @@ class CudaModel(AnalyticModel):
         decl = "\n    static const bool STEP_DEPENDENT = true;" if sd else ""
         targ = ", const int t" if sd else ""
         tvoid = " (void)t;" if sd else ""
+        cp = self.copies > 1
+        decl += f"\n    static const int COPIES = {self.copies};" if cp else ""
+        marg = ", const int m" if cp else ""
+        mvoid = " (void)m;" if cp else ""
         return f"""// generated by pytorch_mppi_b200.models.CudaModel
 namespace mppi {{
 struct UserModel {{
@@ -306,23 +329,23 @@ struct UserModel {{
         for (int i = 0; i < NP; ++i)
             P_.v[i] = (real)(i < {_cabi.MPPI_MODEL_PARAM_DOUBLES} ? b[i] : (ext != nullptr && i - {_cabi.MPPI_MODEL_PARAM_DOUBLES} < n_ext ? ext[i - {_cabi.MPPI_MODEL_PARAM_DOUBLES}] : 0.0));
     }}
-    template <typename real> static MPPI_HD void step(const P<real>& P_, real* x, const real* u{targ}) {{
+    template <typename real> static MPPI_HD void step(const P<real>& P_, real* x, const real* u{targ}{marg}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p;{tvoid}
+        (void)p;{tvoid}{mvoid}
         {self._step_code}
     }}
-    template <typename real> static MPPI_HD real cost(const P<real>& P_, const real* x, const real* u{targ}) {{
+    template <typename real> static MPPI_HD real cost(const P<real>& P_, const real* x, const real* u{targ}{marg}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p; (void)u;{tvoid}
+        (void)p; (void)u;{tvoid}{mvoid}
         {self._cost_code}
     }}
     template <typename real> static MPPI_HD bool has_terminal(const P<real>&) {{ return {"true" if self.has_terminal else "false"}; }}
-    template <typename real> static MPPI_HD real terminal(const P<real>& P_, const real* x) {{
+    template <typename real> static MPPI_HD real terminal(const P<real>& P_, const real* x{marg}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p; (void)x;
+        (void)p; (void)x;{mvoid}
         {term}
     }}
 }};
@@ -333,7 +356,8 @@ struct UserModel {{
         """(cubin bytes, lowered kernel names) of this model's kernels for one dtype and controller variant
         (0 MPPI / 1 SMPPI / 2 KMPPI): NVRTC, cached on disk.  Needs no GPU."""
         from . import rtc
-        return rtc.compile_user_model(self.header_text(), "float" if dtype == torch.float32 else "double", int(variant))
+        return rtc.compile_user_model(self.header_text(), "float" if dtype == torch.float32 else "double", int(variant),
+                                      self.copies)
 
     def rtc_handle(self, lib, dtype, variant):
         """The handle `MppiFusedParams.user_model` takes: the compiled kernels registered with the C library on the
@@ -348,6 +372,8 @@ struct UserModel {{
             rc = lib.mppi_user_model_register(buf, len(cubin), self.nx, self.nu, max(len(self.params), 1),
                                               _cabi.F32 if dtype == torch.float32 else _cabi.F64, int(variant), arr, C.byref(handle))
             _cabi.check(rc, "mppi_user_model_register")
+            if self.copies > 1:
+                _cabi.check(lib.mppi_user_model_set_copies(handle, self.copies), "mppi_user_model_set_copies")
             self._rtc_handles[key] = handle
         return self._rtc_handles[key]
 

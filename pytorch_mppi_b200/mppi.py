@@ -6,8 +6,9 @@ Two execution routes, chosen at construction:
 * fused  — dynamics / running_cost (/ terminal cost) are bound methods of one registered analytic
            model (pytorch_mppi_b200.models): ONE kernel launch per ``command()`` does sampling,
            rollout, softmin and the nominal update (csrc/mppi_fused.cuh `fused_command_kernel`).
-           A step-dependent CudaModel takes this route with ``step_dependent_dynamics=True``.
-* stepped — arbitrary Python callables (a torch MLP, plain step-dependent functions, M>1 rollouts, a
+           A step-dependent CudaModel takes this route with ``step_dependent_dynamics=True``, a CudaModel compiled
+           with ``copies=M`` with ``rollout_samples=M``.
+* stepped — arbitrary Python callables (a torch MLP, plain step-dependent functions, M>1 rollouts of other models, a
            SpecificActionSampler): the T-loop stays in Python exactly like mppi.py:312-322, with the
            sampling (`mppi_sample_perturb`), cost accumulation (`mppi_cost_accumulate`) and softmin
            update (`mppi_softmin_update`) as kernels.
@@ -76,15 +77,21 @@ def fused_route_model(dynamics, running_cost, terminal_state_cost, nx, nu, rollo
     """The registered model a controller with these arguments runs on the fused route, or None (stepped route).
     A model's compiled bodies take the horizon index t exactly when the reference would pass it (mppi.py:147-157): a
     step-dependent CudaModel needs step_dependent_dynamics=True, and a model without t takes the fused route only
-    without it."""
+    without it.  A CudaModel compiled with copies=M is the M-copy rollout of rollout_samples=M (mppi.py:334-373): it
+    needs rollout_samples == M, and runs fused without a SpecificActionSampler."""
     owner = AnalyticModel.owner_of(dynamics) or AnalyticModel.owner_of(running_cost)
     if owner is not None and owner.step_dependent and not step_dependent_dynamics:
         raise ValueError("this model is step-dependent (its dynamics / running_cost take the horizon index t): "
                          "pass step_dependent_dynamics=True")
-    if rollout_samples != 1 or specific_action_sampler is not None:
+    copies = owner.copies if owner is not None else 1
+    if copies > 1 and rollout_samples != copies:
+        raise ValueError(f"this model is compiled with copies={copies} (its bodies take the copy index m): "
+                         f"pass rollout_samples={copies}")
+    if rollout_samples != copies or specific_action_sampler is not None:
         return None
     m = resolve_fused_model(dynamics, running_cost, terminal_state_cost)
-    if m is None or m.nx != nx or m.nu != nu or m.step_dependent != bool(step_dependent_dynamics):
+    if (m is None or m.nx != nx or m.nu != nu or m.step_dependent != bool(step_dependent_dynamics)
+            or m.copies != copies):
         return None
     return m
 
@@ -294,6 +301,8 @@ class MPPI:
     u_max = _mk("u_max")
     noise_mu = _mk("noise_mu")
     u_init = _mk("u_init")
+    rollout_var_cost = _mk("rollout_var_cost")
+    rollout_var_discount = _mk("rollout_var_discount")
     del _mk
 
     # ------------------------------------------------------------------------------------------
@@ -409,6 +418,13 @@ class MPPI:
                 p.sigma_inv[i * _cabi.MPPI_MAX_NU + j] = float(Si[i, j]) if inside else 0.0
         p.w_action_seq_cost = 0.0
         p.delta_t = 1.0
+        # rollout_samples M > 1 on the fused route (a CudaModel with copies=M): the (T) discount table, mppi.py:174-175
+        self._var_disc = None
+        if self._model is not None and self.M > 1:
+            self._var_disc = (self.rollout_var_discount ** torch.arange(self.T, dtype=self.dtype)).to(self.d)
+        p.rollout_samples = self.M if self._model is not None else 0
+        p.rollout_var_cost = float(self.rollout_var_cost)
+        p.var_discount = None if self._var_disc is None else self._var_disc.data_ptr()
         self._ext_arr = self._fill_model_params(p)
         self._model_version = self._model._param_version if self._model is not None else 0
         self._base_flags = ((_cabi.FLAG_NULL_ACTION if self.sample_null_action else 0)
@@ -1179,7 +1195,7 @@ class MPPI:
         nth = None if self._noise_theta_buf is None else self._noise_theta_buf.data_ptr()
         st_ptr = None
         if want_states:
-            self._states_buf = torch.empty(self._K_local, self.T, self.nx, device=self.d, dtype=self.dtype)
+            self._states_buf = torch.empty(self.M, self._K_local, self.T, self.nx, device=self.d, dtype=self.dtype)
             st_ptr = self._states_buf.data_ptr()
         _cabi.check(self._lib.mppi_materialize(C.byref(p), self._pa_buf.data_ptr(), self._noise_buf.data_ptr(), nth,
                                                st_ptr, stream), "mppi_materialize")
@@ -1217,13 +1233,13 @@ class MPPI:
 
     @property
     def states(self):
-        """(1,K,T,nx) iff a terminal cost is set (mppi.py:307-310, test_mppi.py:241-260)"""
+        """(M,K,T,nx) iff a terminal cost is set (mppi.py:307-310, 345, test_mppi.py:241-260); M = rollout_samples"""
         if self.cost_total is None or self.terminal_state_cost is None:
             return None
         if self._model is None:
             return self._states
         self._materialize(want_states=True)
-        return self._states_buf.unsqueeze(0)
+        return self._states_buf
 
     @property
     def actions(self):
@@ -1232,7 +1248,8 @@ class MPPI:
         if self._model is None:
             return self._actions
         self._materialize()
-        return self._pa_buf.unsqueeze(0)          # (u_scale * pa) / u_scale, mppi.py:412
+        # (u_scale * pa) / u_scale, mppi.py:412; the M copies of a sample share its actions (mppi.py:355)
+        return self._pa_buf.unsqueeze(0).expand(self.M, -1, -1, -1)
 
     @property
     def beta(self):

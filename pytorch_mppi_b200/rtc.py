@@ -72,20 +72,23 @@ def _sources_hash() -> str:
     return h.hexdigest()
 
 
-def kernel_names(real: str, variant: int):
+def kernel_names(real: str, variant: int, copies: int = 1):
     """Name expressions of the kernels one (dtype, controller variant) needs, in mppi_user_model_register's order:
-    fused, split-cost, batched (MPPI variant only), resident, states."""
+    fused, split-cost, batched (MPPI variant only), resident, states.  A model with copies > 1 has only the fused
+    (single-loop) and states kernels: the split-cost rollout and the kernels built on it roll out one copy per sample,
+    and MPPI_Batched has no rollout_samples."""
     m = "mppi::UserModel"
+    one = copies == 1
     return [f"&mppi::fused_command_kernel<{m}, {real}, {variant}, false, false>",
-            f"&mppi::fused_command_kernel<{m}, {real}, {variant}, false, true>",
-            f"&mppi::fused_command_kernel<{m}, {real}, 0, true>" if variant == 0 else None,
-            f"&mppi::resident_command_kernel<{m}, {real}, {variant}>",
+            f"&mppi::fused_command_kernel<{m}, {real}, {variant}, false, true>" if one else None,
+            f"&mppi::fused_command_kernel<{m}, {real}, 0, true>" if variant == 0 and one else None,
+            f"&mppi::resident_command_kernel<{m}, {real}, {variant}>" if one else None,
             f"&mppi::states_kernel<{m}, {real}>"]
 
 
-def compile_user_model(header_text: str, real: str, variant: int):
+def compile_user_model(header_text: str, real: str, variant: int, copies: int = 1):
     """-> (cubin bytes, [lowered kernel name or None] x 5).  Cached on disk."""
-    tag = hashlib.sha1(f"{header_text}|{real}|{variant}|{_sources_hash()}".encode()).hexdigest()[:20]
+    tag = hashlib.sha1(f"{header_text}|{real}|{variant}|{copies}|{_sources_hash()}".encode()).hexdigest()[:20]
     cubin_path = os.path.join(CACHE, f"rtc_{tag}.cubin")
     names_path = os.path.join(CACHE, f"rtc_{tag}.json")
     if os.path.exists(cubin_path) and os.path.exists(names_path):
@@ -97,7 +100,7 @@ def compile_user_model(header_text: str, real: str, variant: int):
     if lib.nvrtcCreateProgram(C.byref(prog), src.encode(), b"mppi_user_model.cu", 0, None, None) != 0:
         raise RtcError("nvrtcCreateProgram failed")
     try:
-        exprs = kernel_names(real, variant)
+        exprs = kernel_names(real, variant, copies)
         for e in exprs:
             if e is not None and lib.nvrtcAddNameExpression(prog, e.encode()) != 0:
                 raise RtcError(f"nvrtcAddNameExpression({e}) failed")

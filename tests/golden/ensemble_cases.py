@@ -1,0 +1,135 @@
+"""Golden cases of rollout_samples M > 1 with copies that differ (reference mppi.py:334-373): the models of
+tests/ensemble_models.py under MPPI, SMPPI and KMPPI.  Fixtures tests/golden/ens_*.npz, produced by the live reference
+(tests/golden/make_golden_ensemble.py); kept apart from cases.CASES so that the tests parametrised over those do not see
+them.  The step-dependent case hands the oracle its callables through step_cases.HorizonClock: an M-copy rollout also
+calls dynamics, then the running cost, once per horizon step.
+
+The oracle's `mppi_command` rolls out through `rollout`, which dispatches on M (mppi.py:292-295), but its `smppi_command`
+and `kmppi_command` call the one-copy `rollout_costs` by name, while the reference's SMPPI and KMPPI dispatch on M too
+(mppi.py:564, inherited `_compute_rollout_costs`).  `EnsembleOracleRunner` therefore binds that name to
+`rollout_costs_multi` for the duration of each command (`multi_copy_rollouts`); the oracle itself is unchanged."""
+import contextlib
+import functools
+
+import torch
+
+from oracle import mppi_oracle as orc
+from tests import ensemble_models as em
+from tests.golden.cases import _DT
+from tests.golden.replay import Stream
+from tests.golden.step_cases import HorizonClock
+
+ENSEMBLE_CASES = {
+    "ens_pend_mppi_f64": dict(variant="mppi", model="pendulum", dtype="f64", M=4, K=512, T=20, lambda_=1.0,
+                              noise_sigma=1.0, u_max=2.0, x0=[2.5, 0.5], var_cost=0.5, var_discount=0.9, steps=3, seed=901),
+    "ens_pend_smppi_f32": dict(variant="smppi", model="pendulum", dtype="f32", M=3, K=1024, T=16, lambda_=1.0,
+                               noise_sigma=0.5, u_max=2.0, x0=[2.0, -0.3], var_cost=0.8, var_discount=0.95,
+                               smooth=dict(w=0.5, delta_t=0.5, action_max=2.0), steps=3, seed=902),
+    "ens_pend_kmppi_f64": dict(variant="kmppi", model="pendulum", dtype="f64", M=8, K=256, T=16, lambda_=1.0,
+                               noise_sigma=1.0, u_max=2.0, x0=[2.8, 0.0], var_cost=0.3, var_discount=0.85,
+                               kernel=dict(S=5, sigma=2.0), steps=3, seed=903),
+    "ens_stepint_mppi_f64": dict(variant="mppi", model="scenario_integrator", dtype="f64", M=4, K=384, T=15, lambda_=1.0,
+                                 noise_sigma=1.0, u_max=3.0, x0=[0.0, 0.0], var_cost=1.0, var_discount=0.9, steps=3,
+                                 seed=904),
+}
+
+
+def case_params(case):
+    if case["model"] == "pendulum":
+        return em.pendulum_params(case["M"])
+    return em.scenario_params(case["M"], case["T"])
+
+
+def callables(case, params=None):
+    """(dynamics, running_cost, terminal cost) the reference is given for these parameters (default: the case's);
+    the scenario integrator's take t."""
+    p = case_params(case) if params is None else params
+    M, K, T = case["M"], case["K"], case["T"]
+    if case["model"] == "pendulum":
+        return (functools.partial(em.pend_dyn, p=p, M=M, K=K), functools.partial(em.pend_cost, p=p),
+                functools.partial(em.pend_term, p=p, M=M))
+    return (functools.partial(em.si_dyn, p=p, M=M, T=T, K=K), functools.partial(em.si_cost, p=p),
+            functools.partial(em.si_term, p=p, M=M))
+
+
+def shifted_params(case, shift):
+    """The case's parameters with copy m's values at copy m - shift: what a twin whose copy index is off by `shift`
+    reads.  (Every copy's rollout is then another copy's, so only a twin that also evaluates a copy-dependent cost with
+    the right index, as the terminal costs here, can tell.)"""
+    p, M, T = case_params(case), case["M"], case["T"]
+    perm = [(m + shift) % M for m in range(M)]
+    if case["model"] == "pendulum":
+        return p[:6] + [p[6 + j] for j in perm] + [p[6 + M + j] for j in perm]
+    return p[:3 + M] + sum((p[3 + M + j * T:3 + M + (j + 1) * T] for j in perm), [])
+
+
+def ensemble_problem(case, dyn_params=None):
+    """The oracle's Problem of a case; with `dyn_params`, its dynamics read those parameters instead of the case's."""
+    dt = _DT[case["dtype"]]
+    f, c, term = callables(case)
+    if dyn_params is not None:
+        f = callables(case, dyn_params)[0]
+    if case["model"] == "scenario_integrator":
+        clock = HorizonClock(f, c, case["T"])
+        f, c = clock.dynamics, clock.running_cost
+    return orc.Problem(f, c, 2, torch.tensor(case["noise_sigma"], dtype=dt), K=case["K"], T=case["T"],
+                       lambda_=case["lambda_"], u_max=torch.tensor(case["u_max"], dtype=dt), terminal_state_cost=term,
+                       rollout_samples=case["M"], rollout_var_cost=case["var_cost"],
+                       rollout_var_discount=case["var_discount"])
+
+
+@contextlib.contextmanager
+def multi_copy_rollouts():
+    """Inside: the oracle's `rollout_costs` is `rollout_costs_multi`, the rollout of an M > 1 command (see the module
+    docstring).  Only for problems with rollout_samples > 1."""
+    one_copy = orc.rollout_costs
+    orc.rollout_costs = orc.rollout_costs_multi
+    try:
+        yield
+    finally:
+        orc.rollout_costs = one_copy
+
+
+def plant_step(case, x, u):
+    """The closed loop's simulated system: copy 0 (at t = 0)."""
+    f, _, _ = callables(case)
+    return f(x, u) if case["model"] == "pendulum" else f(x, u, 0)
+
+
+class EnsembleOracleRunner:
+    """Steps the oracle through an ensemble case on the fixture's injected draws."""
+
+    def __init__(self, case, dyn_params=None):
+        self.case = case
+        self.prob = ensemble_problem(case, dyn_params)
+        dt = self.prob.dtype
+        self.stream = Stream(case, self.prob)
+        T = case["T"]
+        self.U = self.stream.U0.clone()
+        if case["variant"] == "smppi":
+            sm = case["smooth"]
+            self.U, self.A = torch.zeros(T, 1, dtype=dt), torch.zeros(T, 1, dtype=dt)
+            self.sp = orc.SmoothParams(w_action_seq_cost=sm["w"], delta_t=sm["delta_t"],
+                                       action_max=torch.tensor(sm["action_max"], dtype=dt))
+        if case["variant"] == "kmppi":
+            S, sig = case["kernel"]["S"], case["kernel"]["sigma"]
+            self.theta = torch.zeros(S, 1, dtype=dt)
+            self.W, self.Wshift = orc.kernel_matrices(T, S, lambda a, b: orc.rbf_kernel(a, b, sig), dt)
+
+    def step(self, x, z):
+        v = self.case["variant"]
+        if v == "mppi":
+            r = orc.mppi_command(self.prob, self.U, x, z)
+        elif v == "smppi":
+            with multi_copy_rollouts():
+                r = orc.smppi_command(self.prob, self.sp, self.U, self.A, x, z)
+            self.A = r["action_sequence"]
+        else:
+            with multi_copy_rollouts():
+                r = orc.kmppi_command(self.prob, self.U, self.theta, x, z, self.W, self.Wshift)
+            self.theta = r["theta"]
+        self.U = r["U"]
+        return r
+
+    def advance(self, x, action):
+        return plant_step(self.case, x.view(1, -1), (self.prob.u_scale * action).view(1, -1)).view(-1)
