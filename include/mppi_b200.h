@@ -51,6 +51,8 @@ typedef enum MppiModel {
     MPPI_MODEL_PENDULUM = 1,      /* reference tests/pendulum.py:30-60                      */
     MPPI_MODEL_LINEAR_POINT = 2,  /* tests/test_mppi.py:24-51 and tests/smooth_mppi.py:29-142    */
     MPPI_MODEL_PENDULUM_MLP = 3,  /* tests/pendulum_approximate.py:47-67 (3-32-32-2 tanh residual MLP) */
+    MPPI_MODEL_PENDULUM_MLP_ENSEMBLE = 4,  /* rollout_samples = M networks of PENDULUM_MLP's shape, one per copy
+                                              (a bootstrapped ensemble of learned dynamics); weights in model_weights */
     MPPI_MODEL_USER = 100         /* a user-written model compiled at run time and registered with
                                      mppi_user_model_register (see pytorch_mppi_b200.models.CudaModel): the
                                      reference accepts arbitrary Python callables (mppi.py:63-64) — this is the
@@ -66,6 +68,10 @@ typedef enum MppiModel {
  *                 wgmma kernel, fp32 accumulate: 1 = hi/lo-split bf16 operands, 2 = plain bf16; 3 = automatic:
  *                 mode 1 wherever that kernel exists — fp32, one environment — else the FFMA kernel); the 1,250 weights go in
  *                 model_params_ext: W1 (32x3 row-major), b1 (32), W2 (32x32), b2 (32), W3 (2x32), b3 (2)
+ *  PENDULUM_MLP_ENSEMBLE : [0..3] as PENDULUM_MLP.  The M = rollout_samples (2..MPPI_MAX_COPIES) networks' weights are
+ *                 NOT in model_params_ext but in the device buffer model_weights: (M, 1250) in the controller dtype, row
+ *                 m = network m in PENDULUM_MLP's model_params_ext order.  Copy m of every sample is rolled out through
+ *                 network m.  No split-cost, batched or resident kernels.
  */
 
 enum {
@@ -187,6 +193,9 @@ typedef struct MppiFusedParams {
     double rollout_var_cost;
     const void* var_discount;    /* (T) device buffer of the controller dtype: rollout_var_discount ** arange(T)
                                     (mppi.py:174-175); required when rollout_samples > 1                        */
+    const void* model_weights;   /* model == MPPI_MODEL_PENDULUM_MLP_ENSEMBLE: (rollout_samples, 1250) DEVICE buffer of
+                                    the controller dtype, one network per row (see the model_params layouts); read by
+                                    every command, so it must outlive the plan.  Required for that model, else unused */
 } MppiFusedParams;
 
 typedef struct MppiLaunchInfo {
@@ -207,7 +216,8 @@ typedef struct MppiLaunchInfo {
 
 int mppi_b200_abi_version(void);
 /* Layout probe for foreign-language mirrors of MppiFusedParams: which=0 sizeof, 1 offsetof(seed),
- * 2 offsetof(state), 3 offsetof(U), 4 offsetof(rank), 5 offsetof(partial_out), 6 sizeof(MppiLaunchInfo). */
+ * 2 offsetof(state), 3 offsetof(U), 4 offsetof(rank), 5 offsetof(partial_out), 6 sizeof(MppiLaunchInfo),
+ * 7 offsetof(model_weights). */
 uint64_t mppi_abi_layout(int which);
 const char* mppi_status_string(int status);
 const char* mppi_last_cuda_error(void);

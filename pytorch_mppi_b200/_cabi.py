@@ -22,6 +22,7 @@ ABI_VERSION = 1
 VARIANT_MPPI, VARIANT_SMPPI, VARIANT_KMPPI = 0, 1, 2
 F32, F64 = 0, 1
 MODEL_PENDULUM, MODEL_LINEAR_POINT, MODEL_PENDULUM_MLP = 1, 2, 3
+MODEL_PENDULUM_MLP_ENSEMBLE = 4
 MODEL_USER = 100
 FLAG_SHIFT = 1 << 0
 FLAG_NULL_ACTION = 1 << 1
@@ -110,6 +111,7 @@ class MppiFusedParams(C.Structure):
         ("rollout_samples", C.c_int32),
         ("rollout_var_cost", C.c_double),
         ("var_discount", C.c_void_p),
+        ("model_weights", C.c_void_p),
     ]
 
 

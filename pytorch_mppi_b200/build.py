@@ -34,7 +34,7 @@ NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-
 
 # name -> (source, extra defines, headers it depends on)
 UNITS = {"cabi": ("mppi_b200.cu", [], CABI_HEADERS)}
-for _mid, _mname in ((1, "pendulum"), (2, "linear_point"), (3, "pendulum_mlp")):
+for _mid, _mname in ((1, "pendulum"), (2, "linear_point"), (3, "pendulum_mlp"), (4, "pendulum_mlp_ensemble")):
     for _f64 in (0, 1):
         UNITS[f"model_{_mname}_{'f64' if _f64 else 'f32'}"] = (
             "mppi_model_tu.cu", [f"-DMPPI_TU_MODEL={_mid}", f"-DMPPI_TU_F64={_f64}"], MODEL_HEADERS)

@@ -18,6 +18,8 @@ const ModelKernels* model_kernels_linear_point_f32();
 const ModelKernels* model_kernels_linear_point_f64();
 const ModelKernels* model_kernels_pendulum_mlp_f32();
 const ModelKernels* model_kernels_pendulum_mlp_f64();
+const ModelKernels* model_kernels_pendulum_mlp_ensemble_f32();
+const ModelKernels* model_kernels_pendulum_mlp_ensemble_f64();
 }  // namespace mppi_host
 
 namespace {
@@ -45,6 +47,13 @@ const ModelKernels* find_kernels(const MppiFusedParams* p, int* rc) {
             }
             get = f32 ? model_kernels_pendulum_mlp_f32 : model_kernels_pendulum_mlp_f64;
             break;
+        case MPPI_MODEL_PENDULUM_MLP_ENSEMBLE:
+            if (p->model_weights == nullptr) {
+                *rc = MPPI_ERR_BAD_ARG;
+                return nullptr;
+            }
+            get = f32 ? model_kernels_pendulum_mlp_ensemble_f32 : model_kernels_pendulum_mlp_ensemble_f64;
+            break;
         case MPPI_MODEL_USER: {
             const UserModelHandle* h = reinterpret_cast<const UserModelHandle*>(p->user_model);
             if (h == nullptr || h->magic != kUserMagic || h->mk.is_double != (f32 ? 0 : 1)) {
@@ -57,11 +66,13 @@ const ModelKernels* find_kernels(const MppiFusedParams* p, int* rc) {
     return get != nullptr ? get() : nullptr;
 }
 
-// rollout_samples M > 1 (mppi.py:334-373) on the fused route: only a user model compiled with M copies makes its copies
-// differ (a registered model's M rollouts would be identical).  No CUDA call.
+// rollout_samples M > 1 (mppi.py:334-373) on the fused route: only a user model compiled with M copies, or the ensemble
+// of M networks, makes its copies differ (another registered model's M rollouts would be identical).  No CUDA call.
 int check_rollout_samples(const MppiFusedParams* p, const ModelKernels* mk) {
     if (p->rollout_samples < 0) return MPPI_ERR_BAD_ARG;
     const int M = p->rollout_samples > 1 ? p->rollout_samples : 1;
+    if (p->model == MPPI_MODEL_PENDULUM_MLP_ENSEMBLE)
+        return M >= 2 && M <= MPPI_MAX_COPIES && p->var_discount != nullptr ? MPPI_OK : MPPI_ERR_BAD_ARG;
     if (M > 1 && p->model != MPPI_MODEL_USER)
         return UNSUPPORTED("rollout_samples > 1 on the fused route needs a user model compiled with that many copies");
     const int copies = mk->copies > 1 ? mk->copies : 1;
@@ -310,6 +321,7 @@ uint64_t mppi_abi_layout(int which) {
         case 4: return offsetof(MppiFusedParams, rank);
         case 5: return offsetof(MppiFusedParams, partial_out);
         case 6: return sizeof(MppiLaunchInfo);
+        case 7: return offsetof(MppiFusedParams, model_weights);
     }
     return 0;
 }
@@ -399,14 +411,14 @@ int mppi_plan_command(void* plan, const double* state, const void* state_dev, ui
 int mppi_plan_set_model_params(void* plan, const double* model_params, const double* ext, int32_t n_ext) {
     Plan* pl = reinterpret_cast<Plan*>(plan);
     if (pl == nullptr || model_params == nullptr || n_ext < 0 || (n_ext > 0 && ext == nullptr)) return MPPI_ERR_BAD_ARG;
-    if (pl->mk->is_mlp && (n_ext < PendulumMLPModel::N_EXT || model_params[2] != pl->p.model_params[2] ||
+    if (pl->mk->is_mlp && ((pl->mk->is_mlp == 1 && n_ext < PendulumMLPModel::N_EXT) || model_params[2] != pl->p.model_params[2] ||
                            model_params[3] != pl->p.model_params[3]))
         return MPPI_ERR_BAD_ARG;      // the weights are required, and [2] / [3] selected the plan's kernel
     if (pl->res.armed) return UNSUPPORTED("the resident grid holds the parameters it was launched with: stop it first");
     memcpy(pl->p.model_params, model_params, sizeof(pl->p.model_params));
     pl->p.model_params_ext = ext;
     pl->p.n_model_params_ext = n_ext;
-    pl->mk->load(pl->mk, pl->mparams, pl->p.model_params, ext, n_ext);
+    load_model_params(pl->mk, &pl->p, pl->mparams);
     return MPPI_OK;
 }
 

@@ -1487,23 +1487,27 @@ MPPI_UNROLL_N(2)
 }
 
 // one step's costs c[0..M-1] of the M copies (mppi.py:362-364): cs[m] += c[m], and var += var_m(c) * disc with the
-// two-pass unbiased variance of cost_accumulate_kernel (mean = sum_m c / M, then sum_m (c - mean)^2 / (M - 1))
+// two-pass unbiased variance of cost_accumulate_kernel (mean = sum_m c / M, then sum_m (c - mean)^2 / (M - 1)).
+// Models with copies at run time: M is the arrays' capacity and the first n <= M copies are folded.
 template <typename real, int M>
-__device__ __forceinline__ void copies_fold(real* cs, real& var, const real* c, real disc) {
+__device__ __forceinline__ void copies_fold(real* cs, real& var, const real* c, real disc, const int n = M) {
     typedef Ops<real> O;
     real mean = c[0];
 #pragma unroll
-    for (int m = 1; m < M; ++m) mean = O::add(mean, c[m]);
-    mean = O::div(mean, (real)M);
+    for (int m = 1; m < M; ++m)
+        if (m < n) mean = O::add(mean, c[m]);
+    mean = O::div(mean, (real)n);
     real ss = (real)0;
 #pragma unroll
     for (int m = 0; m < M; ++m) {
+        if (m >= n) break;
         const real d = O::sub(c[m], mean);
         ss = O::add(ss, O::mul(d, d));
     }
-    var = O::add(var, O::mul(O::div(ss, (real)(M - 1)), disc));
+    var = O::add(var, O::mul(O::div(ss, (real)(n - 1)), disc));
 #pragma unroll
-    for (int m = 0; m < M; ++m) cs[m] = O::add(cs[m], c[m]);
+    for (int m = 0; m < M; ++m)
+        if (m < n) cs[m] = O::add(cs[m], c[m]);
 }
 
 // ---- stage C'', rollout of a model with COPIES = M > 1 (rollout_samples, mppi.py:334-373), on the sample's rollout
@@ -1511,11 +1515,16 @@ __device__ __forceinline__ void copies_fold(real* cs, real& var, const real* c, 
 // chains, interleaved in registers.  Per copy the running costs are summed t = 0..T-1, the discounted variance over the
 // copies is accumulated per step, then cost = (mean_m(cost_m + terminal_m) + var * rollout_var_cost) + perturbation
 // (+ SMPPI smoothness), in the reference's order (mppi.py:369-372, 415-416).  Stores cost_total[k] and returns it.
+// A model with copies at run time (PendulumMLPEnsembleModel: a network per copy) rolls out mc = Model::copies(P) <= M
+// copies, and the loops over them stay rolled (UNR = 1): its step is inlined once, and the per-copy arrays live in
+// local memory (a few L1 accesses per copy and step, against the step's 1,184 FMAs).
 template <class Model, typename real, int VARIANT>
 __device__ __forceinline__ real copies_rollout(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
                                                int k, unsigned long long kg) {
     typedef Ops<real> O;
     constexpr int NX = Model::NX, NU = Model::NU, M = ModelCopies<Model>::value;
+    constexpr int UNR = CopiesAtRunTime<Model>::value ? 1 : M;
+    const int mc = model_copies<Model, real>(mp);
     const NoiseModel<real>& nm = a.nm;
     const int T = a.T;
     real x[M][NX];
@@ -1546,22 +1555,22 @@ __device__ __forceinline__ real copies_rollout(const KArgs<real>& a, const typen
         for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);                // mppi.py:355
 #if MPPI_ROLLOUT_PIPELINED
         // step t-1's costs in iteration t, as the single loop of one copy: its variance takes disc[t-1]
-#pragma unroll
-        for (int m = 0; m < M; ++m) {
+        MPPI_UNROLL_N(UNR)
+        for (int m = 0; m < mc; ++m) {
             real xs[NX];
 #pragma unroll
             for (int i = 0; i < NX; ++i) xs[i] = x[m][i];
             model_step<Model, real>(mp, x[m], u, t, m);                                 // mppi.py:357
             if (t > 0) c[m] = model_cost<Model, real>(mp, xs, uprev, t - 1, m);         // mppi.py:362 (step t-1)
         }
-        if (t > 0) copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t - 1));         // mppi.py:363-364
+        if (t > 0) copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t - 1), mc);     // mppi.py:363-364
 #else
-#pragma unroll
-        for (int m = 0; m < M; ++m) {
+        MPPI_UNROLL_N(UNR)
+        for (int m = 0; m < mc; ++m) {
             model_step<Model, real>(mp, x[m], u, t, m);                                 // mppi.py:357
             c[m] = model_cost<Model, real>(mp, x[m], u, t, m);                          // mppi.py:362
         }
-        copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t));                         // mppi.py:363-364
+        copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t), mc);                     // mppi.py:363-364
 #endif
         pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
         if (VARIANT == V_SMPPI) {
@@ -1581,19 +1590,20 @@ __device__ __forceinline__ real copies_rollout(const KArgs<real>& a, const typen
 #if MPPI_ROLLOUT_PIPELINED
     {
         real c[M];
-#pragma unroll
-        for (int m = 0; m < M; ++m) c[m] = model_cost<Model, real>(mp, x[m], uprev, T - 1, m);   // step T-1
-        copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + T - 1));
+        MPPI_UNROLL_N(UNR)
+        for (int m = 0; m < mc; ++m) c[m] = model_cost<Model, real>(mp, x[m], uprev, T - 1, m);  // step T-1
+        copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + T - 1), mc);
     }
 #endif
     if (Model::template has_terminal<real>(mp)) {
-#pragma unroll
-        for (int m = 0; m < M; ++m) cs[m] = O::add(cs[m], model_terminal<Model, real>(mp, x[m], m));   // mppi.py:369-370
+        MPPI_UNROLL_N(UNR)
+        for (int m = 0; m < mc; ++m) cs[m] = O::add(cs[m], model_terminal<Model, real>(mp, x[m], m));  // mppi.py:369-370
     }
     real mean = cs[0];
 #pragma unroll
-    for (int m = 1; m < M; ++m) mean = O::add(mean, cs[m]);
-    mean = O::div(mean, (real)M);                                                         // mppi.py:371
+    for (int m = 1; m < M; ++m)
+        if (m < mc) mean = O::add(mean, cs[m]);
+    mean = O::div(mean, (real)mc);                                                        // mppi.py:371
     real c_tot = O::add(O::add(mean, O::mul(var, a.var_cost)), pert);                     // mppi.py:372, 416
     if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));           // mppi.py:562,569
     a.cost_total[k] = c_tot;

@@ -72,7 +72,9 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     Geometry g;
     int rc;
     if (tc_route) {
-        rc = plan_geometry<real>(kernel, &pg, 0, false, g);
+        // the ensemble's kernel keeps every copy's network and step buffers behind the layout
+        const int ens_bytes = mk->is_mlp == 2 ? PendulumMLPEnsembleModel::tc_smem_bytes(p->rollout_samples) : 0;
+        rc = plan_geometry<real>(kernel, &pg, 0, false, g, ens_bytes);
         if (rc) return rc;
         c = FusedChoice{kernel, g, 0, 1};
         return MPPI_OK;
@@ -202,7 +204,7 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
     finish_kargs<real>(p, c, *a);
     if (a->world > 1 && rows_of(p) > MPPI_XCHG_MAX_R) return UNSUPPORTED("T*nu exceeds the peer mailbox record size");
     if (a->export_partial && p->partial_out == nullptr) return MPPI_ERR_BAD_ARG;
-    mk->load(mk, pl->mparams, p->model_params, p->model_params_ext, p->n_model_params_ext);
+    load_model_params(mk, p, pl->mparams);
     pl->mk = mk;
     pl->kernel = c.kernel;
     pl->res_kernel = nullptr;
@@ -230,7 +232,7 @@ int launch_states(const ModelKernels* mk, const MppiFusedParams* p, KArgs<real>&
                   long long stride, cudaStream_t stream, int copies = 1) {
     alignas(16) unsigned char mp[MPPI_MODEL_BLOCK_BYTES];
     if (mk->param_bytes > (int)sizeof(mp)) return UNSUPPORTED("model parameter block too large");
-    mk->load(mk, mp, p->model_params, p->model_params_ext, p->n_model_params_ext);
+    load_model_params(mk, p, mp);
     const real* pa = (const real*)actions;
     real* st = (real*)states;
     void* argv[5] = {(void*)&pa, (void*)&st, (void*)&a, (void*)mp, (void*)&stride};

@@ -65,7 +65,8 @@ struct Plan {
 struct ModelKernels {
     int nx, nu;
     int is_double;
-    int is_mlp;                      // PendulumMLP: no split-cost / resident variants; tensor-core kernels in `tc`
+    int is_mlp;                      // 1 PendulumMLP, 2 its ensemble: no split-cost / resident variants; tensor-core
+                                     // kernels in `tc`
     int np;                          // run-time user models: reals in the parameter block (P = { real v[np]; })
     int param_bytes;                 // sizeof(Model::P<real>)
     void (*load)(const ModelKernels* self, void* dst, const double* blob, const double* ext, int n_ext);
@@ -76,6 +77,7 @@ struct ModelKernels {
     const void* resident_stamped;    // the one instantiation with %globaltimer stamps, or nullptr
     const void* states;              // states_kernel<Model, real>
     const void* tc[3][2][2];         // mlp_tc_command_kernel<V, SPLIT = 2 - mode, FAST>, [V][mode - 1][fast]; fp32 MLP only
+                                     // (the ensemble: mlp_ens_tc_command_kernel)
     void* library;                   // run-time user models: the cudaLibrary_t that owns the kernels
     int copies;                      // run-time user models: the COPIES their kernels were compiled with (0 or 1: none)
 };
@@ -136,6 +138,16 @@ inline int validate(const MppiFusedParams* p, bool fused = false) {
 }
 
 inline int rows_of(const MppiFusedParams* p) { return (p->variant == MPPI_VARIANT_KMPPI ? p->S : p->T) * p->nu; }
+
+// The model's parameter block for these parameters (the packer of its unit).  The ensemble's block also carries the
+// device weight table and the copy count, which are not doubles of model_params.
+inline void load_model_params(const ModelKernels* mk, const MppiFusedParams* p, void* dst) {
+    mk->load(mk, dst, p->model_params, p->model_params_ext, p->n_model_params_ext);
+    if (p->model == MPPI_MODEL_PENDULUM_MLP_ENSEMBLE) {
+        if (mk->is_double) PendulumMLPEnsembleModel::bind<double>(*reinterpret_cast<PendulumMLPEnsembleModel::P<double>*>(dst), p->model_weights, p->rollout_samples);
+        else PendulumMLPEnsembleModel::bind<float>(*reinterpret_cast<PendulumMLPEnsembleModel::P<float>*>(dst), p->model_weights, p->rollout_samples);
+    }
+}
 
 template <typename real> void fill_noise_model(const MppiFusedParams* p, NoiseModel<real>& nm) {
     for (int i = 0; i < MPPI_MAX_NU; ++i) {
@@ -327,24 +339,26 @@ inline int refuse_capture(cudaStream_t stream, const Geometry& g) {
 
 struct GeomKey {
     const void* kernel;
-    int dev, variant, K, T, nu, S, bt, tp, gb, r2, single, ne;
+    int dev, variant, K, T, nu, S, bt, tp, gb, r2, single, ne, xb;
     bool operator==(const GeomKey& o) const {
         return kernel == o.kernel && dev == o.dev && variant == o.variant && K == o.K && T == o.T && nu == o.nu && S == o.S &&
-               bt == o.bt && tp == o.tp && gb == o.gb && r2 == o.r2 && single == o.single && ne == o.ne;
+               bt == o.bt && tp == o.tp && gb == o.gb && r2 == o.r2 && single == o.single && ne == o.ne && xb == o.xb;
     }
 };
 
 // Launch geometry for (kernel, dimensions).  The occupancy / attribute queries cost microseconds, so
 // the last few results are cached per thread: a steady-state command() pays only the lookup.
+// extra_bytes: dynamic shared memory the kernel uses behind the layout (the ensemble wgmma kernel's per-copy tiles).
 template <typename real, typename KernelT>
-int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool single_partial_grid, Geometry& g) {
+int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool single_partial_grid, Geometry& g,
+                  int extra_bytes = 0) {
     static thread_local GeomKey keys[8];
     static thread_local Geometry vals[8];
     static thread_local int n_cached = 0, next_slot = 0;
     int dev = 0;
     CK(cudaGetDevice(&dev));
     const GeomKey key{(const void*)kernel, dev, p->variant, p->K, p->T, p->nu, p->S, p->block_threads, p->threads_per_sample,
-                      p->grid_blocks, need_rows2, single_partial_grid ? 1 : 0, p->n_env > 1 ? p->n_env : 1};
+                      p->grid_blocks, need_rows2, single_partial_grid ? 1 : 0, p->n_env > 1 ? p->n_env : 1, extra_bytes};
     for (int i = 0; i < n_cached; ++i)
         if (keys[i] == key) {
             g = vals[i];
@@ -376,6 +390,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         const long long want_threads = per_sm < 768 ? per_sm : 768;
         for (int bs = 64; bs <= 512; bs += (bs < 128 ? 64 : 32)) {     // 64-sample tiles let K < 128 x SMs reach every SM
             SmemLayout Lc = make_layout<real>(p->variant, p->T, p->nu, p->S, R, bs, bs, single_partial_grid ? 1 : di.sm_count * 4, need_rows2);
+            Lc.total += extra_bytes;
             if (Lc.total > dyn0) continue;
             int occ_c = 0;
             CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ_c, kernel, bs, Lc.total));
@@ -426,6 +441,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
     SmemLayout L;
     for (int it = 0; it < 4; ++it) {
         L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
+        L.total += extra_bytes;
         if (L.total > dyn_limit) return UNSUPPORTED("shared-memory tile does not fit");
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, BD, L.total));
         if (occ < 1) return UNSUPPORTED("kernel does not fit on an SM with this block size");
@@ -437,6 +453,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         nb = nb2;
     }
     L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
+    L.total += extra_bytes;
     g.BS = BS;
     g.tps = tps;
     g.BD = BD;

@@ -319,6 +319,274 @@ __global__ void __launch_bounds__(256, 2) mlp_tc_command_kernel(const __grid_con
     publish_and_finish<real, VARIANT, NU>(a, sm, beta_run, eta_run);
 }
 
+// =================================================================================================
+// The ensemble (PendulumMLPEnsembleModel, rollout_samples = M networks, one per copy) on the same tiles.  Setup: every
+// copy's network is staged once per CTA from the device table into dynamic shared memory (PendulumMLPEnsembleModel::TC_*:
+// bf16 hi / lo tiles of W2 and W3, fp32 W1, b1, b2, b3).  Per step: the roller thread of a sample writes its clamped
+// action (its M states already sit in the copies' layer-1 input rows), one barrier, then for each copy m the warpgroups
+// run the network of mlp_tc_command_kernel on copy m's tiles into copy m's outputs, one barrier, and the roller updates
+// its M states in place.  Two barriers per step whatever M is.  The roller evaluates the M running costs of the states a
+// step produced one step later (as copies_rollout does) and folds them with copies_fold; after the loop,
+// (mean + var * rollout_var_cost) + perturbation (+ SMPPI smoothness).
+// M is a run-time value: the loop over the copies' networks stays rolled (nothing in it is indexed by m in registers),
+// and the roller's cost sums are unrolled to MPPI_MAX_COPIES with guards, so they stay in registers — one kernel per
+// (variant, operand mode, tanh) serves every M.  (With the M states in registers too, 4 of the 12 instantiations spilled
+// 4 B at this launch bound's 128-register cap; now none spills.)
+template <int VARIANT, int SPLIT, int FAST>
+__global__ void __launch_bounds__(256, 2) mlp_ens_tc_command_kernel(const __grid_constant__ KArgs<float> a,
+                                                                 const __grid_constant__ PendulumMLPEnsembleModel::P<float> mp) {
+    typedef float real;
+    typedef Ops<real> O;
+    typedef PendulumMLPEnsembleModel Model;
+    constexpr int NX = 2, NU = 1, H = tc::H, MC = Model::COPIES;
+    extern __shared__ __align__(16) unsigned char smem[];
+    const int tid = threadIdx.x, BD = blockDim.x;      // BD == 256: thread = (sample row tid % 128, half tid / 128)
+    const int row = tid & 127, half = tid >> 7;
+    const int lane = tid & 31, g = lane >> 2, t4 = lane & 3;
+    const int r0 = 64 * half + 16 * ((tid >> 5) & 3) + g, r1 = r0 + 8;
+    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BD / a.tps, gridDim.x, 0);
+    Smem<real> sm(smem, L);
+    const NoiseModel<real>& nm = a.nm;
+    const int T = a.T, M = mp.M;
+    // per-copy blocks behind the layout (the host adds Model::tc_smem_bytes(M) to the launch's dynamic shared memory)
+    unsigned char* const ens = smem + align_up(L.total, 128);
+    float* const sU = reinterpret_cast<float*>(ens + M * Model::TC_COPY);       // clamped action of every sample
+
+    // ---- one-time setup: every copy's network from the table -----------------------------------------------------------
+    for (int i = tid; i < M * (8 * H * 2 / 4); i += BD) {                      // W3 tiles: rows 2..7 stay zero
+        unsigned char* cp = ens + (i / (8 * H * 2 / 4)) * Model::TC_COPY;
+        const int j = i % (8 * H * 2 / 4);
+        reinterpret_cast<uint32_t*>(cp + Model::TC_W3)[j] = 0u;
+        reinterpret_cast<uint32_t*>(cp + Model::TC_W3LO)[j] = 0u;
+    }
+    __syncthreads();
+    for (int e = tid; e < M * H * H; e += BD) {
+        const int m = e / (H * H), nk = e - m * H * H, n = nk / H, k = nk - n * H;
+        unsigned char* cp = ens + m * Model::TC_COPY;
+        __nv_bfloat16 wh, wl;
+        tc::split_bf16(__ldg(mp.w + (size_t)m * Model::N_W + Model::OFF_W2 + nk), wh, wl);     // W2[n][k]
+        reinterpret_cast<__nv_bfloat16*>(cp + Model::TC_W2)[tc::tile_off(n, k) / 2] = wh;
+        reinterpret_cast<__nv_bfloat16*>(cp + Model::TC_W2LO)[tc::tile_off(n, k) / 2] = wl;
+    }
+    for (int e = tid; e < M * 2 * H; e += BD) {
+        const int m = e / (2 * H), nk = e - m * 2 * H, n = nk / H, k = nk - n * H;
+        unsigned char* cp = ens + m * Model::TC_COPY;
+        __nv_bfloat16 wh, wl;
+        tc::split_bf16(__ldg(mp.w + (size_t)m * Model::N_W + Model::OFF_W3 + nk), wh, wl);     // W3[n][k]
+        reinterpret_cast<__nv_bfloat16*>(cp + Model::TC_W3)[tc::tile_off(n, k) / 2] = wh;
+        reinterpret_cast<__nv_bfloat16*>(cp + Model::TC_W3LO)[tc::tile_off(n, k) / 2] = wl;
+    }
+    for (int e = tid; e < M * H; e += BD) {
+        const int m = e / H, i = e - m * H;
+        const float* w = mp.w + (size_t)m * Model::N_W;
+        unsigned char* cp = ens + m * Model::TC_COPY;
+        float* w1 = reinterpret_cast<float*>(cp + Model::TC_W1);
+#pragma unroll
+        for (int c = 0; c < 3; ++c) w1[c * H + i] = __ldg(w + 3 * i + c);                         // W1t[c][i] = W1[i][c]
+        reinterpret_cast<float*>(cp + Model::TC_B1)[i] = __ldg(w + Model::OFF_B1 + i);
+        reinterpret_cast<float*>(cp + Model::TC_B2)[i] = __ldg(w + Model::OFF_B2 + i);
+        if (i < 2) reinterpret_cast<float*>(cp + Model::TC_B3)[i] = __ldg(w + Model::OFF_B3 + i);
+    }
+    // the tiles are read by the async proxy (wgmma)
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+
+    stage_issue<real, VARIANT, NU>(a, sm);
+    bool staged = false;
+    real beta_run = O::inf(), eta_run = (real)0;
+
+    const int BS = BD / a.tps;
+    const bool roller = half == 0;                     // warp-uniform
+    for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
+        const int k = tile * BS + (tid % BS);
+        const bool in_range = k < a.K;
+        const bool active = in_range && roller;
+        const int nvalid = min(BS, a.K - tile * BS);
+        const unsigned long long kg = (unsigned long long)(a.k_offset + k);
+        fill_normals<real>(a, sm, tile, in_range, kg, nvalid);
+        if (!staged) {
+            stage_finish<real, VARIANT, NU>(a, sm);
+            staged = true;
+        } else {
+            __syncthreads();
+        }
+        if (in_range) transform_column<real, VARIANT, NU>(a, sm, kg);
+        __syncthreads();
+
+        // ---- rollout of the M copies: the MMAs are warpgroup-wide, so every thread keeps the step's two barriers -------
+        // The M states live in the copies' layer-1 input rows (TC_X), which only the sample's roller writes: x(m) is its
+        // copy-m state, read and updated there after the step's second barrier.
+        auto xrow = [&](int m) -> float2& { return reinterpret_cast<float2*>(ens + m * Model::TC_COPY + Model::TC_X)[row]; };
+        if (roller) {
+            real x0 = (real)0, x1 = (real)0;
+            if (active) {
+                if (a.state_dev != nullptr) {
+                    const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
+                    x0 = sp[0];
+                    x1 = sp[1];
+                } else {
+                    x0 = a.x0[0];
+                    x1 = a.x0[1];
+                }
+            }
+#pragma unroll
+            for (int m = 0; m < MC; ++m)
+                if (m < M) xrow(m) = make_float2(x0, x1);
+        }
+        real cs[MC];
+#pragma unroll
+        for (int m = 0; m < MC; ++m) cs[m] = (real)0;
+        real var = (real)0, pert = (real)0, smooth = (real)0, vprev = (real)0, u_prev = (real)0;
+        for (int t = 0; t < T; ++t) {
+            real v[NU] = {(real)0}, eps[NU] = {(real)0};
+            real u = (real)0;
+            if (roller) {
+                if (active) {
+                    action_at<real, VARIANT, NU>(a, sm, kg, t, v);
+                    noise_at<real, VARIANT, NU>(a, sm, t, v, eps);
+                }
+                u = O::mul(nm.u_scale, v[0]);
+                sU[row] = clamp<real>(u, -mp.max_torque, mp.max_torque);
+            }
+            __syncthreads();
+            // the running costs of the states the PREVIOUS step produced (x_t)
+            if (active) {
+                if (t > 0) {
+                    real c[MC];
+#pragma unroll
+                    for (int m = 0; m < MC; ++m) {
+                        const float2 xm = xrow(m < M ? m : 0);
+                        const real xv[NX] = {xm.x, xm.y};
+                        c[m] = m < M ? Model::template cost<real>(mp, xv, &u_prev, m) : (real)0;
+                    }
+                    copies_fold<real, MC>(cs, var, c, __ldg(a.var_disc + t - 1), M);      // mppi.py:362-364 (step t-1)
+                }
+                pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
+                if (VARIANT == V_SMPPI) {
+                    if (t > 0) {
+                        const real d = O::mul(nm.u_scale, O::sub(v[0], vprev));
+                        smooth = O::add(smooth, O::mul(d, d));
+                    }
+                    vprev = v[0];
+                }
+            }
+            u_prev = u;
+            const float ua = sU[r0], ub = sU[r1];
+#pragma unroll 1
+            for (int m = 0; m < M; ++m) {
+                unsigned char* cp = ens + m * Model::TC_COPY;
+                const float* w1 = reinterpret_cast<const float*>(cp + Model::TC_W1);
+                const float* b1 = reinterpret_cast<const float*>(cp + Model::TC_B1);
+                const float* b2 = reinterpret_cast<const float*>(cp + Model::TC_B2);
+                const float* b3 = reinterpret_cast<const float*>(cp + Model::TC_B3);
+                uint32_t ahi[2][4], alo[2][4];
+                float h[16];
+                {   // layer 1 on the FP32 pipe (exact fp32): rows r0, r1 x columns 8j + 2t, +1 -> tanh -> layer 2's A fragments
+                    const float2 xa = reinterpret_cast<const float2*>(cp + Model::TC_X)[r0];
+                    const float2 xb = reinterpret_cast<const float2*>(cp + Model::TC_X)[r1];
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const int c = 8 * j + 2 * t4;
+                        const float2 w0 = *reinterpret_cast<const float2*>(w1 + 0 * H + c);
+                        const float2 w1v = *reinterpret_cast<const float2*>(w1 + 1 * H + c);
+                        const float2 w2 = *reinterpret_cast<const float2*>(w1 + 2 * H + c);
+                        const float2 bb = *reinterpret_cast<const float2*>(b1 + c);
+                        h[4 * j + 0] = fmaf(w2.x, ua, fmaf(w1v.x, xa.y, fmaf(w0.x, xa.x, bb.x)));
+                        h[4 * j + 1] = fmaf(w2.y, ua, fmaf(w1v.y, xa.y, fmaf(w0.y, xa.x, bb.y)));
+                        h[4 * j + 2] = fmaf(w2.x, ub, fmaf(w1v.x, xb.y, fmaf(w0.x, xb.x, bb.x)));
+                        h[4 * j + 3] = fmaf(w2.y, ub, fmaf(w1v.y, xb.y, fmaf(w0.y, xb.x, bb.y)));
+                    }
+#pragma unroll
+                    for (int i = 0; i < 16; i += 4) PendulumMLPModel::tanh4_(h + i, FAST);
+                    tc::to_operand<SPLIT>(h, ahi, alo);
+                }
+                // layer 2: accumulators start at the bias
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const float2 bb = *reinterpret_cast<const float2*>(b2 + 8 * j + 2 * t4);
+                    h[4 * j + 0] = h[4 * j + 2] = bb.x;
+                    h[4 * j + 1] = h[4 * j + 3] = bb.y;
+                }
+                const uint64_t dW2 = tc::smem_desc(cp + Model::TC_W2), dW2lo = tc::smem_desc(cp + Model::TC_W2LO);
+                tc::fence_regs(h);
+                tc::wgmma_fence();
+#pragma unroll
+                for (int s = 0; s < 2; ++s) {
+                    tc::wgmma_n32(h, ahi[s], dW2 + s * tc::KSTEP);
+                    if (SPLIT) {
+                        tc::wgmma_n32(h, alo[s], dW2 + s * tc::KSTEP);
+                        tc::wgmma_n32(h, ahi[s], dW2lo + s * tc::KSTEP);
+                    }
+                }
+                tc::wgmma_commit();
+                tc::wgmma_wait();
+                tc::fence_regs(h);
+                // layer 2 -> tanh -> layer 3's A fragments (the accumulator fragment, repacked in place)
+#pragma unroll
+                for (int i = 0; i < 16; i += 4) PendulumMLPModel::tanh4_(h + i, FAST);
+                tc::to_operand<SPLIT>(h, ahi, alo);
+                const float b30 = t4 == 0 ? b3[0] : 0.0f, b31 = t4 == 0 ? b3[1] : 0.0f;
+                float o[4] = {b30, b31, b30, b31};
+                const uint64_t dW3 = tc::smem_desc(cp + Model::TC_W3), dW3lo = tc::smem_desc(cp + Model::TC_W3LO);
+                tc::fence_regs(o);
+                tc::wgmma_fence();
+#pragma unroll
+                for (int s = 0; s < 2; ++s) {
+                    tc::wgmma_n8(o, ahi[s], dW3 + s * tc::KSTEP);
+                    if (SPLIT) {
+                        tc::wgmma_n8(o, alo[s], dW3 + s * tc::KSTEP);
+                        tc::wgmma_n8(o, ahi[s], dW3lo + s * tc::KSTEP);
+                    }
+                }
+                tc::wgmma_commit();
+                tc::wgmma_wait();
+                tc::fence_regs(o);
+                if (t4 == 0) {
+                    float2* so = reinterpret_cast<float2*>(cp + Model::TC_O);
+                    so[r0] = make_float2(o[0], o[1]);
+                    so[r1] = make_float2(o[2], o[3]);
+                }
+            }
+            __syncthreads();
+            if (roller) {
+#pragma unroll
+                for (int m = 0; m < MC; ++m) {
+                    if (m < M) {
+                        const float2 d = reinterpret_cast<const float2*>(ens + m * Model::TC_COPY + Model::TC_O)[row];
+                        float2& xm = xrow(m);
+                        const real th = O::add(xm.x, d.x);
+                        xm = make_float2(O::sub(remainder<real>(O::add(th, mp.pi), mp.two_pi), mp.pi),   // pendulum_approximate.py:65
+                                         O::add(xm.y, d.y));
+                    }
+                }
+            }
+        }
+        real c_tot = O::inf();
+        if (active) {
+            real c[MC];
+#pragma unroll
+            for (int m = 0; m < MC; ++m) {
+                const float2 xm = xrow(m < M ? m : 0);
+                const real xv[NX] = {xm.x, xm.y};
+                c[m] = m < M ? Model::template cost<real>(mp, xv, &u_prev, m) : (real)0;
+            }
+            copies_fold<real, MC>(cs, var, c, __ldg(a.var_disc + T - 1), M);              // step T-1
+            real mean = cs[0];
+#pragma unroll
+            for (int m = 1; m < MC; ++m)
+                if (m < M) mean = O::add(mean, cs[m]);
+            mean = O::div(mean, (real)M);                                                  // mppi.py:371
+            c_tot = O::add(O::add(mean, O::mul(var, a.var_cost)), pert);                   // mppi.py:372, 416
+            if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));   // mppi.py:562,569
+            a.cost_total[k] = c_tot;
+        }
+        real w_unused;
+        fold_tile<real, VARIANT, false>(a, sm, c_tot, active, nvalid, beta_run, eta_run, w_unused);
+    }
+    if (!staged) stage_finish<real, VARIANT, NU>(a, sm);
+    publish_and_finish<real, VARIANT, NU>(a, sm, beta_run, eta_run);
+}
+
 #endif  // __CUDACC__
 
 }  // namespace mppi

@@ -5,7 +5,7 @@
 // which the generic host code in mppi_b200.cu (mppi_fused_host.cuh) works on.
 //
 // Compiled several times by pytorch_mppi_b200/build.py:
-//     nvcc ... -DMPPI_TU_MODEL=<1 pendulum | 2 linear point | 3 pendulum MLP> -DMPPI_TU_F64=<0|1> -c
+//     nvcc ... -DMPPI_TU_MODEL=<1 pendulum | 2 linear point | 3 pendulum MLP | 4 pendulum MLP ensemble> -DMPPI_TU_F64=<0|1> -c
 // (user models are compiled at run time with NVRTC and registered with mppi_user_model_register — same kernels, same table).
 #include "mppi_host.cuh"
 #include "mppi_mlp_tc.cuh"
@@ -34,6 +34,9 @@ typedef mppi::LinearPointModel TuModel;
 #elif MPPI_TU_MODEL == 3
 typedef mppi::PendulumMLPModel TuModel;
 #define MPPI_TU_NAME pendulum_mlp
+#elif MPPI_TU_MODEL == 4
+typedef mppi::PendulumMLPEnsembleModel TuModel;
+#define MPPI_TU_NAME pendulum_mlp_ensemble
 #else
 #error "unknown MPPI_TU_MODEL"
 #endif
@@ -45,6 +48,7 @@ typedef mppi::PendulumMLPModel TuModel;
 namespace {
 
 constexpr bool kIsMlp = MPPI_TU_MODEL == 3;
+constexpr bool kIsEnsemble = MPPI_TU_MODEL == 4;   // copies at run time: no split-cost, batched or resident kernels
 typedef TuModel::P<TuReal> TuParams;
 static_assert(sizeof(TuParams) <= MPPI_MODEL_BLOCK_BYTES, "model parameter block too large");
 
@@ -53,11 +57,15 @@ void tu_load(const ModelKernels*, void* dst, const double* blob, const double* e
 }
 
 template <int V> const void* split_kernel() {
-    if constexpr (kIsMlp) return nullptr;                     // its step is the network; the cost is nothing
+    if constexpr (kIsMlp || kIsEnsemble) return nullptr;      // its step is the network; the cost is nothing
     else return (const void*)fused_command_kernel<TuModel, TuReal, V, false, true>;
 }
+const void* batched_kernel() {
+    if constexpr (kIsEnsemble) return nullptr;                // MPPI_Batched has no rollout_samples
+    else return (const void*)fused_command_kernel<TuModel, TuReal, V_MPPI, true>;
+}
 template <int V> const void* resident_kernel() {
-    if constexpr (kIsMlp) return nullptr;
+    if constexpr (kIsMlp || kIsEnsemble) return nullptr;
     else return (const void*)resident_command_kernel<TuModel, TuReal, V>;
 }
 const void* stamped_resident_kernel() {
@@ -66,15 +74,16 @@ const void* stamped_resident_kernel() {
 }
 template <int V, int SPLIT, int FAST> const void* tc_kernel() {
     if constexpr (kIsMlp && !MPPI_TU_F64) return (const void*)mlp_tc_command_kernel<V, SPLIT, FAST>;
+    else if constexpr (kIsEnsemble && !MPPI_TU_F64) return (const void*)mlp_ens_tc_command_kernel<V, SPLIT, FAST>;
     else return nullptr;
 }
 
 const ModelKernels g_kernels = {
-    TuModel::NX, TuModel::NU, MPPI_TU_F64, kIsMlp ? 1 : 0, 0, (int)sizeof(TuParams), tu_load,
+    TuModel::NX, TuModel::NU, MPPI_TU_F64, kIsMlp ? 1 : (kIsEnsemble ? 2 : 0), 0, (int)sizeof(TuParams), tu_load,
     {(const void*)fused_command_kernel<TuModel, TuReal, V_MPPI, false>, (const void*)fused_command_kernel<TuModel, TuReal, V_SMPPI, false>,
      (const void*)fused_command_kernel<TuModel, TuReal, V_KMPPI, false>},
     {split_kernel<V_MPPI>(), split_kernel<V_SMPPI>(), split_kernel<V_KMPPI>()},
-    (const void*)fused_command_kernel<TuModel, TuReal, V_MPPI, true>,
+    batched_kernel(),
     {resident_kernel<V_MPPI>(), resident_kernel<V_SMPPI>(), resident_kernel<V_KMPPI>()},
     stamped_resident_kernel(),
     (const void*)states_kernel<TuModel, TuReal>,

@@ -184,24 +184,34 @@ class PendulumMLP(AnalyticModel):
     H = 32
 
     def __init__(self, net: torch.nn.Sequential, max_torque=2.0, w_thdot=0.1, fast_tanh=False, tensor_cores="auto"):
+        self.check_net(net)
+        self.net = net
+        self.max_torque, self.w_thdot, self.fast_tanh = float(max_torque), float(w_thdot), bool(fast_tanh)
+        self.tensor_cores = self.tensor_core_mode(tensor_cores)
+
+    @classmethod
+    def check_net(cls, net):
+        """Raise ValueError unless `net` is the network the kernels compile: Linear(3,32)-Tanh-Linear(32,32)-Tanh-Linear(32,2)."""
         lin = [m for m in net if isinstance(m, torch.nn.Linear)]
         act = [m for m in net if not isinstance(m, torch.nn.Linear)]
         shapes = [tuple(l.weight.shape) for l in lin]
-        if shapes != [(self.H, 3), (self.H, self.H), (2, self.H)] or not all(isinstance(a, torch.nn.Tanh) for a in act):
+        if shapes != [(cls.H, 3), (cls.H, cls.H), (2, cls.H)] or not all(isinstance(a, torch.nn.Tanh) for a in act):
             raise ValueError("PendulumMLP expects Linear(3,32)-Tanh-Linear(32,32)-Tanh-Linear(32,2); got " + str(shapes))
-        self.net = net
-        self.max_torque, self.w_thdot, self.fast_tanh = float(max_torque), float(w_thdot), bool(fast_tanh)
-        # tensor_cores (fp32 controllers only): the hidden and output layers run as wgmma MMAs with fp32 accumulators
-        # (csrc/mppi_mlp_tc.cuh).  True / "bf16x3": operands are hi/lo-split bf16, layer outputs agree with the
-        # fp32 FFMA kernel to ~1e-5 relative.  "bf16": plain bf16 operands for the two hidden-layer products
-        # (~2^-8 relative; the state inputs stay split), the fastest route.
-        # "auto" (default): "bf16x3" wherever the tensor-core kernel exists (fp32 controllers, one environment), the FFMA
-        # kernel elsewhere (fp64, MPPI_Batched); False pins the FFMA kernel.
+
+    @staticmethod
+    def tensor_core_mode(tensor_cores):
+        """model_params[3] of a `tensor_cores` argument.
+        tensor_cores (fp32 controllers only): the hidden and output layers run as wgmma MMAs with fp32 accumulators
+        (csrc/mppi_mlp_tc.cuh).  True / "bf16x3": operands are hi/lo-split bf16, layer outputs agree with the
+        fp32 FFMA kernel to ~1e-5 relative.  "bf16": plain bf16 operands for the two hidden-layer products
+        (~2^-8 relative; the state inputs stay split), the fastest route.
+        "auto" (default): "bf16x3" wherever the tensor-core kernel exists (fp32 controllers, one environment), the FFMA
+        kernel elsewhere (fp64, MPPI_Batched); False pins the FFMA kernel."""
         if not any(tensor_cores is v or tensor_cores == v for v in (False, True, None, "auto", "bf16x3", "bf16")):
             raise ValueError("tensor_cores must be 'auto', False, True, 'bf16x3' or 'bf16'")
         if tensor_cores is True:
             tensor_cores = "bf16x3"
-        self.tensor_cores = {False: 0, None: 0, "bf16x3": 1, "bf16": 2, "auto": 3}[tensor_cores]
+        return {False: 0, None: 0, "bf16x3": 1, "bf16": 2, "auto": 3}[tensor_cores]
 
     def param_blob(self):
         return [self.max_torque, self.w_thdot, 1.0 if self.fast_tanh else 0.0, float(self.tensor_cores)]
@@ -215,15 +225,69 @@ class PendulumMLP(AnalyticModel):
                     out += m.bias.detach().double().cpu().reshape(-1).tolist()
         return out
 
-    def dynamics(self, state, action):
+    @staticmethod
+    def net_step(net, state, action, max_torque):
+        """x' = x + net([x, clamp(u)]), angle wrapped (pendulum_approximate.py:60-67)."""
         with torch.no_grad():
-            u = torch.clamp(action[:, 0:1], -self.max_torque, self.max_torque)
-            nxt = state + self.net(torch.cat((state, u), dim=1))
+            u = torch.clamp(action[:, 0:1], -max_torque, max_torque)
+            nxt = state + net(torch.cat((state, u), dim=1))
             th = Pendulum.angle_normalize(nxt[:, 0])
             return torch.stack((th, nxt[:, 1]), dim=1)
 
+    def dynamics(self, state, action):
+        return self.net_step(self.net, state, action, self.max_torque)
+
     def running_cost(self, state, action):
         return Pendulum.angle_normalize(state[:, 0]) ** 2 + self.w_thdot * state[:, 1] ** 2
+
+
+class PendulumMLPEnsemble(AnalyticModel):
+    """A bootstrapped ensemble of learned pendulum dynamics (PETS-style model uncertainty): M = len(nets) networks of
+    `PendulumMLP`'s shape (2 <= M <= MPPI_MAX_COPIES), one per rollout copy.  Build the controller with
+    ``rollout_samples=M``: every sample's action sequence is rolled out through each network, and its cost is the mean
+    over the networks plus ``rollout_var_cost * sum_t rollout_var_discount**t * var_m(c_{m,t})`` (mppi.py:334-373).
+    MPPI / SMPPI / KMPPI (also sharded) without a SpecificActionSampler then run the fused kernel; resident mode and
+    MPPI_Batched are not available.  `fast_tanh` and `tensor_cores` mean what they mean for `PendulumMLP`.
+
+    The torch callables are called as the reference calls an M-copy rollout: `dynamics` gets M*K rows, copy-major, and
+    sends block m of M equal blocks through ``nets[m]`` (a row count that is not a multiple of M raises ValueError);
+    `running_cost` is PendulumMLP's; there is no terminal cost.  `get_rollouts` on the fused route runs ``nets[0]``.
+    The controller copies the weights to a device table when it packs its constants: call ``refresh()`` on it after
+    retraining the networks.
+    """
+    model_id = _cabi.MODEL_PENDULUM_MLP_ENSEMBLE
+    nx, nu = 2, 1
+
+    def __init__(self, nets, max_torque=2.0, w_thdot=0.1, fast_tanh=False, tensor_cores="auto"):
+        nets = list(nets)
+        if not 2 <= len(nets) <= _cabi.MPPI_MAX_COPIES:
+            raise ValueError(f"an ensemble takes 2..{_cabi.MPPI_MAX_COPIES} networks, got {len(nets)}")
+        for net in nets:
+            PendulumMLP.check_net(net)
+        self.nets = nets
+        self.copies = len(nets)
+        self.max_torque, self.w_thdot, self.fast_tanh = float(max_torque), float(w_thdot), bool(fast_tanh)
+        self.tensor_cores = PendulumMLP.tensor_core_mode(tensor_cores)
+
+    param_blob = PendulumMLP.param_blob
+
+    def weight_table(self, device, dtype):
+        """(M, 1250) tensor of the networks' weights on `device` in `dtype`, row m in PyTorch Linear order
+        (W1, b1, W2, b2, W3, b3): MppiFusedParams.model_weights."""
+        with torch.no_grad():
+            return torch.stack([torch.cat([p.detach().to(device=device, dtype=dtype).reshape(-1)
+                                           for m in net if isinstance(m, torch.nn.Linear) for p in (m.weight, m.bias)])
+                                for net in self.nets]).contiguous()
+
+    def dynamics(self, state, action):
+        n, M = state.shape[0], self.copies
+        if n % M:
+            raise ValueError(f"an ensemble of {M} networks steps M*K rows (copy-major); got {n} rows")
+        K = n // M
+        return torch.cat([PendulumMLP.net_step(net, state[m * K:(m + 1) * K], action[m * K:(m + 1) * K], self.max_torque)
+                          for m, net in enumerate(self.nets)])
+
+    running_cost = PendulumMLP.running_cost
 
 
 class CudaModel(AnalyticModel):

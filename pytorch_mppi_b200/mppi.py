@@ -7,7 +7,7 @@ Two execution routes, chosen at construction:
            model (pytorch_mppi_b200.models): ONE kernel launch per ``command()`` does sampling,
            rollout, softmin and the nominal update (csrc/mppi_fused.cuh `fused_command_kernel`).
            A step-dependent CudaModel takes this route with ``step_dependent_dynamics=True``, a CudaModel compiled
-           with ``copies=M`` with ``rollout_samples=M``.
+           with ``copies=M`` or a PendulumMLPEnsemble of M networks with ``rollout_samples=M``.
 * stepped — arbitrary Python callables (a torch MLP, plain step-dependent functions, M>1 rollouts of other models, a
            SpecificActionSampler): the T-loop stays in Python exactly like mppi.py:312-322, with the
            sampling (`mppi_sample_perturb`), cost accumulation (`mppi_cost_accumulate`) and softmin
@@ -425,6 +425,11 @@ class MPPI:
         p.rollout_samples = self.M if self._model is not None else 0
         p.rollout_var_cost = float(self.rollout_var_cost)
         p.var_discount = None if self._var_disc is None else self._var_disc.data_ptr()
+        # an ensemble of networks (PendulumMLPEnsemble): its (M, 1250) weight table on this device, read by every command
+        self._model_weights = None
+        if self._model is not None and hasattr(self._model, "weight_table"):
+            self._model_weights = self._model.weight_table(self.d, self.dtype)
+        p.model_weights = None if self._model_weights is None else self._model_weights.data_ptr()
         self._ext_arr = self._fill_model_params(p)
         self._model_version = self._model._param_version if self._model is not None else 0
         self._base_flags = ((_cabi.FLAG_NULL_ACTION if self.sample_null_action else 0)
