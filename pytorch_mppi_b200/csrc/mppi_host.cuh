@@ -388,7 +388,10 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         // latency hiding needs ~24 resident warps per SM when the problem is large enough to supply them
         const long long per_sm = ((long long)p->K + di.sm_count - 1) / di.sm_count;
         const long long want_threads = per_sm < 768 ? per_sm : 768;
-        for (int bs = 64; bs <= 512; bs += (bs < 128 ? 64 : 32)) {     // 64-sample tiles let K < 128 x SMs reach every SM
+        // 64-sample tiles let K < 128 x SMs reach every SM; 32-sample tiles are tried only when no larger tile fits in
+        // shared memory (the R x (BS+1) noise tile of long horizons at nu = 3..4), so no geometry that fits changes
+        auto next_bs = [&](int bs) { return bs == 32 ? 0 : bs < 512 ? bs + (bs < 128 ? 64 : 32) : (best_load < 0 ? 32 : 0); };
+        for (int bs = 64; bs != 0; bs = next_bs(bs)) {
             SmemLayout Lc = make_layout<real>(p->variant, p->T, p->nu, p->S, R, bs, bs, single_partial_grid ? 1 : di.sm_count * 4, need_rows2);
             Lc.total += extra_bytes;
             if (Lc.total > dyn0) continue;
@@ -418,25 +421,33 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
     }
     if (BS % 32 != 0 || BS < 32 || BS > 512) return MPPI_ERR_BAD_ARG;
     const int n_tiles = (p->K + BS - 1) / BS;
+    const int cap = di.sm_count * MPPI_MAX_CTAS_PER_SM;     // workspaces are sized for it: max_planned_grid
+    cudaFuncAttributes fa;
+    CK(cudaFuncGetAttributes(&fa, kernel));
+    const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;   // static + dynamic <= opt-in maximum
+    // The layout depends on the grid (rescale factors of nb partials live in shared memory) and the
+    // grid on the occupancy the layout allows: iterate from an optimistic guess to a fixed point.
+    int nb = n_tiles < cap ? n_tiles : cap;
     if (tps <= 0) {
         // helper threads only pay off while an SM hosts a single small CTA
         tps = 1;
         const int envs = p->n_env > 1 ? p->n_env : 1;
         if ((long long)n_tiles * envs <= di.sm_count) tps = 512 / BS >= 8 ? 8 : (512 / BS >= 4 ? 4 : (512 / BS >= 2 ? 2 : 1));
+        // each helper thread's warp adds per-warp partial rows to the tile: fewer helpers where all of them do not fit
+        // (the optimistic grid's layout is the largest of the fixed-point iteration below)
+        while (tps > 1 && BS * tps > 64 && make_layout<real>(p->variant, p->T, p->nu, p->S, R, BS * tps, BS,
+                                                             single_partial_grid ? 1 : nb, need_rows2).total + extra_bytes > dyn_limit)
+            tps >>= 1;
     }
     while (tps > 1 && BS * tps > 512) tps >>= 1;
+    // at least two warps per CTA: the fused command's record combines (combine_records / combine_global) split the
+    // threads into groups of 64 columns, and a one-warp CTA would have none (32-sample tiles run two threads per sample)
+    if (BS * tps < 64) tps = 64 / BS;
     if (tps != 1 && tps != 2 && tps != 4 && tps != 8) return MPPI_ERR_BAD_ARG;
     const int BD = BS * tps;
-    const int cap = di.sm_count * MPPI_MAX_CTAS_PER_SM;     // workspaces are sized for it: max_planned_grid
-    cudaFuncAttributes fa;
-    CK(cudaFuncGetAttributes(&fa, kernel));
-    const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;   // static + dynamic <= opt-in maximum
     // The attribute is a per-kernel LIMIT (setting a smaller value later lowers it), so raise it
     // once to the device maximum; the carve-out actually used follows each launch's request.
     CK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_limit));
-    // The layout depends on the grid (rescale factors of nb partials live in shared memory) and the
-    // grid on the occupancy the layout allows: iterate from an optimistic guess to a fixed point.
-    int nb = n_tiles < cap ? n_tiles : cap;
     int occ = 0;
     SmemLayout L;
     for (int it = 0; it < 4; ++it) {

@@ -178,6 +178,9 @@ def build_problem(case, gold=None):
         model.terminal_cost = None
     elif m["kind"] == "pendulum_mlp":
         model = MlpPendulumModel(load_mlp_net(gold, dt) if gold is not None else make_mlp_net(m["seed"], dt))
+    elif m["kind"] == "shape":
+        from tests.golden.shape_cases import ShapeTwin
+        model = ShapeTwin(m)
     else:
         model = orc.LinearPointModel(B=m["B"], goal=m["goal"], Q=m.get("Q"), R=m.get("R"),
                                      hills=[tuple(h) for h in m.get("hills", [])],

@@ -15,6 +15,9 @@ def make_model(case, gold=None, **model_kw):
         net = (load_mlp_net(gold, dt) if gold is not None else make_mlp_net(m["seed"], dt)).to("cuda")
         model_kw.setdefault("tensor_cores", False)     # the golden tolerance of the fused route is the FFMA kernel's; the
         return eng.PendulumMLP(net, **model_kw)          # tensor-core route is tested with its own (explicit model_kw)
+    if m["kind"] == "shape":
+        from tests.golden.shape_cases import engine_model
+        return engine_model(m)
     return eng.LinearPoint(B=m["B"], goal=m["goal"], Q=m.get("Q"), R=m.get("R"),
                            hills=[tuple(h) for h in m.get("hills", [])], terminal_scale=m.get("terminal_scale", 0.0))
 
@@ -40,7 +43,7 @@ def make_engine(case, U0, device="cuda", route="fused", gold=None, model_kw=None
               u_scale=case.get("u_scale", 1), sample_null_action=case.get("sample_null_action", False),
               noise_abs_cost=case.get("noise_abs_cost", False), terminal_state_cost=term,
               rollout_samples=case.get("rollout_samples", 1), rollout_var_cost=case.get("rollout_var_cost", 0),
-              rollout_var_discount=case.get("rollout_var_discount", 0.95))
+              rollout_var_discount=case.get("rollout_var_discount", 0.95), u_per_command=case.get("u_per_command", 1))
     if case.get("sampler") is not None:
         from tests.golden.cases import sampler_actions
 

@@ -63,7 +63,7 @@ def make_ref_controller(case, prob, model, U_init):
               u_scale=case.get("u_scale", 1), sample_null_action=case.get("sample_null_action", False),
               noise_abs_cost=case.get("noise_abs_cost", False), terminal_state_cost=term,
               rollout_samples=case.get("rollout_samples", 1), rollout_var_cost=case.get("rollout_var_cost", 0),
-              rollout_var_discount=case.get("rollout_var_discount", 0.95))
+              rollout_var_discount=case.get("rollout_var_discount", 0.95), u_per_command=case.get("u_per_command", 1))
     if case.get("sampler") is not None:
         class Sampler(ref.SpecificActionSampler):                       # mppi.py:16-32
             def sample_trajectories(self, state, info):
@@ -148,6 +148,9 @@ def run_case(name, case):
             r = orc.kmppi_command(prob, U, theta, x, z, W, Wshift)
             U, theta = r["U"], r["theta"]
             assert torch.equal(theta, ctrl.theta), f"{name} step {step}: theta mismatch"
+        upc = case.get("u_per_command", 1)
+        if upc > 1:                                    # mppi.py:271-274: the first u_per_command rows
+            r["action"] = r["action_sequence" if variant == "smppi" else "U"][:upc]
         # ---- the pin: oracle == live reference, bit for bit -------------------------------
         assert torch.equal(r["U"], ctrl.U), f"{name} step {step}: U mismatch {(r['U'] - ctrl.U).abs().max()}"
         assert torch.equal(r["cost_total"], ctrl.cost_total), f"{name} step {step}: cost_total mismatch"
@@ -177,7 +180,8 @@ def run_case(name, case):
         if variant == "kmppi":
             out[f"theta_{step}"] = r["theta"].numpy()
         # closed loop on the same model (SURVEY §8d)
-        x = prob.dynamics(x.view(1, -1), (prob.u_scale * r["action"]).view(1, -1)).view(-1)[: prob.nx]
+        a0 = r["action"] if upc == 1 else r["action"][0]
+        x = prob.dynamics(x.view(1, -1), (prob.u_scale * a0).view(1, -1)).view(-1)[: prob.nx]
     out["z_sums"] = np.asarray(zsums)
     out["case_json"] = np.asarray(json.dumps(case))
     return out

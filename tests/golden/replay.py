@@ -68,11 +68,15 @@ class OracleRunner:
         else:
             r = orc.kmppi_command(p, self.U, self.theta, x, z, self.W, self.Wshift)
             self.U, self.theta = r["U"], r["theta"]
+        upc = self.case.get("u_per_command", 1)
+        if upc > 1:                                     # mppi.py:271-274: the first u_per_command rows
+            r["action"] = r["action_sequence" if self.variant == "smppi" else "U"][:upc]
         return r
 
     def advance(self, x, action):
         p = self.prob
-        return p.dynamics(x.view(1, -1), (p.u_scale * action).view(1, -1)).view(-1)[: p.nx]
+        a0 = action if self.case.get("u_per_command", 1) == 1 else action[0]
+        return p.dynamics(x.view(1, -1), (p.u_scale * a0).view(1, -1)).view(-1)[: p.nx]
 
 
 class BatchedOracleRunner:
