@@ -206,7 +206,7 @@ template <typename real, int V, int NU>
 int run_sample(const MppiFusedParams* p, KArgs<real>& a_extra, cudaStream_t stream) {
     auto kernel = sample_kernel<real, V, NU>;
     Geometry g;
-    int rc = plan_geometry<real>(kernel, p, V == V_KMPPI, true, g);
+    int rc = plan_geometry<real>(kernel, p, V == V_KMPPI, false, g);
     if (rc) return rc;
     KArgs<real> a;
     fill_kargs<real>(p, a, g.BS, g.nb, g.tps);
@@ -262,10 +262,12 @@ int run_sample_any(const MppiFusedParams* p, void* pa, void* noise, void* noise_
 template <typename real, int V, int NU>
 int run_softmin(const MppiFusedParams* p, const void* cost, const void* eps, cudaStream_t stream) {
     auto kernel = softmin_update_kernel<real, V, NU>;
+    // the warp-fold tail without clusters, one record per rank: its layout as softmin_update_kernel builds it
+    const int xst = fused_xstage_doubles(sharded_in_kernel(p), p->world, 1, rows_of(p));
     Geometry g;
-    int rc = plan_geometry<real>(kernel, p, 0, false, g);
+    int rc = plan_geometry<real>(kernel, p, layout_extra(0, 0, 1, xst), true, g, p->n_env > 1 ? (int)sizeof(KArgs<real>) : 0);
     if (rc) return rc;
-    const uint64_t need_ws = ws_bytes(g.nb, rows_of(p), (int)sizeof(real));
+    const uint64_t need_ws = ws_bytes(g.nb, rows_of(p));
     if (p->workspace == nullptr || p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
     if (p->n_env > 1 && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env)) return MPPI_ERR_WORKSPACE;
     KArgs<real> a;
@@ -350,7 +352,7 @@ int mppi_fused_query(const MppiFusedParams* p, MppiLaunchInfo* out) {
         DevInfo di;
         if ((rc = get_dev_info(di)) != MPPI_OK) return rc;
         out->sm_count = di.sm_count;
-        out->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p), p->dtype == MPPI_F64 ? 8 : 4);
+        out->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p));
         return MPPI_OK;
     }
     if ((rc = validate(p, true)) != MPPI_OK) return rc;
@@ -618,10 +620,8 @@ int mppi_apply_partials(const MppiFusedParams* p, const void* partials, void* st
     return MPPI_ERR_BAD_ARG;
 }
 
-// two epoch parities of MPPI_XCHG_PARITY_WORDS flagged 8-byte words: world x records x 2 (R+2) words per command (the
-// fused kernel's record layout), or the stepped route's [source rank][MPPI_XCHG_MAX_WORDS] layout — both fit
+// two epoch parities of MPPI_XCHG_PARITY_WORDS flagged 8-byte words: world x records x 2 (R+2) words per command
 uint64_t mppi_xchg_bytes(void) { return (uint64_t)2 * MPPI_XCHG_PARITY_WORDS * sizeof(unsigned long long); }
-static_assert(MPPI_MAX_RANKS * MPPI_XCHG_MAX_WORDS <= MPPI_XCHG_PARITY_WORDS, "mailbox parity too small for the rank-record layout");
 
 int mppi_xchg_create(void** mailbox, void* ipc_handle_out_64B) {
     if (mailbox == nullptr || ipc_handle_out_64B == nullptr) return MPPI_ERR_BAD_ARG;

@@ -44,7 +44,7 @@ inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedPara
 struct FusedChoice {
     const void* kernel;
     Geometry g;
-    int split, tc;
+    int split;
 };
 
 // the rank records of a command are exchanged with peers inside the kernel (else they stay in this GPU's own mailbox)
@@ -71,17 +71,12 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     if (p->K_geom > p->K) pg.K = p->K_geom;
     Geometry g;
     int rc;
-    if (tc_route) {
-        // the ensemble's kernel keeps every copy's network and step buffers behind the layout
-        const int ens_bytes = mk->is_mlp == 2 ? PendulumMLPEnsembleModel::tc_smem_bytes(p->rollout_samples) : 0;
-        rc = plan_geometry<real>(kernel, &pg, 0, false, g, ens_bytes);
-        if (rc) return rc;
-        c = FusedChoice{kernel, g, 0, 1};
-        return MPPI_OK;
-    }
     const int xst1 = sharded ? world * (R + 2) : 0;          // staging of the rank-record exchange
-    const int tile2 = V != V_MPPI;                          // SMPPI: effective-noise tile, KMPPI: interpolated-trajectory tile
-    rc = plan_geometry<real>(kernel, &pg, layout_extra(tile2, 0, 1, xst1), true, g);
+    // SMPPI: effective-noise tile, KMPPI: interpolated-trajectory tile (the tensor-core kernels have neither)
+    const int tile2 = V != V_MPPI && !tc_route;
+    // the ensemble's tensor-core kernel keeps every copy's network and step buffers behind the layout
+    const int ens_bytes = tc_route && mk->is_mlp == 2 ? PendulumMLPEnsembleModel::tc_smem_bytes(p->rollout_samples) : 0;
+    rc = plan_geometry<real>(kernel, &pg, layout_extra(tile2, 0, 1, xst1), false, g, ens_bytes);
     if (rc) return rc;
     int split = 0;
     if (mk->split[V] != nullptr) {      // (the MLP has none: its step is the network, the cost is nothing)
@@ -92,7 +87,7 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
             p2.threads_per_sample = g.tps;
             p2.grid_blocks = g.nb;
             Geometry g2;
-            if (plan_geometry<real>(k2, &p2, layout_extra(tile2, mk->nx, 1, xst1), true, g2) == MPPI_OK &&
+            if (plan_geometry<real>(k2, &p2, layout_extra(tile2, mk->nx, 1, xst1), false, g2) == MPPI_OK &&
                 g2.BS == g.BS && g2.tps == g.tps) {
                 kernel = k2;
                 g = g2;
@@ -125,30 +120,30 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
         if (const char* e = getenv("MPPI_B200_XCHG_DIRECT"))
             if (atoi(e) == 0) npub = 1;
         const int xst = fused_xstage_doubles(sharded, world, npub, R);
-        const SmemLayout L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, g.BD, g.BS, fused_layout_nb(NC, npub),
-                                               layout_extra(tile2, split ? mk->nx : 0, cs, xst));
-        if (L.total > dyn_limit) continue;
+        const int smem = make_layout<real>(p->variant, p->T, p->nu, p->S, R, g.BD, g.BS, fused_layout_nb(NC, npub),
+                                           layout_extra(tile2, split ? mk->nx : 0, cs, xst)).total + ens_bytes;
+        if (smem > dyn_limit) continue;
         if (cs > 1) {
             cudaLaunchConfig_t cfg;
             cudaLaunchAttribute at[3];
-            launch_config(cfg, at, nbp, g.BD, L.total, nullptr, (p->flags & MPPI_FLAG_PDL) != 0, envs, cs);
+            launch_config(cfg, at, nbp, g.BD, smem, nullptr, (p->flags & MPPI_FLAG_PDL) != 0, envs, cs);
             int max_clusters = 0;
             if (cudaOccupancyMaxActiveClusters(&max_clusters, kernel, &cfg) != cudaSuccess) {
                 cudaGetLastError();
                 continue;
             }
             if (getenv("MPPI_B200_DEBUG_GEOM"))
-                fprintf(stderr, "[mppi_b200] cluster %d: grid %d, smem %d, max active clusters %d (need %d)\n", cs, nbp, L.total, max_clusters, NC * envs);
+                fprintf(stderr, "[mppi_b200] cluster %d: grid %d, smem %d, max active clusters %d (need %d)\n", cs, nbp, smem, max_clusters, NC * envs);
             if (max_clusters < NC * envs) continue;                       // a cluster left for a second wave doubles the time
         }
         g.cluster = cs;
         g.nb = nbp;
-        g.smem = L.total;
+        g.smem = smem;
         g.npub = npub;
         break;
     }
     if (g.cluster == 0) return UNSUPPORTED("shared-memory tile does not fit");
-    c = FusedChoice{kernel, g, split, 0};
+    c = FusedChoice{kernel, g, split};
     return MPPI_OK;
 }
 
@@ -175,7 +170,7 @@ template <typename real> int query_fused(const ModelKernels* mk, const MppiFused
     info->regs_per_thread = g.regs;
     info->max_blocks_per_sm = g.occ;
     info->sm_count = di.sm_count;
-    info->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p), (int)sizeof(real));
+    info->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p));
     info->tma_staging = a.tma_ok;
     info->split_cost = c.split;
     info->cluster_size = g.cluster;
@@ -194,7 +189,7 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
     pl->g = c.g;
     if (p->U == nullptr || p->cost_total == nullptr || p->nominal_used == nullptr || p->stats == nullptr || p->workspace == nullptr)
         return MPPI_ERR_BAD_ARG;
-    const uint64_t need_ws = ws_bytes(pl->g.nb, rows_of(p), (int)sizeof(real));
+    const uint64_t need_ws = ws_bytes(pl->g.nb, rows_of(p));
     if (p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
     if (batched && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env ||
                     p->env_u_stride < p->T * p->nu))

@@ -170,17 +170,12 @@ template <typename real> void fill_noise_model(const MppiFusedParams* p, NoiseMo
     nm.abs_cost = (p->flags & MPPI_FLAG_ABS_COST) ? 1 : 0;
 }
 
-// ticket + per-CTA partials (beta_b, eta_b, V_b[R]) of type `real` (stepped-route / resident / tensor-core tails), or
-// ticket + per-cluster records of (R + 2) doubles (fused kernel's warp-fold tail): the larger of the two
+// ticket + the records of the warp-fold tail's ticket mode: one of (R + 2) doubles per cluster (at most one per CTA)
 // ... followed by this GPU's own record mailbox (single-GPU LL mode): two epoch parities of MPPI_LL_LOCAL_WORDS flagged words
 #define MPPI_LL_STAGE_BYTES 49152                          // finisher staging budget: LL mode needs xw x clusters x (R+2) x 8 <= this
 #define MPPI_LL_LOCAL_WORDS (2 * MPPI_LL_STAGE_BYTES / 8)  // words per parity of the local mailbox (2 words per double)
-inline uint64_t ws_partials_bytes(int nb, int R, int es) {
-    const uint64_t per_cta = 16 + 2 * (uint64_t)align_up(nb * es, 16) + (uint64_t)align_up(nb * R * es, 16);
-    const uint64_t per_cluster = 16 + (uint64_t)nb * (uint64_t)(R + 2) * 8;
-    return ((per_cta > per_cluster ? per_cta : per_cluster) + 255) / 256 * 256;
-}
-inline uint64_t ws_bytes(int nb, int R, int es) { return ws_partials_bytes(nb, R, es) + 2ull * MPPI_LL_LOCAL_WORDS * 8; }
+inline uint64_t ws_partials_bytes(int nb, int R) { return (16 + (uint64_t)nb * (uint64_t)(R + 2) * 8 + 255) / 256 * 256; }
+inline uint64_t ws_bytes(int nb, int R) { return ws_partials_bytes(nb, R) + 2ull * MPPI_LL_LOCAL_WORDS * 8; }
 
 #define MPPI_MAX_CTAS_PER_SM 16                            // plan_geometry's grid cap
 // The largest grid any kernel of these dimensions can be planned with, on any route: tiles hold at least 32 samples, the
@@ -240,9 +235,6 @@ template <typename real> int fill_kargs(const MppiFusedParams* p, KArgs<real>& a
     if (p->workspace != nullptr) {
         unsigned char* w = (unsigned char*)p->workspace;
         a.ticket = (unsigned int*)w;
-        a.betaP = (real*)(w + 16);
-        a.etaP = (real*)(w + 16 + align_up(nb * es, 16));
-        a.VP = (real*)(w + 16 + 2 * align_up(nb * es, 16));
         a.crec = (double*)(w + 16);
     }
     a.xchg_npub = 1;
@@ -275,7 +267,7 @@ template <typename real> int fill_kargs(const MppiFusedParams* p, KArgs<real>& a
     if (!any_peer || a.export_partial) a.world = a.export_partial ? a.world : 1;
     if (p->workspace != nullptr && (a.world == 1 || a.export_partial)) {
         // not sharded in-kernel: the record mailbox is this GPU's own, behind the partials in the workspace
-        a.peers[0] = (unsigned long long*)((unsigned char*)p->workspace + ws_partials_bytes(nb, a.R, es));
+        a.peers[0] = (unsigned long long*)((unsigned char*)p->workspace + ws_partials_bytes(nb, a.R));
         a.xchg_parity_words = MPPI_LL_LOCAL_WORDS;
     }
     return MPPI_OK;
@@ -339,18 +331,20 @@ inline int refuse_capture(cudaStream_t stream, const Geometry& g) {
 
 struct GeomKey {
     const void* kernel;
-    int dev, variant, K, T, nu, S, bt, tp, gb, r2, single, ne, xb;
+    int dev, variant, K, T, nu, S, bt, tp, gb, r2, grid_recs, ne, xb;
     bool operator==(const GeomKey& o) const {
         return kernel == o.kernel && dev == o.dev && variant == o.variant && K == o.K && T == o.T && nu == o.nu && S == o.S &&
-               bt == o.bt && tp == o.tp && gb == o.gb && r2 == o.r2 && single == o.single && ne == o.ne && xb == o.xb;
+               bt == o.bt && tp == o.tp && gb == o.gb && r2 == o.r2 && grid_recs == o.grid_recs && ne == o.ne && xb == o.xb;
     }
 };
 
 // Launch geometry for (kernel, dimensions).  The occupancy / attribute queries cost microseconds, so
 // the last few results are cached per thread: a steady-state command() pays only the lookup.
+// grid_records: the kernel's finisher rescales one record per CTA of the grid (the warp-fold tail in ticket mode without
+// clusters: softmin_update_kernel), so the layout grows with the grid; the fused routes size their final layout themselves.
 // extra_bytes: dynamic shared memory the kernel uses behind the layout (the ensemble wgmma kernel's per-copy tiles).
 template <typename real, typename KernelT>
-int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool single_partial_grid, Geometry& g,
+int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool grid_records, Geometry& g,
                   int extra_bytes = 0) {
     static thread_local GeomKey keys[8];
     static thread_local Geometry vals[8];
@@ -358,7 +352,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
     int dev = 0;
     CK(cudaGetDevice(&dev));
     const GeomKey key{(const void*)kernel, dev, p->variant, p->K, p->T, p->nu, p->S, p->block_threads, p->threads_per_sample,
-                      p->grid_blocks, need_rows2, single_partial_grid ? 1 : 0, p->n_env > 1 ? p->n_env : 1, extra_bytes};
+                      p->grid_blocks, need_rows2, grid_records ? 1 : 0, p->n_env > 1 ? p->n_env : 1, extra_bytes};
     for (int i = 0; i < n_cached; ++i)
         if (keys[i] == key) {
             g = vals[i];
@@ -392,7 +386,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         // shared memory (the R x (BS+1) noise tile of long horizons at nu = 3..4), so no geometry that fits changes
         auto next_bs = [&](int bs) { return bs == 32 ? 0 : bs < 512 ? bs + (bs < 128 ? 64 : 32) : (best_load < 0 ? 32 : 0); };
         for (int bs = 64; bs != 0; bs = next_bs(bs)) {
-            SmemLayout Lc = make_layout<real>(p->variant, p->T, p->nu, p->S, R, bs, bs, single_partial_grid ? 1 : di.sm_count * 4, need_rows2);
+            SmemLayout Lc = make_layout<real>(p->variant, p->T, p->nu, p->S, R, bs, bs, grid_records ? di.sm_count * 4 : 1, need_rows2);
             Lc.total += extra_bytes;
             if (Lc.total > dyn0) continue;
             int occ_c = 0;
@@ -425,7 +419,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
     cudaFuncAttributes fa;
     CK(cudaFuncGetAttributes(&fa, kernel));
     const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;   // static + dynamic <= opt-in maximum
-    // The layout depends on the grid (rescale factors of nb partials live in shared memory) and the
+    // The layout may depend on the grid (grid_records: one rescale factor per CTA in shared memory) and the
     // grid on the occupancy the layout allows: iterate from an optimistic guess to a fixed point.
     int nb = n_tiles < cap ? n_tiles : cap;
     if (tps <= 0) {
@@ -436,7 +430,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         // each helper thread's warp adds per-warp partial rows to the tile: fewer helpers where all of them do not fit
         // (the optimistic grid's layout is the largest of the fixed-point iteration below)
         while (tps > 1 && BS * tps > 64 && make_layout<real>(p->variant, p->T, p->nu, p->S, R, BS * tps, BS,
-                                                             single_partial_grid ? 1 : nb, need_rows2).total + extra_bytes > dyn_limit)
+                                                             grid_records ? nb : 1, need_rows2).total + extra_bytes > dyn_limit)
             tps >>= 1;
     }
     while (tps > 1 && BS * tps > 512) tps >>= 1;
@@ -451,7 +445,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
     int occ = 0;
     SmemLayout L;
     for (int it = 0; it < 4; ++it) {
-        L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
+        L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, grid_records ? nb : 1, need_rows2);
         L.total += extra_bytes;
         if (L.total > dyn_limit) return UNSUPPORTED("shared-memory tile does not fit");
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, BD, L.total));
@@ -463,7 +457,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         if (nb2 == nb) break;
         nb = nb2;
     }
-    L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, single_partial_grid ? 1 : nb, need_rows2);
+    L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, grid_records ? nb : 1, need_rows2);
     L.total += extra_bytes;
     g.BS = BS;
     g.tps = tps;

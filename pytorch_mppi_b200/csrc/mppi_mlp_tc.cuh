@@ -13,7 +13,7 @@
 //     the lane with t = 0 -> shared memory -> the sample's thread, which owns the state, the action and the cost.
 // Two CTA barriers per step: the inputs of layer 1 (x, clamped u of every sample) and the outputs of layer 3.  The
 // running cost of the state a step produced is evaluated one step LATER, in the shadow of the layer-2 MMAs (same
-// values, same summation order).  Everything else (sampling, clamp, cost, softmin fold, last-CTA update) is the code of
+// values, same summation order).  Everything else (sampling, clamp, cost, the warp-fold softmin tail) is the code of
 // mppi_fused.cuh.
 //
 // Precision: operands are bf16.  In the default (SPLIT) mode activations and weights are split into hi + lo bf16
@@ -117,8 +117,14 @@ __global__ void __launch_bounds__(256, 2) mlp_tc_command_kernel(const __grid_con
     // wgmma fragment of this thread: rows r0 = 64 * warpgroup + 16 * (warp % 4) + g and r0 + 8, column pairs 2t (+ 8j)
     const int lane = tid & 31, g = lane >> 2, t4 = lane & 3;
     const int r0 = 64 * half + 16 * ((tid >> 5) & 3) + g, r1 = r0 + 8;
-    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BD / a.tps, gridDim.x, 0);
+    const int BS = BD / a.tps;
+    const int xst = fused_xstage_doubles(a.world > 1 && !a.export_partial, a.world, a.xchg_npub, a.R);
+    const int cs_ = (int)cluster_nctarank();
+    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BS, fused_layout_nb((int)gridDim.x / cs_, a.xchg_npub),
+                                           layout_extra(0, 0, cs_, xst));
     Smem<real> sm(smem, L);
+    warp_records_init<real>(a, sm);      // published by the first barrier of the setup
+    if (cs_ > 1) cluster_arrive_relaxed();   // phase 0 of the cluster barrier, as in fused_command_kernel
     const NoiseModel<real>& nm = a.nm;
     const int T = a.T;
 
@@ -173,11 +179,9 @@ __global__ void __launch_bounds__(256, 2) mlp_tc_command_kernel(const __grid_con
 
     stage_issue<real, VARIANT, NU>(a, sm);
     bool staged = false;
-    real beta_run = O::inf(), eta_run = (real)0;
 
     // Tile = 128 samples; the two threads of a sample share its draws and its colour/clamp pass (a.tps == 2), thread 0
     // of the pair (half 0, warps 0-3) carries the state and the cost.
-    const int BS = BD / a.tps;
     const bool roller = half == 0;                     // warp-uniform
     for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
         const int k = tile * BS + (tid % BS);
@@ -312,11 +316,11 @@ __global__ void __launch_bounds__(256, 2) mlp_tc_command_kernel(const __grid_con
             if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));
             a.cost_total[k] = c_tot;
         }
-        real w_unused;
-        fold_tile<real, VARIANT, false>(a, sm, c_tot, active, nvalid, beta_run, eta_run, w_unused);
+        if (roller) warp_fold<real, VARIANT, false>(a, sm, c_tot, active, nvalid);
+        if (tile + (int)gridDim.x < a.n_tiles) __syncthreads();      // the tile is refilled by the next pass
     }
     if (!staged) stage_finish<real, VARIANT, NU>(a, sm);
-    publish_and_finish<real, VARIANT, NU>(a, sm, beta_run, eta_run);
+    warp_tail<real, VARIANT, NU>(a, sm);
 }
 
 // =================================================================================================
@@ -344,8 +348,14 @@ __global__ void __launch_bounds__(256, 2) mlp_ens_tc_command_kernel(const __grid
     const int row = tid & 127, half = tid >> 7;
     const int lane = tid & 31, g = lane >> 2, t4 = lane & 3;
     const int r0 = 64 * half + 16 * ((tid >> 5) & 3) + g, r1 = r0 + 8;
-    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BD / a.tps, gridDim.x, 0);
+    const int BS = BD / a.tps;
+    const int xst = fused_xstage_doubles(a.world > 1 && !a.export_partial, a.world, a.xchg_npub, a.R);
+    const int cs_ = (int)cluster_nctarank();
+    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BS, fused_layout_nb((int)gridDim.x / cs_, a.xchg_npub),
+                                           layout_extra(0, 0, cs_, xst));
     Smem<real> sm(smem, L);
+    warp_records_init<real>(a, sm);      // published by the first barrier of the setup
+    if (cs_ > 1) cluster_arrive_relaxed();   // phase 0 of the cluster barrier, as in fused_command_kernel
     const NoiseModel<real>& nm = a.nm;
     const int T = a.T, M = mp.M;
     // per-copy blocks behind the layout (the host adds Model::tc_smem_bytes(M) to the launch's dynamic shared memory)
@@ -393,9 +403,7 @@ __global__ void __launch_bounds__(256, 2) mlp_ens_tc_command_kernel(const __grid
 
     stage_issue<real, VARIANT, NU>(a, sm);
     bool staged = false;
-    real beta_run = O::inf(), eta_run = (real)0;
 
-    const int BS = BD / a.tps;
     const bool roller = half == 0;                     // warp-uniform
     for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
         const int k = tile * BS + (tid % BS);
@@ -580,11 +588,11 @@ __global__ void __launch_bounds__(256, 2) mlp_ens_tc_command_kernel(const __grid
             if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));   // mppi.py:562,569
             a.cost_total[k] = c_tot;
         }
-        real w_unused;
-        fold_tile<real, VARIANT, false>(a, sm, c_tot, active, nvalid, beta_run, eta_run, w_unused);
+        if (roller) warp_fold<real, VARIANT, false>(a, sm, c_tot, active, nvalid);
+        if (tile + (int)gridDim.x < a.n_tiles) __syncthreads();      // the tile is refilled by the next pass
     }
     if (!staged) stage_finish<real, VARIANT, NU>(a, sm);
-    publish_and_finish<real, VARIANT, NU>(a, sm, beta_run, eta_run);
+    warp_tail<real, VARIANT, NU>(a, sm);
 }
 
 #endif  // __CUDACC__

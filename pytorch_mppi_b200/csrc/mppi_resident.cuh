@@ -74,7 +74,6 @@ __device__ void stage_resident(const KArgs<real>& a, Smem<real>& sm) {
         sm.Uraw[j] = __ldcg(a.U + j);
         if (VARIANT == V_SMPPI) sm.Araw[j] = __ldcg(a.A + j);
     }
-    for (int j = tid; j < R; j += BD) sm.Vrun[j] = (real)0;
     if (VARIANT == V_KMPPI) {
         for (int j = tid; j < R; j += BD) sm.thraw[j] = __ldcg(a.theta + j);
         for (int j = tid; j < T * S; j += BD) sm.Ws[j] = a.W[j];            // constants of the controller
