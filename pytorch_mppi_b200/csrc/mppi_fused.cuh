@@ -226,6 +226,7 @@ template <typename real> struct Smem {
     real *Uraw, *Araw, *thraw, *Us, *As, *ths, *Ws, *Wsh, *rows, *rows2, *xs;
     double *part2, *numd, *wrec, *xstage, *sqd;
     int LD;
+    Smem() = default;
     __device__ Smem(unsigned char* smem, const SmemLayout& L) {
         bar = reinterpret_cast<unsigned long long*>(smem);
         Uraw = reinterpret_cast<real*>(smem + L.off_uraw);
@@ -1085,6 +1086,227 @@ __device__ void make_env_args(const KArgs<real>& in, KArgs<real>* out) {
     __syncthreads();
 }
 
+// ---- Rollouts of models with a fast range (FastRange, mppi_math.cuh).  Every thread of a sample checks
+// in_fast_range on x_0; when it holds, the sample's rollout runs on the model's fast step and cost, inlined; when it
+// does not (a start far out, or a non-finite one), on the exact forms, out of line.  Models without a fast range keep
+// the rollouts below these (split_cost_rollout's own body and the kernel's single loop) as they are.
+
+// the rollout thread's state at t = 0 (mppi.py:303-305): the controller's state, or the sample's own (state_per_sample)
+template <typename real, int NX>
+__device__ __forceinline__ void initial_state(const KArgs<real>& a, int k, real* x) {
+    if (a.state_dev != nullptr) {
+        const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
+#pragma unroll
+        for (int i = 0; i < NX; ++i) x[i] = sp[i];
+    } else {
+#pragma unroll
+        for (int i = 0; i < NX; ++i) x[i] = a.x0[i];
+    }
+}
+
+// what a sample's rollout loop carries from step to step besides its actions: the state, the running-cost sum (single
+// loop only), the action cost and the SMPPI smoothness cost
+template <typename real, int NX> struct RolloutCarry {
+    real x[NX];
+    real roll, pert, smooth;
+};
+
+// the recurrence of the split-cost rollout on the sample's rollout thread: every x_t to the sample's column of xs, the
+// action cost (and SMPPI smoothness) accumulated alongside.  FAST: the model's fast step.
+template <class Model, typename real, int VARIANT, bool FAST>
+__device__ __forceinline__ void split_recurrence(const KArgs<real>& a, const typename Model::template P<real>& mp, const Smem<real>& sm,
+                                                 unsigned long long kg, real* xcol, RolloutCarry<real, Model::NX>& c) {
+    typedef Ops<real> O;
+    constexpr int NX = Model::NX, NU = Model::NU;
+    const NoiseModel<real>& nm = a.nm;
+    const int BS = blockDim.x / a.tps, T = a.T;
+    real vprev[NU];
+#pragma unroll
+    for (int n = 0; n < NU; ++n) vprev[n] = (real)0;
+MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
+    for (int t = 0; t < T; ++t) {
+        real v[NU], u[NU], eps[NU];
+        action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
+        noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
+#pragma unroll
+        for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
+        model_step<Model, real, FAST>(mp, c.x, u, t);                             // mppi.py:314
+#pragma unroll
+        for (int i = 0; i < NX; ++i) xcol[(t * NX + i) * BS] = c.x[i];
+        c.pert = O::add(c.pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
+        if (VARIANT == V_SMPPI) {
+            if (t > 0) {
+#pragma unroll
+                for (int n = 0; n < NU; ++n) {
+                    const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
+                    c.smooth = O::add(c.smooth, O::mul(d, d));
+                }
+            }
+#pragma unroll
+            for (int n = 0; n < NU; ++n) vprev[n] = v[n];
+        }
+    }
+}
+
+// The tiles a rollout reads (the first, the second and the nominal sequence), for the out-of-line rollouts: passing the
+// whole Smem would keep all of its pointers live in the caller up to the call.
+template <typename real> struct RolloutTiles {
+    real *rows, *rows2, *Us;
+    int LD;
+    __device__ __forceinline__ RolloutTiles(const Smem<real>& sm) : rows(sm.rows), rows2(sm.rows2), Us(sm.Us), LD(sm.LD) {}
+    __device__ __forceinline__ Smem<real> smem() const {
+        Smem<real> sm;
+        sm.rows = rows;
+        sm.rows2 = rows2;
+        sm.Us = Us;
+        sm.LD = LD;
+        return sm;
+    }
+};
+
+// split_recurrence on the exact step, out of line (DESIGN §4.2 item 4: the straight path stays compact on a cold
+// instruction cache).  The carry goes in and out by value, so that the inlined fast path keeps it in registers.
+template <class Model, typename real, int VARIANT>
+__device__ __noinline__ RolloutCarry<real, Model::NX> split_recurrence_rare(const KArgs<real>& a, const typename Model::template P<real>& mp,
+                                                                            const RolloutTiles<real> tiles, unsigned long long kg, real* xcol,
+                                                                            RolloutCarry<real, Model::NX> c) {
+    split_recurrence<Model, real, VARIANT, false>(a, mp, tiles.smem(), kg, xcol, c);
+    return c;
+}
+
+// the T running costs of a split-cost rollout, spread over the sample's tps threads: cost_t overwrites x_t[0] in xs
+template <class Model, typename real, int VARIANT, bool FAST>
+__device__ __forceinline__ void split_costs(const KArgs<real>& a, const typename Model::template P<real>& mp, const Smem<real>& sm,
+                                            unsigned long long kg, real* xcol) {
+    typedef Ops<real> O;
+    constexpr int NX = Model::NX, NU = Model::NU;
+    const int tid = threadIdx.x, BS = blockDim.x / a.tps, T = a.T;
+MPPI_UNROLL_N(2)
+    for (int t = tid / BS; t < T; t += a.tps) {      // independent across t: two in flight per thread
+        real v[NU], u[NU], xt[NX];
+        action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
+#pragma unroll
+        for (int n = 0; n < NU; ++n) u[n] = O::mul(a.nm.u_scale, v[n]);
+#pragma unroll
+        for (int i = 0; i < NX; ++i) xt[i] = xcol[(t * NX + i) * BS];
+        xcol[(t * NX) * BS] = model_cost<Model, real, FAST>(mp, xt, u, t);      // mppi.py:318
+    }
+}
+
+// split_cost_rollout of a model with a fast range
+template <class Model, typename real, int VARIANT>
+__device__ __forceinline__ real split_cost_rollout_fast(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
+                                                        int k, unsigned long long kg, bool in_range, bool active) {
+    typedef Ops<real> O;
+    constexpr int NX = Model::NX;
+    const int tid = threadIdx.x, BS = blockDim.x / a.tps, T = a.T;
+    real c_tot = O::inf();
+    real* xcol = sm.xs + (tid % BS);
+    RolloutCarry<real, NX> c;
+    c.pert = (real)0;
+    c.smooth = (real)0;
+    bool fast = false;
+    if (in_range) {
+        initial_state<real, NX>(a, k, c.x);
+        fast = Model::template in_fast_range<real>(mp, c.x, T);
+    }
+    if (active) {
+        if (fast) split_recurrence<Model, real, VARIANT, true>(a, mp, sm, kg, xcol, c);
+        else c = split_recurrence_rare<Model, real, VARIANT>(a, mp, RolloutTiles<real>(sm), kg, xcol, c);
+    }
+    __syncthreads();
+    if (in_range) {
+        if (fast) split_costs<Model, real, VARIANT, true>(a, mp, sm, kg, xcol);
+        else split_costs<Model, real, VARIANT, false>(a, mp, sm, kg, xcol);
+    }
+    __syncthreads();
+    if (active) {
+        real roll = (real)0;
+        for (int t = 0; t < T; ++t) roll = O::add(roll, xcol[(t * NX) * BS]);         // mppi.py:319, t = 0..T-1
+        if (Model::template has_terminal<real>(mp)) roll = O::add(roll, Model::template terminal<real>(mp, c.x));
+        c_tot = O::add(roll, c.pert);                                                 // mppi.py:416
+        if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(c.smooth, a.nm.w_smooth));  // mppi.py:562,569
+        a.cost_total[k] = c_tot;
+    }
+    return c_tot;
+}
+
+// the single-loop rollout (the kernel's stage C) on the sample's rollout thread: dynamics, running cost, action cost
+// (and SMPPI smoothness) per step, as the kernel's own loop.  FAST: the model's fast step and cost.
+template <class Model, typename real, int VARIANT, bool FAST>
+__device__ __forceinline__ void single_loop(const KArgs<real>& a, const typename Model::template P<real>& mp, const Smem<real>& sm,
+                                            unsigned long long kg, RolloutCarry<real, Model::NX>& c) {
+    typedef Ops<real> O;
+    constexpr int NX = Model::NX, NU = Model::NU;
+    const NoiseModel<real>& nm = a.nm;
+    const int T = a.T;
+    real vprev[NU], uprev[NU];
+#pragma unroll
+    for (int n = 0; n < NU; ++n) { vprev[n] = (real)0; uprev[n] = (real)0; }
+MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
+    for (int t = 0; t < T; ++t) {
+        real v[NU], u[NU], eps[NU], xs[NX];
+        action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
+        noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
+#pragma unroll
+        for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
+#pragma unroll
+        for (int i = 0; i < NX; ++i) xs[i] = c.x[i];
+#if MPPI_ROLLOUT_PIPELINED
+        model_step<Model, real, FAST>(mp, c.x, u, t);                             // mppi.py:314
+        if (t > 0) c.roll = O::add(c.roll, model_cost<Model, real, FAST>(mp, xs, uprev, t - 1));   // mppi.py:318-319 (step t-1)
+#else
+        model_step<Model, real, FAST>(mp, c.x, u, t);                             // mppi.py:314
+        c.roll = O::add(c.roll, model_cost<Model, real, FAST>(mp, c.x, u, t));    // mppi.py:318-319
+#endif
+        c.pert = O::add(c.pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
+        if (VARIANT == V_SMPPI) {
+            if (t > 0) {
+#pragma unroll
+                for (int n = 0; n < NU; ++n) {
+                    const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
+                    c.smooth = O::add(c.smooth, O::mul(d, d));
+                }
+            }
+#pragma unroll
+            for (int n = 0; n < NU; ++n) vprev[n] = v[n];
+        }
+#pragma unroll
+        for (int n = 0; n < NU; ++n) uprev[n] = u[n];
+    }
+#if MPPI_ROLLOUT_PIPELINED
+    c.roll = O::add(c.roll, model_cost<Model, real, FAST>(mp, c.x, uprev, T - 1));  // step T-1
+#endif
+}
+
+// single_loop on the exact step and cost, out of line (as split_recurrence_rare)
+template <class Model, typename real, int VARIANT>
+__device__ __noinline__ RolloutCarry<real, Model::NX> single_loop_rare(const KArgs<real>& a, const typename Model::template P<real>& mp,
+                                                                       const RolloutTiles<real> tiles, unsigned long long kg,
+                                                                       RolloutCarry<real, Model::NX> c) {
+    single_loop<Model, real, VARIANT, false>(a, mp, tiles.smem(), kg, c);
+    return c;
+}
+
+// the single-loop rollout of a model with a fast range: stores cost_total[k] and returns it
+template <class Model, typename real, int VARIANT>
+__device__ __forceinline__ real single_loop_rollout_fast(const KArgs<real>& a, const typename Model::template P<real>& mp,
+                                                         const Smem<real>& sm, int k, unsigned long long kg) {
+    typedef Ops<real> O;
+    RolloutCarry<real, Model::NX> c;
+    initial_state<real, Model::NX>(a, k, c.x);
+    c.roll = (real)0;
+    c.pert = (real)0;
+    c.smooth = (real)0;
+    if (Model::template in_fast_range<real>(mp, c.x, a.T)) single_loop<Model, real, VARIANT, true>(a, mp, sm, kg, c);
+    else c = single_loop_rare<Model, real, VARIANT>(a, mp, RolloutTiles<real>(sm), kg, c);
+    if (Model::template has_terminal<real>(mp)) c.roll = O::add(c.roll, Model::template terminal<real>(mp, c.x));
+    real c_tot = O::add(c.roll, c.pert);                                              // mppi.py:416
+    if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(c.smooth, a.nm.w_smooth));  // mppi.py:562,569
+    a.cost_total[k] = c_tot;
+    return c_tot;
+}
+
 // ---- stage C', split-cost rollout as a function: recurrence on the rollout thread | running costs on all tps
 // threads of the sample | ordered sum.  Returns the sample's total cost on its rollout thread (+inf elsewhere) and
 // stores it to cost_total[k].  Contains two CTA barriers: every thread must call it.
@@ -1093,73 +1315,76 @@ template <class Model, typename real, int VARIANT>
 __device__ __forceinline__ real split_cost_rollout(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
                                                    int k, unsigned long long kg, bool in_range, bool active) {
     static_assert(ModelCopies<Model>::value == 1, "models with COPIES > 1 run the single-loop rollout (copies_rollout)");
-    typedef Ops<real> O;
-    constexpr int NX = Model::NX, NU = Model::NU;
-    const NoiseModel<real>& nm = a.nm;
-    const int tid = threadIdx.x, BS = blockDim.x / a.tps, T = a.T;
-    real c_tot = O::inf();
-    real* xcol = sm.xs + (tid % BS);
-    real x[NX];
-    real pert = (real)0, smooth = (real)0;
-    if (active) {
-        if (a.state_dev != nullptr) {
-            const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
+    if constexpr (FastRange<Model, real>::value) return split_cost_rollout_fast<Model, real, VARIANT>(a, mp, sm, k, kg, in_range, active);
+    else {
+        typedef Ops<real> O;
+        constexpr int NX = Model::NX, NU = Model::NU;
+        const NoiseModel<real>& nm = a.nm;
+        const int tid = threadIdx.x, BS = blockDim.x / a.tps, T = a.T;
+        real c_tot = O::inf();
+        real* xcol = sm.xs + (tid % BS);
+        real x[NX];
+        real pert = (real)0, smooth = (real)0;
+        if (active) {
+            if (a.state_dev != nullptr) {
+                const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
 #pragma unroll
-            for (int i = 0; i < NX; ++i) x[i] = sp[i];
-        } else {
+                for (int i = 0; i < NX; ++i) x[i] = sp[i];
+            } else {
 #pragma unroll
-            for (int i = 0; i < NX; ++i) x[i] = a.x0[i];
-        }
-        real vprev[NU];
+                for (int i = 0; i < NX; ++i) x[i] = a.x0[i];
+            }
+            real vprev[NU];
 #pragma unroll
-        for (int n = 0; n < NU; ++n) vprev[n] = (real)0;
+            for (int n = 0; n < NU; ++n) vprev[n] = (real)0;
 MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
-        for (int t = 0; t < T; ++t) {
-            real v[NU], u[NU], eps[NU];
-            action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
-            noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
+            for (int t = 0; t < T; ++t) {
+                real v[NU], u[NU], eps[NU];
+                action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
+                noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
 #pragma unroll
-            for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
-            model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
+                for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
+                model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
 #pragma unroll
-            for (int i = 0; i < NX; ++i) xcol[(t * NX + i) * BS] = x[i];
-            pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
-            if (VARIANT == V_SMPPI) {
-                if (t > 0) {
+                for (int i = 0; i < NX; ++i) xcol[(t * NX + i) * BS] = x[i];
+                pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
+                if (VARIANT == V_SMPPI) {
+                    if (t > 0) {
 #pragma unroll
-                    for (int n = 0; n < NU; ++n) {
-                        const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
-                        smooth = O::add(smooth, O::mul(d, d));
+                        for (int n = 0; n < NU; ++n) {
+                            const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
+                            smooth = O::add(smooth, O::mul(d, d));
+                        }
                     }
-                }
 #pragma unroll
-                for (int n = 0; n < NU; ++n) vprev[n] = v[n];
+                    for (int n = 0; n < NU; ++n) vprev[n] = v[n];
+                }
             }
         }
-    }
-    __syncthreads();
-    if (in_range) {
+        __syncthreads();
+        if (in_range) {
 MPPI_UNROLL_N(2)
-        for (int t = tid / BS; t < T; t += a.tps) {      // independent across t: two in flight per thread
-            real v[NU], u[NU], xt[NX];
-            action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
+            for (int t = tid / BS; t < T; t += a.tps) {      // independent across t: two in flight per thread
+                real v[NU], u[NU], xt[NX];
+                action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
 #pragma unroll
-            for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);
+                for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);
 #pragma unroll
-            for (int i = 0; i < NX; ++i) xt[i] = xcol[(t * NX + i) * BS];
-            xcol[(t * NX) * BS] = model_cost<Model, real>(mp, xt, u, t);              // mppi.py:318
+                for (int i = 0; i < NX; ++i) xt[i] = xcol[(t * NX + i) * BS];
+                xcol[(t * NX) * BS] = model_cost<Model, real>(mp, xt, u, t);              // mppi.py:318
+            }
         }
+        __syncthreads();
+        if (active) {
+            real roll = (real)0;
+            for (int t = 0; t < T; ++t) roll = O::add(roll, xcol[(t * NX) * BS]);         // mppi.py:319, t = 0..T-1
+            if (Model::template has_terminal<real>(mp)) roll = O::add(roll, Model::template terminal<real>(mp, x));
+            c_tot = O::add(roll, pert);                                                   // mppi.py:416
+            if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));   // mppi.py:562,569
+            a.cost_total[k] = c_tot;
+        }
+        return c_tot;
     }
-    __syncthreads();
-    if (active) {
-        real roll = (real)0;
-        for (int t = 0; t < T; ++t) roll = O::add(roll, xcol[(t * NX) * BS]);         // mppi.py:319, t = 0..T-1
-        if (Model::template has_terminal<real>(mp)) roll = O::add(roll, Model::template terminal<real>(mp, x));
-        c_tot = O::add(roll, pert);                                                   // mppi.py:416
-        if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));   // mppi.py:562,569
-        a.cost_total[k] = c_tot;
-    }
-    return c_tot;
 }
 
 // one step's costs c[0..M-1] of the M copies (mppi.py:362-364): cs[m] += c[m], and var += var_m(c) * disc with the
@@ -1378,6 +1603,8 @@ __global__ void __launch_bounds__(512, MINB) fused_command_kernel(const __grid_c
         } else if constexpr (ModelCopies<Model>::value > 1) {
             // C''. M copies of the sample's rollout, interleaved in registers
             if (active) c_tot = copies_rollout<Model, real, VARIANT>(a, mp, sm, k, kg);
+        } else if constexpr (FastRange<Model, real>::value) {
+            if (active) c_tot = single_loop_rollout_fast<Model, real, VARIANT>(a, mp, sm, k, kg);
         } else if (active) {
 
             // C. rollout (mppi.py:297-332) + action cost (mppi.py:409,415) [+ smoothness :559-562]
@@ -1571,6 +1798,17 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
         for (int i = 0; i < NX; ++i) x[i] = sp[i];
     } else {
         for (int i = 0; i < NX; ++i) x[i] = a.x0[i];
+    }
+    if constexpr (FastRange<Model, real>::value) {      // the fast step where the command's rollouts take it
+        if (Model::template in_fast_range<real>(mp, x, a.T)) {
+            for (int t = 0; t < a.T; ++t) {
+                real u[NU];
+                for (int n = 0; n < NU; ++n) u[n] = O::mul(a.nm.u_scale, pa[t * NU + n]);         // mppi.py:313 / :445
+                model_step<Model, real, true>(mp, x, u, t);
+                for (int i = 0; i < NX; ++i) states[((size_t)k * a.T + t) * NX + i] = x[i];
+            }
+            return;
+        }
     }
     for (int t = 0; t < a.T; ++t) {
         real u[NU];
