@@ -23,7 +23,7 @@
 extern "C" {
 #endif
 
-#define MPPI_B200_ABI_VERSION 1
+#define MPPI_B200_ABI_VERSION 2
 
 #define MPPI_MAX_NU 4            /* control dimension supported by the fused registry            */
 #define MPPI_MAX_NX 8            /* state dimension supported by the fused registry              */
@@ -212,6 +212,8 @@ typedef struct MppiLaunchInfo {
                                     reduce their softmin partials through distributed shared memory        */
     int32_t xchg_records;        /* sharded controllers: records each rank publishes per command (its cluster records
                                     in direct mode, 1 = the rank's combined record); 0 = not sharded       */
+    int32_t ll_tail;             /* 1 if the command runs the split-cost kernel specialised for one GPU in LL mode (every
+                                    cluster record through this GPU's own mailbox): its softmin tail is inlined   */
 } MppiLaunchInfo;
 
 int mppi_b200_abi_version(void);
@@ -302,7 +304,9 @@ int mppi_apply_partials(const MppiFusedParams* p, const void* partials, void* st
  * with NVRTC in process).  `cubin` is the compiled module, `names` the lowered names of its kernels:
  * [0] fused_command_kernel<UserModel, real, variant, false, false>   [1] ... split-cost (or NULL)
  * [2] ... batched, MPPI variant (or NULL)   [3] resident_command_kernel<UserModel, real, variant> (or NULL)
- * [4] states_kernel<UserModel, real>.  The handle goes into MppiFusedParams.user_model with model = MPPI_MODEL_USER. */
+ * [4] states_kernel<UserModel, real>.  A module with a split-cost kernel also exports its single-GPU LL form as
+ * `mppi_user_fused_command_kernel_ll` (MPPI_USER_KERNEL_LL).  The handle goes into MppiFusedParams.user_model with
+ * model = MPPI_MODEL_USER. */
 int mppi_user_model_register(const void* cubin, uint64_t cubin_bytes, int32_t nx, int32_t nu, int32_t n_params, int32_t dtype,
                              int32_t variant, const char* const* names, void** handle_out);
 int mppi_user_model_release(void* handle);

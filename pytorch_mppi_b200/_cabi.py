@@ -16,7 +16,7 @@ MPPI_MAX_NX = 8
 MPPI_MODEL_PARAM_DOUBLES = 48
 MPPI_MAX_RANKS = 8
 MPPI_MAX_COPIES = 8
-ABI_VERSION = 1
+ABI_VERSION = 2
 
 # enums
 VARIANT_MPPI, VARIANT_SMPPI, VARIANT_KMPPI = 0, 1, 2
@@ -130,6 +130,7 @@ class MppiLaunchInfo(C.Structure):
         ("wide_regs", C.c_int32),
         ("cluster_size", C.c_int32),
         ("xchg_records", C.c_int32),
+        ("ll_tail", C.c_int32),
     ]
 
 

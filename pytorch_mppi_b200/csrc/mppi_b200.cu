@@ -557,6 +557,17 @@ int mppi_user_model_register(const void* cubin, uint64_t cubin_bytes, int32_t nx
         }
         *slots[i] = (const void*)k;
     }
+    if (mk.split[variant] != nullptr) {
+        // its single-GPU LL form, which the module exports under a fixed name (MPPI_USER_KERNEL_LL in mppi_fused.cuh)
+        cudaKernel_t k = nullptr;
+        cudaError_t e = cudaLibraryGetKernel(&k, lib, "mppi_user_fused_command_kernel_ll");
+        if (e != cudaSuccess) {
+            cudaLibraryUnload(lib);
+            delete h;
+            return cuda_fail(e, "mppi_user_fused_command_kernel_ll");
+        }
+        mk.split_ll[variant] = (const void*)k;
+    }
     if (mk.fused[variant] == nullptr || mk.states == nullptr) {
         cudaLibraryUnload(lib);
         delete h;

@@ -706,8 +706,8 @@ __device__ __forceinline__ void warp_fold(const KArgs<real>& a, Smem<real>& sm, 
 // the tail runs once per command on a cold instruction cache, where instruction count, not arithmetic, sets its time
 // (ncu: `no_instruction` is the third-largest stall of the kernel).
 template <typename real>
-__device__ __noinline__ void combine_records(const double* recs, int nrec, int R, double nfl, double* part2, double* sq,
-                                             double* numd) {
+__device__ __forceinline__ void combine_records_body(const double* recs, int nrec, int R, double nfl, double* part2, double* sq,
+                                                     double* numd) {
     typedef Ops<real> O;
     const int RW = R + 2, C = R + 1;                      // columns: eta, V[0..R)
     const int tid = threadIdx.x, BD = blockDim.x, nG = BD >> 6, g = tid >> 6, jl = tid & 63, nw = BD >> 5;
@@ -754,6 +754,11 @@ __device__ __noinline__ void combine_records(const double* recs, int nrec, int R
         numd[1 + j] = t;
     }
     __syncthreads();
+}
+template <typename real>
+__device__ __noinline__ void combine_records(const double* recs, int nrec, int R, double nfl, double* part2, double* sq,
+                                             double* numd) {
+    combine_records_body<real>(recs, nrec, R, nfl, part2, sq, numd);
 }
 
 // ---- the same combination for records in the L2 workspace (ticket mode: grids of hundreds of CTAs) ---------------------
@@ -814,7 +819,7 @@ __device__ __noinline__ void combine_global(const double* recs, int nrec, int R,
 // and 32 cluster records per GPU at BASELINE config 2 — the barrier-and-scratch form above cost 2.3 + 2.9 us there
 // (every warp of the CTA walks its ~600 instructions, contending with the co-resident CTA at large K), this one a fraction.
 template <typename real>
-__device__ __noinline__ void combine_narrow(const double* recs, int nrec, int R, double nfl, double* numd) {
+__device__ __forceinline__ void combine_narrow_body(const double* recs, int nrec, int R, double nfl, double* numd) {
     typedef Ops<real> O;
     const int RW = R + 2, C = R + 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
@@ -848,20 +853,31 @@ __device__ __noinline__ void combine_narrow(const double* recs, int nrec, int R,
     }
     __syncthreads();
 }
+template <typename real>
+__device__ __noinline__ void combine_narrow(const double* recs, int nrec, int R, double nfl, double* numd) {
+    combine_narrow_body<real>(recs, nrec, R, nfl, numd);
+}
 #define MPPI_COMBINE_NARROW_MAX 64
 
-template <typename real>
+// INLINE: the combination's code in the caller's instruction stream (the single-GPU LL tail, see warp_tail), else one
+// out-of-line copy per form that every call site of the kernel shares
+template <typename real, bool INLINE = false>
 __device__ __forceinline__ void combine(Smem<real>& sm, const double* recs, int nrec, int R, double nfl) {
-    if (nrec <= MPPI_COMBINE_NARROW_MAX) combine_narrow<real>(recs, nrec, R, nfl, sm.numd);
-    else combine_records<real>(recs, nrec, R, nfl, sm.part2, sm.sqd, sm.numd);
+    if (INLINE) {
+        if (nrec <= MPPI_COMBINE_NARROW_MAX) combine_narrow_body<real>(recs, nrec, R, nfl, sm.numd);
+        else combine_records_body<real>(recs, nrec, R, nfl, sm.part2, sm.sqd, sm.numd);
+    } else {
+        if (nrec <= MPPI_COMBINE_NARROW_MAX) combine_narrow<real>(recs, nrec, R, nfl, sm.numd);
+        else combine_records<real>(recs, nrec, R, nfl, sm.part2, sm.sqd, sm.numd);
+    }
 }
 
 // ---- record mailboxes: records of (R+2) doubles as LL words (payload32 | flag32), record r at word r * 2 (R+2) ------
 // a.peers[g], g < xw, are the mailboxes the record goes to: every rank's (sharded controller, over NVLink) or just this
 // GPU's own (single GPU: a region of the workspace) — self-validating words need no fence and no ticket, the finisher
 // sees a record one store-to-poll latency after it was written.
-static __device__ __noinline__ void xchg_publish_words(unsigned long long* const* peers, int xw, unsigned long long epoch, unsigned int parity_words,
-                                                int rec_index, int R, const double* src) {
+static __device__ __forceinline__ void xchg_publish_body(unsigned long long* const* peers, int xw, unsigned long long epoch,
+                                                         unsigned int parity_words, int rec_index, int R, const double* src) {
     const int nwords = 2 * (R + 2);
     const uint32_t flag = (uint32_t)(epoch & 0x7fffffffull) | 0x80000000u;
     const size_t off = (size_t)(epoch & 1ull) * parity_words + (size_t)rec_index * nwords;
@@ -874,14 +890,19 @@ static __device__ __noinline__ void xchg_publish_words(unsigned long long* const
     // (measured and rejected: a system-scope fence after the remote stores, meant to push the posted NVLink writes out
     // sooner, costs 4.5 us per command at two GPUs — 24.2 against 19.7 us back to back)
 }
-template <typename real>
+static __device__ __noinline__ void xchg_publish_words(unsigned long long* const* peers, int xw, unsigned long long epoch, unsigned int parity_words,
+                                                int rec_index, int R, const double* src) {
+    xchg_publish_body(peers, xw, epoch, parity_words, rec_index, R, src);
+}
+template <typename real, bool INLINE = false>
 __device__ __forceinline__ void xchg_publish(const KArgs<real>& a, int xw, int rec_index, const double* src) {
-    xchg_publish_words(a.peers, xw, a.epoch, a.xchg_parity_words, rec_index, a.R, src);
+    if (INLINE) xchg_publish_body(a.peers, xw, a.epoch, a.xchg_parity_words, rec_index, a.R, src);
+    else xchg_publish_words(a.peers, xw, a.epoch, a.xchg_parity_words, rec_index, a.R, src);
 }
 // all threads of the CTA; nrec records from this rank's own mailbox into sm.xstage (doubles), PB polls in flight per
 // thread.  Returns 0, or 1 on timeout.
-static __device__ __noinline__ int xchg_collect_words(const unsigned long long* mine, unsigned long long epoch, unsigned long long timeout_ns,
-                                               int nwords, uint32_t* dst) {
+static __device__ __forceinline__ int xchg_collect_body(const unsigned long long* mine, unsigned long long epoch,
+                                                        unsigned long long timeout_ns, int nwords, uint32_t* dst) {
     constexpr int PB = 8;
     const int BD = blockDim.x;
     const uint32_t flag = (uint32_t)(epoch & 0x7fffffffull) | 0x80000000u;
@@ -920,10 +941,16 @@ static __device__ __noinline__ int xchg_collect_words(const unsigned long long* 
     __syncthreads();
     return s_timeout;
 }
-template <typename real>
+static __device__ __noinline__ int xchg_collect_words(const unsigned long long* mine, unsigned long long epoch, unsigned long long timeout_ns,
+                                               int nwords, uint32_t* dst) {
+    return xchg_collect_body(mine, epoch, timeout_ns, nwords, dst);
+}
+template <typename real, bool INLINE = false>
 __device__ __forceinline__ int xchg_collect(const KArgs<real>& a, Smem<real>& sm, int own, int nrec) {
-    return xchg_collect_words(a.peers[own] + (size_t)(a.epoch & 1ull) * a.xchg_parity_words, a.epoch, a.xchg_timeout_ns,
-                              nrec * 2 * (a.R + 2), reinterpret_cast<uint32_t*>(sm.xstage));
+    const unsigned long long* mine = a.peers[own] + (size_t)(a.epoch & 1ull) * a.xchg_parity_words;
+    uint32_t* dst = reinterpret_cast<uint32_t*>(sm.xstage);
+    if (INLINE) return xchg_collect_body(mine, a.epoch, a.xchg_timeout_ns, nrec * 2 * (a.R + 2), dst);
+    return xchg_collect_words(mine, a.epoch, a.xchg_timeout_ns, nrec * 2 * (a.R + 2), dst);
 }
 
 // a peer never delivered: report it (device stats, pinned host word) and return a DEFINED action — the nominal the
@@ -945,11 +972,20 @@ __device__ void xchg_timed_out(const KArgs<real>& a, Smem<real>& sm, int nu) {
         *a.ticket = 0u;
     }
 }
+template <typename real, int VARIANT>
+__device__ __noinline__ void xchg_timed_out_rare(const KArgs<real>& a, Smem<real>& sm, int nu) {
+    xchg_timed_out<real, VARIANT>(a, sm, nu);
+}
 
 // ---- the tail: returns true in the CTA that finished the command --------------------------------------------------
 // PERSISTENT (resident kernel): the grid outlives the command, so the non-leader CTAs of a cluster complete the barrier
 // phase (arrive + wait) instead of exiting after their arrive.
-template <typename real, int VARIANT, int NU, bool PERSISTENT = false>
+// LL1: the launch is known to be single-GPU LL mode (NC > 1 clusters, every cluster record published to this GPU's own
+// mailbox; fused_command_kernel_ll).  Then the tail is one path — cluster stage, combine, publish, collect, combine,
+// finish_update — and its combines, publish and collect are inlined into it: the finisher runs on a cold instruction
+// cache (the L2 flushed between commands), where every jump into out-of-line code that no SM has fetched yet waits on
+// memory while the rest of the GPU idles.  Only the timeout report stays out of line.
+template <typename real, int VARIANT, int NU, bool PERSISTENT = false, bool LL1 = false>
 __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
     const int tid = threadIdx.x, BD = blockDim.x, lane = tid & 31, warp = tid >> 5;
     const int R = a.R, RW = R + 2;
@@ -957,13 +993,13 @@ __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
     const int cs = (int)cluster_nctarank();                  // cluster dims are (cs, 1, 1)
     const int cr = blockIdx.x % cs, cid = blockIdx.x / cs, NC = gridDim.x / cs;
     const double nfl = (double)a.nm.neg_inv_lambda;
-    const bool sharded = a.world > 1 && !a.export_partial;
+    const bool sharded = !LL1 && a.world > 1 && !a.export_partial;
     const int xw = sharded ? a.world : 1;                    // ranks whose records the finisher combines
     const int xr = sharded ? a.rank : 0;                     // this rank's slot among them
     // LL mode: the cluster records go out as flagged words (to this GPU's mailbox, and every peer's on a sharded
     // controller); the leader of cluster 0 polls for all xw x NC of them — no fence, no ticket.  Otherwise (grids whose
     // records do not fit the finisher's staging area): records to the L2 workspace, ticket among the leaders.
-    const bool ll = NC > 1 && a.xchg_npub == NC;
+    const bool ll = LL1 || (NC > 1 && a.xchg_npub == NC);
     __shared__ int s_is_last;
 
     // (1) warp records -> the cluster leader's shared memory
@@ -987,12 +1023,12 @@ __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
 
     // (2) leader: cs x nrw warp records -> one cluster record in sm.numd
     {
-        combine<real>(sm, sm.wrec, cs * nrw, R, nfl);
+        combine<real, LL1>(sm, sm.wrec, cs * nrw, R, nfl);
     }
     stamp(a.dbg, 9);
     // (3) publish the cluster record
     if (ll) {
-        xchg_publish<real>(a, xw, xr * NC + cid, sm.numd);
+        xchg_publish<real, LL1>(a, xw, xr * NC + cid, sm.numd);
         if (cid != 0) return false;                          // the leader of cluster 0 finishes the command
     } else if (NC > 1) {
         for (int i = tid; i < RW; i += BD) a.crec[(size_t)cid * RW + i] = sm.numd[i];
@@ -1010,17 +1046,18 @@ __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
 
     // (4) finisher: all records -> (beta, eta, numerators) in sm.numd
     if (ll) {
-        if (xchg_collect<real>(a, sm, xr, xw * NC)) {
-            xchg_timed_out<real, VARIANT>(a, sm, NU);
+        if (xchg_collect<real, LL1>(a, sm, xr, xw * NC)) {
+            if (LL1) xchg_timed_out_rare<real, VARIANT>(a, sm, NU);
+            else xchg_timed_out<real, VARIANT>(a, sm, NU);
             return true;
         }
         stamp(a.dbg, 12);
-        combine<real>(sm, sm.xstage, xw * NC, R, nfl);
+        combine<real, LL1>(sm, sm.xstage, xw * NC, R, nfl);
     } else if (NC > 1) {
         combine_global<real>(a.crec, NC, R, nfl, sm.part2, sm.sqd, sm.numd);
     }
     stamp(a.dbg, 10);
-    if (a.export_partial) {   // library-collective route: caller all-gathers, mppi_apply_partials finishes
+    if (!LL1 && a.export_partial) {   // library-collective route: caller all-gathers, mppi_apply_partials finishes
         const int TN = a.TN;
         for (int j = tid; j < RW; j += BD) a.partial_out[j] = sm.numd[j];
         for (int j = tid; j < TN; j += BD) {
@@ -1535,9 +1572,9 @@ template <class Model> struct FusedMinBlocks {
 };
 template <> struct FusedMinBlocks<PendulumMLPModel> { static constexpr int value = 1; };
 
-template <class Model, typename real, int VARIANT, bool BATCHED, bool SPLIT = false, int MINB = (SPLIT ? 1 : FusedMinBlocks<Model>::value)>
-__global__ void __launch_bounds__(512, MINB) fused_command_kernel(const __grid_constant__ KArgs<real> a_in,
-                                                            const __grid_constant__ typename Model::template P<real> mp) {
+// LL1: the tail of warp_tail<..., LL1 = true> (fused_command_kernel_ll below)
+template <class Model, typename real, int VARIANT, bool BATCHED, bool SPLIT, bool LL1>
+__device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, const typename Model::template P<real>& mp) {
     typedef Ops<real> O;
     constexpr int NX = Model::NX, NU = Model::NU;
     extern __shared__ __align__(16) unsigned char smem[];
@@ -1671,9 +1708,34 @@ MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
         if (tile + (int)gridDim.x < a.n_tiles) __syncthreads();      // the tile is refilled by the next pass
     }
     if (!staged) stage_finish<real, VARIANT, NU>(a, sm);
-    warp_tail<real, VARIANT, NU>(a, sm);
+    warp_tail<real, VARIANT, NU, false, LL1>(a, sm);
     stamp(a.dbg, 7);
 }
+
+template <class Model, typename real, int VARIANT, bool BATCHED, bool SPLIT = false, int MINB = (SPLIT ? 1 : FusedMinBlocks<Model>::value)>
+__global__ void __launch_bounds__(512, MINB) fused_command_kernel(const __grid_constant__ KArgs<real> a_in,
+                                                            const __grid_constant__ typename Model::template P<real> mp) {
+    fused_command_body<Model, real, VARIANT, BATCHED, SPLIT, false>(a_in, mp);
+}
+
+// The split-cost kernel of single-GPU plans in LL mode (the host selects it: NC > 1 clusters, every cluster record in this
+// GPU's own mailbox, no peers, no export): its tail is the one path that geometry runs, inlined (warp_tail, LL1).  Every
+// other plan keeps fused_command_kernel, whose tail serves all modes through shared out-of-line code.
+template <class Model, typename real, int VARIANT>
+__global__ void __launch_bounds__(512, 1) fused_command_kernel_ll(const __grid_constant__ KArgs<real> a_in,
+                                                                  const __grid_constant__ typename Model::template P<real> mp) {
+    fused_command_body<Model, real, VARIANT, false, true, true>(a_in, mp);
+}
+
+#ifdef __CUDACC_RTC__
+// A user model (NVRTC, one module per dtype and controller variant) exports its fused_command_kernel_ll under one unmangled
+// name, which mppi_user_model_register looks up beside the kernels it is given by name.
+#define MPPI_USER_KERNEL_LL(Model, real, VARIANT)                                                                            \
+    extern "C" __global__ void __launch_bounds__(512, 1) mppi_user_fused_command_kernel_ll(                                 \
+        const __grid_constant__ mppi::KArgs<real> a_in, const __grid_constant__ Model::P<real> mp) {                         \
+        mppi::fused_command_body<Model, real, VARIANT, false, true, true>(a_in, mp);                                         \
+    }
+#endif
 
 // =================================================================================================
 // Generic path, part 1: sample + perturb with coalesced write-out (mppi.py:375-385, 409, 415;

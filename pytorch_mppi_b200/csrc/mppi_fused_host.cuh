@@ -41,10 +41,13 @@ inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedPara
 //              one CTA per SM and all its clusters are co-resident (cudaOccupancyMaxActiveClusters), else 1
 //   npub       sharded controllers: the records a rank publishes to its peers per command — its cluster records when
 //              their staging (world x clusters x (R+2) doubles) is small (direct mode), else its one combined record
+//   ll         split-cost plans of one GPU whose clusters all publish to its own mailbox (LL mode) run
+//              fused_command_kernel_ll, the instantiation whose tail is that one path, inlined (mppi_fused.cuh, warp_tail)
 struct FusedChoice {
     const void* kernel;
     Geometry g;
     int split;
+    int ll;
 };
 
 // the rank records of a command are exchanged with peers inside the kernel (else they stay in this GPU's own mailbox)
@@ -103,8 +106,9 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     if (const char* e = getenv("MPPI_B200_CLUSTER")) want = atoi(e);
     cudaFuncAttributes fa;
     CK(cudaFuncGetAttributes(&fa, kernel));
-    const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;
     const int envs = batched ? p->n_env : 1;
+    const bool may_ll = split && !sharded && !(p->flags & MPPI_FLAG_EXPORT_PARTIAL) && mk->split_ll[V] != nullptr;
+    const void* chosen = kernel;
     g.cluster = 0;
     g.npub = 1;
     for (int cs = 8; cs >= 1; cs >>= 1) {
@@ -120,6 +124,10 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
         if (const char* e = getenv("MPPI_B200_XCHG_DIRECT"))
             if (atoi(e) == 0) npub = 1;
         const int xst = fused_xstage_doubles(sharded, world, npub, R);
+        const void* kc = may_ll && NC > 1 && npub == NC ? mk->split_ll[V] : kernel;
+        CK(cudaFuncGetAttributes(&fa, kc));
+        const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;
+        if (kc != kernel) CK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_limit));
         const int smem = make_layout<real>(p->variant, p->T, p->nu, p->S, R, g.BD, g.BS, fused_layout_nb(NC, npub),
                                            layout_extra(tile2, split ? mk->nx : 0, cs, xst)).total + ens_bytes;
         if (smem > dyn_limit) continue;
@@ -128,7 +136,7 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
             cudaLaunchAttribute at[3];
             launch_config(cfg, at, nbp, g.BD, smem, nullptr, (p->flags & MPPI_FLAG_PDL) != 0, envs, cs);
             int max_clusters = 0;
-            if (cudaOccupancyMaxActiveClusters(&max_clusters, kernel, &cfg) != cudaSuccess) {
+            if (cudaOccupancyMaxActiveClusters(&max_clusters, kc, &cfg) != cudaSuccess) {
                 cudaGetLastError();
                 continue;
             }
@@ -140,10 +148,12 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
         g.nb = nbp;
         g.smem = smem;
         g.npub = npub;
+        g.regs = fa.numRegs;
+        chosen = kc;
         break;
     }
     if (g.cluster == 0) return UNSUPPORTED("shared-memory tile does not fit");
-    c = FusedChoice{kernel, g, split};
+    c = FusedChoice{chosen, g, split, chosen != kernel};
     return MPPI_OK;
 }
 
@@ -175,6 +185,7 @@ template <typename real> int query_fused(const ModelKernels* mk, const MppiFused
     info->split_cost = c.split;
     info->cluster_size = g.cluster;
     info->xchg_records = g.npub;
+    info->ll_tail = c.ll;
     return MPPI_OK;
 }
 

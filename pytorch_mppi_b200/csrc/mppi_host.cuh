@@ -72,6 +72,7 @@ struct ModelKernels {
     void (*load)(const ModelKernels* self, void* dst, const double* blob, const double* ext, int n_ext);
     const void* fused[3];            // fused_command_kernel<Model, real, V, false, false>, V = MPPI / SMPPI / KMPPI
     const void* split[3];            // ... SPLIT = true (nullptr: not available)
+    const void* split_ll[3];         // fused_command_kernel_ll<Model, real, V>: split-cost, single-GPU LL tail (or nullptr)
     const void* batched;             // fused_command_kernel<Model, real, V_MPPI, true>
     const void* resident[3];         // resident_command_kernel<Model, real, V> (nullptr: not available)
     const void* resident_stamped;    // the one instantiation with %globaltimer stamps, or nullptr

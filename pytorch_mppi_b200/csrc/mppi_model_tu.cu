@@ -60,6 +60,10 @@ template <int V> const void* split_kernel() {
     if constexpr (kIsMlp || kIsEnsemble) return nullptr;      // its step is the network; the cost is nothing
     else return (const void*)fused_command_kernel<TuModel, TuReal, V, false, true>;
 }
+template <int V> const void* split_ll_kernel() {
+    if constexpr (kIsMlp || kIsEnsemble) return nullptr;
+    else return (const void*)fused_command_kernel_ll<TuModel, TuReal, V>;
+}
 const void* batched_kernel() {
     if constexpr (kIsEnsemble) return nullptr;                // MPPI_Batched has no rollout_samples
     else return (const void*)fused_command_kernel<TuModel, TuReal, V_MPPI, true>;
@@ -83,6 +87,7 @@ const ModelKernels g_kernels = {
     {(const void*)fused_command_kernel<TuModel, TuReal, V_MPPI, false>, (const void*)fused_command_kernel<TuModel, TuReal, V_SMPPI, false>,
      (const void*)fused_command_kernel<TuModel, TuReal, V_KMPPI, false>},
     {split_kernel<V_MPPI>(), split_kernel<V_SMPPI>(), split_kernel<V_KMPPI>()},
+    {split_ll_kernel<V_MPPI>(), split_ll_kernel<V_SMPPI>(), split_ll_kernel<V_KMPPI>()},
     batched_kernel(),
     {resident_kernel<V_MPPI>(), resident_kernel<V_SMPPI>(), resident_kernel<V_KMPPI>()},
     stamped_resident_kernel(),

@@ -1,6 +1,6 @@
 """What the pendulum's rollout recurrence loop contains, read from the SASS of a built library (no GPU needed: cuobjdump).
 usage: sass_rollout_loop.py [lib.so] [kernel-substring]
-  default kernel: the C2 command kernel, fused_command_kernel<PendulumModel, float, MPPI, not batched, split-cost>
+  default kernel: the C2 command kernel, fused_command_kernel_ll<PendulumModel, float, MPPI> (split-cost, single-GPU LL tail)
 
 The recurrence loop is the innermost backward branch whose body multiplies by 2/pi (the sine's quadrant); between its
 head and its back-edge the script counts every instruction, the float <-> int conversions (F2I, I2F, I2FP), the
@@ -13,7 +13,7 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 lib = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "pytorch_mppi_b200", "csrc", "libmppi_b200.so")
-want = sys.argv[2] if len(sys.argv) > 2 else "fused_command_kernelINS_13PendulumModelEfLi0ELb0ELb1ELi1E"
+want = sys.argv[2] if len(sys.argv) > 2 else "fused_command_kernel_llINS_13PendulumModelEfLi0EE"
 
 txt = subprocess.run(["cuobjdump", "-sass", lib], capture_output=True, text=True, check=True).stdout
 code, cur = [], None
