@@ -23,13 +23,14 @@
 extern "C" {
 #endif
 
-#define MPPI_B200_ABI_VERSION 2
+#define MPPI_B200_ABI_VERSION 3
 
 #define MPPI_MAX_NU 4            /* control dimension supported by the fused registry            */
 #define MPPI_MAX_NX 8            /* state dimension supported by the fused registry              */
 #define MPPI_MODEL_PARAM_DOUBLES 48
 #define MPPI_MAX_RANKS 8         /* GPUs of one NVSwitch box                                     */
 #define MPPI_MAX_COPIES 8        /* rollout_samples of a user model compiled with copies (registers) */
+#define MPPI_MAX_MODEL_TENSORS 8 /* device tensors a user model's bodies may read                */
 
 typedef enum MppiStatus {
     MPPI_OK = 0,
@@ -42,7 +43,17 @@ typedef enum MppiStatus {
 } MppiStatus;
 
 typedef enum MppiVariant { MPPI_VARIANT_MPPI = 0, MPPI_VARIANT_SMPPI = 1, MPPI_VARIANT_KMPPI = 2 } MppiVariant;
-typedef enum MppiDType { MPPI_F32 = 0, MPPI_F64 = 1 } MppiDType;
+typedef enum MppiDType { MPPI_F32 = 0, MPPI_F64 = 1, MPPI_U8 = 2, MPPI_I32 = 3 } MppiDType;   /* U8 / I32: tensor elements only */
+
+/* A read-only device tensor a user model's bodies read (CudaModel(tensors=...)): contiguous, row-major, element type
+ * `dtype` (MPPI_F32 / MPPI_F64 / MPPI_U8 / MPPI_I32), 1 <= ndim <= 4, shape[d] > 0 for d < ndim, at most 2^31 - 1
+ * elements.  Its data must outlive every command that may read it. */
+typedef struct MppiTensorRef {
+    const void* data;
+    int32_t dtype;
+    int32_t ndim;
+    int64_t shape[4];
+} MppiTensorRef;
 
 /* Registry of analytic models whose dynamics + running cost are compiled into the fused kernel.
  * (The reference takes arbitrary Python callables, mppi.py:147-157; arbitrary callables use the
@@ -193,6 +204,11 @@ typedef struct MppiFusedParams {
     double rollout_var_cost;
     const void* var_discount;    /* (T) device buffer of the controller dtype: rollout_var_discount ** arange(T)
                                     (mppi.py:174-175); required when rollout_samples > 1                        */
+    /* ---- device tensors of a user model (mppi_user_model_set_tensors): HOST array of n_model_tensors references, in
+     * the order and with the dtypes / ndims the model was compiled with; read at call / plan-creation time (a plan keeps
+     * its own copy).  0 / NULL for every other model. */
+    const MppiTensorRef* model_tensors;
+    int32_t n_model_tensors;
     const void* model_weights;   /* model == MPPI_MODEL_PENDULUM_MLP_ENSEMBLE: (rollout_samples, 1250) DEVICE buffer of
                                     the controller dtype, one network per row (see the model_params layouts); read by
                                     every command, so it must outlive the plan.  Required for that model, else unused */
@@ -219,7 +235,7 @@ typedef struct MppiLaunchInfo {
 int mppi_b200_abi_version(void);
 /* Layout probe for foreign-language mirrors of MppiFusedParams: which=0 sizeof, 1 offsetof(seed),
  * 2 offsetof(state), 3 offsetof(U), 4 offsetof(rank), 5 offsetof(partial_out), 6 sizeof(MppiLaunchInfo),
- * 7 offsetof(model_weights). */
+ * 7 offsetof(model_weights), 8 offsetof(model_tensors). */
 uint64_t mppi_abi_layout(int which);
 const char* mppi_status_string(int status);
 const char* mppi_last_cuda_error(void);
@@ -259,6 +275,13 @@ int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint
  * MPPI_ERR_BAD_ARG: null plan or model_params, n_ext < 0, ext NULL with n_ext > 0.  MPPI_ERR_UNSUPPORTED while a
  * resident grid is armed (its parameters are frozen; mppi_resident_stop first). */
 int mppi_plan_set_model_params(void* plan, const double* model_params, const double* ext, int32_t n_ext);
+/* New device tensors for a user model's plan (MppiFusedParams.model_tensors): the plan re-packs only the tensor views of
+ * its parameter block — no kernel selection, geometry, allocation or CUDA call.  The count, dtypes and ndims must be the
+ * model's; shapes and data pointers may change.  Commands already launched keep the views they were launched with.
+ * Edits of a tensor's contents need no call: a command reads them in stream order.
+ * MPPI_ERR_BAD_ARG: null plan, refs NULL with n > 0, or a reference the model's signature refuses (see
+ * mppi_user_model_set_tensors).  MPPI_ERR_UNSUPPORTED while a resident grid is armed. */
+int mppi_plan_set_model_tensors(void* plan, const MppiTensorRef* refs, int32_t n);
 
 /* ---- Resident mode: command() without a kernel launch ---------------------------------------------
  * For a host control loop (mppi.py:240-252 called once per control step).  One cooperative launch leaves the
@@ -315,6 +338,14 @@ int mppi_user_model_release(void* handle);
  * or resident kernels (names[1..3] NULL), so its commands run the single-loop rollout and resident mode is refused.
  * MPPI_ERR_BAD_ARG: bad handle, copies outside 1..MPPI_MAX_COPIES, or copies > 1 with any of those kernels. */
 int mppi_user_model_set_copies(void* handle, int32_t copies);
+/* The device tensors a user model's kernels were compiled to read (CudaModel(tensors=...)): their count (0..
+ * MPPI_MAX_MODEL_TENSORS), element types and ndims, in the order of the views in its parameter block
+ * `struct P { real v[n_params]; View t0; ...; }`, View = { const T* data; int32_t shape[4]; } (24 bytes, 8-aligned).
+ * The shapes and pointers come with every plan (MppiFusedParams.model_tensors), which must then match this signature:
+ * same count, dtypes and ndims, non-null data, positive dimensions, at most 2^31 - 1 elements (else MPPI_ERR_BAD_ARG).
+ * MPPI_ERR_BAD_ARG: bad handle, n outside 0..MPPI_MAX_MODEL_TENSORS, NULL arrays with n > 0, an unknown dtype or an ndim
+ * outside 1..4.  MPPI_ERR_UNSUPPORTED: the parameter block would exceed the largest block a kernel takes. */
+int mppi_user_model_set_tensors(void* handle, int32_t n, const int32_t* dtypes, const int32_t* ndims);
 /* Highest command epoch this plan has used (the tag of its reduction records, shared by the launch and resident routes);
  * pass it as MppiFusedParams.epoch when re-creating the plan so that stale records can never match. */
 uint64_t mppi_plan_epoch(void* plan);

@@ -16,11 +16,13 @@ MPPI_MAX_NX = 8
 MPPI_MODEL_PARAM_DOUBLES = 48
 MPPI_MAX_RANKS = 8
 MPPI_MAX_COPIES = 8
-ABI_VERSION = 2
+MPPI_MAX_MODEL_TENSORS = 8
+ABI_VERSION = 3
 
 # enums
 VARIANT_MPPI, VARIANT_SMPPI, VARIANT_KMPPI = 0, 1, 2
 F32, F64 = 0, 1
+U8, I32 = 2, 3                       # element types of model tensors only
 MODEL_PENDULUM, MODEL_LINEAR_POINT, MODEL_PENDULUM_MLP = 1, 2, 3
 MODEL_PENDULUM_MLP_ENSEMBLE = 4
 MODEL_USER = 100
@@ -38,6 +40,16 @@ FLAG_WIDE_REGS = 1 << 10
 
 STATUS = {0: "ok", -1: "bad argument", -2: "unsupported", -3: "workspace too small", -4: "CUDA error",
           -5: "ABI mismatch", -6: "peer exchange timeout"}
+
+
+class MppiTensorRef(C.Structure):
+    """Mirror of `struct MppiTensorRef`: one device tensor a user model's bodies read."""
+    _fields_ = [
+        ("data", C.c_void_p),
+        ("dtype", C.c_int32),
+        ("ndim", C.c_int32),
+        ("shape", C.c_int64 * 4),
+    ]
 
 
 class MppiFusedParams(C.Structure):
@@ -111,6 +123,8 @@ class MppiFusedParams(C.Structure):
         ("rollout_samples", C.c_int32),
         ("rollout_var_cost", C.c_double),
         ("var_discount", C.c_void_p),
+        ("model_tensors", C.c_void_p),
+        ("n_model_tensors", C.c_int32),
         ("model_weights", C.c_void_p),
     ]
 
@@ -150,6 +164,7 @@ SYMBOLS = [
     ("mppi_plan_command_host", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mppi_plan_set_model_params", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),
+    ("mppi_plan_set_model_tensors", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     ("mppi_resident_start", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     ("mppi_resident_command", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]),
     ("mppi_resident_sync", C.c_int, [C.c_void_p]),
@@ -160,6 +175,7 @@ SYMBOLS = [
                                            C.POINTER(C.c_char_p), C.POINTER(C.c_void_p)]),
     ("mppi_user_model_release", C.c_int, [C.c_void_p]),
     ("mppi_user_model_set_copies", C.c_int, [C.c_void_p, C.c_int32]),
+    ("mppi_user_model_set_tensors", C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     ("mppi_apply_partials", C.c_int, [_P, C.c_void_p, C.c_void_p]),
     ("mppi_xchg_create", C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
     ("mppi_xchg_open", C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),

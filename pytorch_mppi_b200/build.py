@@ -26,7 +26,8 @@ def _h(*names):
     return [os.path.join(CSRC, n) for n in names]
 
 
-COMMON_HEADERS = _h("mppi_host.cuh", "mppi_fused.cuh", "mppi_math.cuh", "mppi_resident.cuh", "mppi_resident_host.h") + [PUBLIC_HEADER]
+COMMON_HEADERS = _h("mppi_host.cuh", "mppi_fused.cuh", "mppi_math.cuh", "mppi_resident.cuh", "mppi_resident_host.h",
+                    "mppi_model_tensors.h") + [PUBLIC_HEADER]
 MODEL_HEADERS = COMMON_HEADERS + _h("mppi_mlp_tc.cuh")
 CABI_HEADERS = COMMON_HEADERS + _h("mppi_fused_host.cuh")
 

@@ -80,6 +80,12 @@ int check_rollout_samples(const MppiFusedParams* p, const ModelKernels* mk) {
     return MPPI_OK;
 }
 
+// the checks every route that packs the model's parameter block makes first: rollout copies and tensors.  No CUDA call.
+int check_model_args(const MppiFusedParams* p, const ModelKernels* mk) {
+    const int rc = check_rollout_samples(p, mk);
+    return rc ? rc : check_model_tensors(mk, p->model_tensors, p->n_model_tensors);
+}
+
 template <typename real>
 inline void plan_update(Plan* pl, const double* state, const void* state_dev, uint32_t flags, uint64_t seed, uint64_t offset,
                         const void* z, void* action_out, void* host_mailbox) {
@@ -324,6 +330,7 @@ uint64_t mppi_abi_layout(int which) {
         case 5: return offsetof(MppiFusedParams, partial_out);
         case 6: return sizeof(MppiLaunchInfo);
         case 7: return offsetof(MppiFusedParams, model_weights);
+        case 8: return offsetof(MppiFusedParams, model_tensors);
     }
     return 0;
 }
@@ -358,7 +365,7 @@ int mppi_fused_query(const MppiFusedParams* p, MppiLaunchInfo* out) {
     if ((rc = validate(p, true)) != MPPI_OK) return rc;
     const ModelKernels* mk = find_kernels(p, &rc);
     if (mk == nullptr) return rc;
-    if ((rc = check_rollout_samples(p, mk)) != MPPI_OK) return rc;
+    if ((rc = check_model_args(p, mk)) != MPPI_OK) return rc;
     return mk->is_double ? query_fused<double>(mk, p, out) : query_fused<float>(mk, p, out);
 }
 
@@ -385,7 +392,7 @@ int mppi_plan_create(const MppiFusedParams* p, void** plan_out) {
     Plan* pl = new (std::nothrow) Plan();
     if (pl == nullptr) return MPPI_ERR_BAD_ARG;
     const ModelKernels* mk = find_kernels(p, &rc);
-    if (mk != nullptr) rc = check_rollout_samples(p, mk);
+    if (mk != nullptr) rc = check_model_args(p, mk);
     if (mk != nullptr && rc == MPPI_OK) rc = mk->is_double ? build_plan<double>(mk, p, pl) : build_plan<float>(mk, p, pl);
     if (rc) {
         delete pl;
@@ -421,6 +428,16 @@ int mppi_plan_set_model_params(void* plan, const double* model_params, const dou
     pl->p.model_params_ext = ext;
     pl->p.n_model_params_ext = n_ext;
     load_model_params(pl->mk, &pl->p, pl->mparams);
+    return MPPI_OK;
+}
+
+// as mppi_plan_set_model_params, for the tensor views only (the parameters stay as they are)
+int mppi_plan_set_model_tensors(void* plan, const MppiTensorRef* refs, int32_t n) {
+    Plan* pl = reinterpret_cast<Plan*>(plan);
+    if (pl == nullptr || check_model_tensors(pl->mk, refs, n) != MPPI_OK) return MPPI_ERR_BAD_ARG;
+    if (pl->res.armed) return UNSUPPORTED("the resident grid holds the tensors it was launched with: stop it first");
+    if (n > 0) memcpy(pl->tensors, refs, sizeof(MppiTensorRef) * n);
+    load_model_tensors(pl->mk, pl->tensors, pl->mparams);
     return MPPI_OK;
 }
 
@@ -597,6 +614,24 @@ int mppi_user_model_set_copies(void* handle, int32_t copies) {
     return MPPI_OK;
 }
 
+int mppi_user_model_set_tensors(void* handle, int32_t n, const int32_t* dtypes, const int32_t* ndims) {
+    UserModelHandle* h = reinterpret_cast<UserModelHandle*>(handle);
+    if (h == nullptr || h->magic != kUserMagic || n < 0 || n > MPPI_MAX_MODEL_TENSORS) return MPPI_ERR_BAD_ARG;
+    if (n > 0 && (dtypes == nullptr || ndims == nullptr)) return MPPI_ERR_BAD_ARG;
+    for (int i = 0; i < n; ++i)
+        if (!mppi_tensors::known_dtype(dtypes[i]) || ndims[i] < 1 || ndims[i] > 4) return MPPI_ERR_BAD_ARG;
+    ModelKernels& mk = h->mk;
+    const int bytes = mppi_tensors::block_bytes(mk.np, mk.is_double ? 8 : 4, n);
+    if (bytes > MPPI_MODEL_BLOCK_BYTES) return UNSUPPORTED("user model parameter block (parameters and tensor views) too large");
+    for (int i = 0; i < n; ++i) {
+        mk.tensor_dtype[i] = dtypes[i];
+        mk.tensor_ndim[i] = ndims[i];
+    }
+    mk.n_tensors = n;
+    mk.param_bytes = bytes;
+    return MPPI_OK;
+}
+
 uint64_t mppi_plan_epoch(void* plan) {
     Plan* pl = reinterpret_cast<Plan*>(plan);
     if (pl == nullptr) return 0;
@@ -683,7 +718,7 @@ int mppi_materialize(const MppiFusedParams* p, void* perturbed_action, void* noi
     if (rc || states == nullptr) return rc;
     const ModelKernels* mk = find_kernels(p, &rc);
     if (mk == nullptr) return rc;
-    if ((rc = check_rollout_samples(p, mk)) != MPPI_OK) return rc;
+    if ((rc = check_model_args(p, mk)) != MPPI_OK) return rc;
     return mk->is_double ? run_states<double>(mk, p, perturbed_action, states, s) : run_states<float>(mk, p, perturbed_action, states, s);
 }
 
@@ -697,6 +732,7 @@ int mppi_rollout_states(const MppiFusedParams* p, const void* start_states, cons
     int rc = MPPI_ERR_UNSUPPORTED;
     const ModelKernels* mk = find_kernels(p, &rc);
     if (mk == nullptr) return rc;
+    if ((rc = check_model_tensors(mk, p->model_tensors, p->n_model_tensors)) != MPPI_OK) return rc;
     return mk->is_double ? run_rollout_states<double>(mk, p, start_states, actions, actions_stride, n_rollouts, T, states_out, s)
                          : run_rollout_states<float>(mk, p, start_states, actions, actions_stride, n_rollouts, T, states_out, s);
 }

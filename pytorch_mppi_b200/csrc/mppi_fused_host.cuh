@@ -230,6 +230,9 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
     pl->res_epoch_off = 0;
     pl->host_epoch = p->host_epoch;      // monotonic across re-plans: a stale mailbox tag of an earlier plan can never match
     pl->p = *p;
+    // mppi_plan_set_model_params re-packs the whole block from pl->p: the tensor references it reads are the plan's own
+    if (mk->n_tensors > 0) memcpy(pl->tensors, p->model_tensors, sizeof(MppiTensorRef) * mk->n_tensors);
+    pl->p.model_tensors = pl->tensors;
     return MPPI_OK;
 }
 

@@ -13,6 +13,7 @@
 
 #include "../../include/mppi_b200.h"
 #include "mppi_fused.cuh"
+#include "mppi_model_tensors.h"
 #include "mppi_resident.cuh"
 #include "mppi_resident_host.h"
 
@@ -56,6 +57,7 @@ struct Plan {
     unsigned long long res_epoch_off;  // resident mode: record-mailbox epoch of command seq = res_epoch_off + seq
     alignas(16) unsigned char kargs[sizeof(KArgs<double>)];
     alignas(16) unsigned char mparams[MPPI_MODEL_BLOCK_BYTES];
+    MppiTensorRef tensors[MPPI_MAX_MODEL_TENSORS];   // the plan's copy of p.model_tensors (p.model_tensors points here)
 };
 
 // What one (model, dtype) pair contributes: its kernels (as launchable handles) and how to pack its parameter block.
@@ -81,6 +83,8 @@ struct ModelKernels {
                                      // (the ensemble: mlp_ens_tc_command_kernel)
     void* library;                   // run-time user models: the cudaLibrary_t that owns the kernels
     int copies;                      // run-time user models: the COPIES their kernels were compiled with (0 or 1: none)
+    int n_tensors;                   // run-time user models: device tensor views behind the parameters (mppi_model_tensors.h)
+    int32_t tensor_dtype[MPPI_MAX_MODEL_TENSORS], tensor_ndim[MPPI_MAX_MODEL_TENSORS];
 };
 }  // namespace mppi_host
 
@@ -140,10 +144,21 @@ inline int validate(const MppiFusedParams* p, bool fused = false) {
 
 inline int rows_of(const MppiFusedParams* p) { return (p->variant == MPPI_VARIANT_KMPPI ? p->S : p->T) * p->nu; }
 
+// MPPI_OK if p->model_tensors match the tensors the model was compiled to read (none for every other model).  No CUDA call.
+inline int check_model_tensors(const ModelKernels* mk, const MppiTensorRef* refs, int n) {
+    return mppi_tensors::check_refs(mk->tensor_dtype, mk->tensor_ndim, mk->n_tensors, refs, n);
+}
+
+// The tensor views of a user model's block (checked references: check_model_tensors).
+inline void load_model_tensors(const ModelKernels* mk, const MppiTensorRef* refs, void* dst) {
+    if (mk->n_tensors > 0) mppi_tensors::pack_views(dst, mk->np, mk->is_double ? 8 : 4, refs, mk->n_tensors);
+}
+
 // The model's parameter block for these parameters (the packer of its unit).  The ensemble's block also carries the
-// device weight table and the copy count, which are not doubles of model_params.
+// device weight table and the copy count, which are not doubles of model_params; a user model's, its tensor views.
 inline void load_model_params(const ModelKernels* mk, const MppiFusedParams* p, void* dst) {
     mk->load(mk, dst, p->model_params, p->model_params_ext, p->n_model_params_ext);
+    load_model_tensors(mk, p->model_tensors, dst);
     if (p->model == MPPI_MODEL_PENDULUM_MLP_ENSEMBLE) {
         if (mk->is_double) PendulumMLPEnsembleModel::bind<double>(*reinterpret_cast<PendulumMLPEnsembleModel::P<double>*>(dst), p->model_weights, p->rollout_samples);
         else PendulumMLPEnsembleModel::bind<float>(*reinterpret_cast<PendulumMLPEnsembleModel::P<float>*>(dst), p->model_weights, p->rollout_samples);

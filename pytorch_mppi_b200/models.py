@@ -337,11 +337,27 @@ class CudaModel(AnalyticModel):
     belongs to copy ``r // K``.  Your twins therefore have to know K (the controller's num_samples; on a sharded
     controller, its shard's sample count).  `get_rollouts` runs copy 0, which is what such a twin computes for
     ``num_rollouts <= K`` rows.
+
+    Device tensors (costmaps, lookup tables, reference paths: data too large for `params`, or indexed by the state):
+    ``tensors={"costmap": cm, "path": path}`` makes each tensor a read-only view with its own name in `step_code`,
+    `cost_code` and `terminal_code`.  ``costmap(i, j)`` takes one integer index per dimension and returns the element
+    (``float``, ``double``, ``unsigned char`` or ``int`` for float32 / float64 / uint8 / int32 tensors); each index is
+    clamped to ``[0, costmap.size(d) - 1]``, so a lookup never leaves the tensor and acts as border replication outside a
+    map.  Tensors are contiguous, 1- to 4-dimensional, with at most 2**31 - 1 elements, on the controller's device
+    (at most MPPI_MAX_MODEL_TENSORS of them).  Only their names, dtypes and ndims are compiled into the kernels; a meta
+    tensor can stand in for one to compile ahead of time without a GPU (swap the real one in with `set_tensors`).
+    Contents edited in place on the controller's stream (``cm.copy_(new)``) take effect at the next `command()`, as
+    edits of `U` do.  `set_tensors(costmap=other)` swaps a tensor (same dtype and ndim, any shape) for the following
+    commands of every controller using the model, without recompiling or re-planning; each controller keeps the tensors
+    its plan points at alive.  Resident mode: the grid keeps running between `command_host()` calls, so it would race
+    with an in-place edit — while resident, change tensor contents only through `set_tensors`, which makes the grid
+    leave (as `set_params` does); the next `command_host()` brings it back.  Your torch callables close over the same
+    tensors (read them through `model.tensors` to follow `set_tensors`).
     """
     model_id = _cabi.MODEL_USER
 
     def __init__(self, nx, nu, step_code, cost_code, params=(), terminal_code=None, dynamics=None, running_cost=None,
-                 terminal_cost=None, step_dependent=False, copies=1):
+                 terminal_cost=None, step_dependent=False, copies=1, tensors=None):
         if not (1 <= nx <= _cabi.MPPI_MAX_NX and 1 <= nu <= _cabi.MPPI_MAX_NU):
             raise ValueError(f"nx <= {_cabi.MPPI_MAX_NX} and nu <= {_cabi.MPPI_MAX_NU} required")
         if isinstance(copies, bool) or not isinstance(copies, int) or not 1 <= copies <= _cabi.MPPI_MAX_COPIES:
@@ -353,6 +369,12 @@ class CudaModel(AnalyticModel):
         self._step_code, self._cost_code, self._terminal_code = step_code, cost_code, terminal_code
         self._dyn, self._cost, self._term = dynamics, running_cost, terminal_cost
         self._rtc_handles = {}
+        tensors = dict(tensors or {})
+        if len(tensors) > _cabi.MPPI_MAX_MODEL_TENSORS:
+            raise ValueError(f"at most {_cabi.MPPI_MAX_MODEL_TENSORS} tensors, got {len(tensors)}")
+        for name, t in tensors.items():
+            _check_tensor(name, t)
+        self.tensors = tensors
 
     @property
     def has_terminal(self):
@@ -373,6 +395,36 @@ class CudaModel(AnalyticModel):
         self.params = values
         self._param_version += 1
 
+    def set_tensors(self, **tensors):
+        """Replace device tensors by name, for the following commands of every controller using this model (see the
+        class docstring).  Each replacement keeps its tensor's dtype and ndim (they are compiled into the kernels); its
+        shape may change, without recompiling or re-planning."""
+        for name, t in tensors.items():
+            if name not in self.tensors:
+                raise ValueError(f"this model has no tensor {name!r} (it has {sorted(self.tensors)})")
+            _check_tensor(name, t)
+            old = self.tensors[name]
+            if t.dtype != old.dtype or t.dim() != old.dim():
+                raise ValueError(f"tensor {name!r} was compiled as {old.dtype} with {old.dim()} dimension(s); "
+                                 f"got {t.dtype} with {t.dim()}")
+        self.tensors = dict(self.tensors, **tensors)
+        self._param_version += 1
+
+    def tensor_refs(self, device):
+        """(MppiTensorRef array, tensors) of MppiFusedParams.model_tensors for a controller on `device`; None if the
+        model has no tensors.  The caller keeps both alive while the library may read them."""
+        if not self.tensors:
+            return None
+        ts = list(self.tensors.values())
+        arr = (_cabi.MppiTensorRef * len(ts))()
+        for r, (name, t) in zip(arr, self.tensors.items()):
+            if t.device != torch.device(device):
+                raise ValueError(f"tensor {name!r} is on {t.device}, the controller on {device}")
+            r.data, r.dtype, r.ndim = t.data_ptr(), _TENSOR_DTYPES[t.dtype][0], t.dim()
+            for d in range(t.dim()):
+                r.shape[d] = t.shape[d]
+        return arr, ts
+
     def header_text(self):
         n = max(len(self.params), 1)
         term = self._terminal_code if self._terminal_code is not None else "return (real)0;"
@@ -384,11 +436,16 @@ class CudaModel(AnalyticModel):
         decl += f"\n    static const int COPIES = {self.copies};" if cp else ""
         marg = ", const int m" if cp else ""
         mvoid = " (void)m;" if cp else ""
+        # device tensors: views behind the parameters (csrc/mppi_model_tensors.h packs them), bound to their names in
+        # every body; nothing of this is emitted for a model without tensors, whose header stays what it always was
+        views = "".join(f" TensorView<{_TENSOR_DTYPES[t.dtype][1]}, {t.dim()}> t{i};" for i, t in enumerate(self.tensors.values()))
+        tbind = "".join(f" const auto& {name} = P_.t{i}; (void){name};" for i, name in enumerate(self.tensors))
+        tview = _TENSOR_VIEW if self.tensors else ""
         return f"""// generated by pytorch_mppi_b200.models.CudaModel
-namespace mppi {{
+namespace mppi {{{tview}
 struct UserModel {{
     static const int NX = {self.nx}, NU = {self.nu}, NP = {n};{decl}
-    template <typename real> struct P {{ real v[NP]; }};
+    template <typename real> struct P {{ real v[NP];{views} }};
     template <typename real> static void load(P<real>& P_, const double* b, const double* ext = nullptr, int n_ext = 0) {{
         for (int i = 0; i < NP; ++i)
             P_.v[i] = (real)(i < {_cabi.MPPI_MODEL_PARAM_DOUBLES} ? b[i] : (ext != nullptr && i - {_cabi.MPPI_MODEL_PARAM_DOUBLES} < n_ext ? ext[i - {_cabi.MPPI_MODEL_PARAM_DOUBLES}] : 0.0));
@@ -396,20 +453,20 @@ struct UserModel {{
     template <typename real> static MPPI_HD void step(const P<real>& P_, real* x, const real* u{targ}{marg}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p;{tvoid}{mvoid}
+        (void)p;{tvoid}{mvoid}{tbind}
         {self._step_code}
     }}
     template <typename real> static MPPI_HD real cost(const P<real>& P_, const real* x, const real* u{targ}{marg}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p; (void)u;{tvoid}{mvoid}
+        (void)p; (void)u;{tvoid}{mvoid}{tbind}
         {self._cost_code}
     }}
     template <typename real> static MPPI_HD bool has_terminal(const P<real>&) {{ return {"true" if self.has_terminal else "false"}; }}
     template <typename real> static MPPI_HD real terminal(const P<real>& P_, const real* x{marg}) {{
         typedef Ops<real> O;
         const real* p = P_.v;
-        (void)p; (void)x;{mvoid}
+        (void)p; (void)x;{mvoid}{tbind}
         {term}
     }}
 }};
@@ -438,6 +495,11 @@ struct UserModel {{
             _cabi.check(rc, "mppi_user_model_register")
             if self.copies > 1:
                 _cabi.check(lib.mppi_user_model_set_copies(handle, self.copies), "mppi_user_model_set_copies")
+            if self.tensors:
+                n = len(self.tensors)
+                dtypes = (C.c_int32 * n)(*[_TENSOR_DTYPES[t.dtype][0] for t in self.tensors.values()])
+                ndims = (C.c_int32 * n)(*[t.dim() for t in self.tensors.values()])
+                _cabi.check(lib.mppi_user_model_set_tensors(handle, n, dtypes, ndims), "mppi_user_model_set_tensors")
             self._rtc_handles[key] = handle
         return self._rtc_handles[key]
 
@@ -460,6 +522,58 @@ struct UserModel {{
         if self._term is None:
             raise NotImplementedError("this CudaModel was created without a torch `terminal_cost` callable")
         return self._term(states, actions)
+
+
+# element types a model tensor may have: torch dtype -> (MppiDType, C++ element type in the bodies)
+_TENSOR_DTYPES = {torch.float32: (_cabi.F32, "float"), torch.float64: (_cabi.F64, "double"),
+                  torch.uint8: (_cabi.U8, "unsigned char"), torch.int32: (_cabi.I32, "int")}
+# names a tensor cannot take: what the generated struct and bodies already use, and C++ keywords
+_RESERVED = set("x u p t m real O P_ NX NU NP COPIES STEP_DEPENDENT".split()) | set("""
+    alignas alignof and and_eq asm auto bitand bitor bool break case catch char char16_t char32_t char8_t class compl
+    concept const consteval constexpr constinit const_cast continue co_await co_return co_yield decltype default delete
+    do double dynamic_cast else enum explicit export extern false float for friend goto if inline int long mutable
+    namespace new noexcept not not_eq nullptr operator or or_eq private protected public register reinterpret_cast
+    requires return short signed sizeof static static_assert static_cast struct switch template this thread_local
+    throw true try typedef typeid typename union unsigned using virtual void volatile wchar_t while xor xor_eq""".split())
+_INT31 = 2 ** 31 - 1
+# the read-only view a body reads a tensor through: one index per dimension, each clamped to [0, size(d) - 1] (border
+# replication outside a map), loads through the read-only data path; no pointer is exposed
+_TENSOR_VIEW = """
+template <typename T, int N> struct TensorView {
+    MPPI_HD int size(int d) const { return shape_[d]; }
+    template <typename... I> MPPI_HD T operator()(I... idx) const {
+        static_assert(sizeof...(I) == N, "a tensor takes one index per dimension");
+        const int ix[N] = {(int)idx...};
+        int off = 0;
+        for (int d = 0; d < N; ++d) off = off * shape_[d] + (ix[d] < 0 ? 0 : (ix[d] < shape_[d] ? ix[d] : shape_[d] - 1));
+#if defined(__CUDA_ARCH__)
+        return __ldg(data_ + off);
+#else
+        return data_[off];
+#endif
+    }
+  private:
+    const T* data_;
+    int shape_[4];
+};"""
+
+
+def _check_tensor(name, t):
+    """ValueError unless `t` can be a model tensor called `name`."""
+    if not isinstance(name, str) or not name.isidentifier() or not name.isascii() or name in _RESERVED or name.startswith("__"):
+        raise ValueError(f"tensor name {name!r} must be a C identifier that the generated model does not already use")
+    if not torch.is_tensor(t):
+        raise ValueError(f"tensor {name!r} must be a torch tensor")
+    if t.dtype not in _TENSOR_DTYPES:
+        raise ValueError(f"tensor {name!r} has dtype {t.dtype}; model tensors are float32, float64, uint8 or int32")
+    if not 1 <= t.dim() <= 4:
+        raise ValueError(f"tensor {name!r} has {t.dim()} dimensions; model tensors have 1 to 4")
+    if not t.is_contiguous():
+        raise ValueError(f"tensor {name!r} must be contiguous")
+    if t.numel() == 0 or t.numel() > _INT31:
+        raise ValueError(f"tensor {name!r} has {t.numel()} elements; model tensors have 1 to 2**31 - 1")
+    if t.device.type not in ("cuda", "meta"):
+        raise ValueError(f"tensor {name!r} must be a CUDA tensor (or a meta tensor standing in for one), got {t.device}")
 
 
 def resolve_fused_model(dynamics, running_cost, terminal_state_cost) -> Optional[AnalyticModel]:

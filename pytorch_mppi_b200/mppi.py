@@ -501,8 +501,9 @@ class MPPI:
             self._make_plan(p)
 
     def _fill_model_params(self, p):
-        """The model's current parameters into `p`; returns the host array `p.model_params_ext` points to (the caller
-        keeps it alive: the library reads it at plan creation / launch)."""
+        """The model's current parameters and device tensors into `p`; returns what `p` points to — the host array of
+        `p.model_params_ext`, and the tensor references with their tensors — which the caller keeps alive: the library
+        reads the arrays at plan creation / launch, and the kernels the tensors."""
         m = self._model
         blob = m.param_blob() if m is not None else []
         for i in range(_cabi.MPPI_MODEL_PARAM_DOUBLES):
@@ -511,18 +512,30 @@ class MPPI:
         arr = (C.c_double * len(ext))(*ext) if ext else None
         p.model_params_ext = None if arr is None else C.cast(arr, C.c_void_p)
         p.n_model_params_ext = len(ext)
-        return arr
+        refs = m.tensor_refs(self.d) if getattr(m, "tensors", None) else None
+        p.model_tensors = None if refs is None else C.cast(refs[0], C.c_void_p)
+        p.n_model_tensors = 0 if refs is None else len(refs[1])
+        return arr, refs
 
     def _take_model_params(self):
-        """`CudaModel.set_params` since this controller's last command: its plan takes the new values (no re-plan).
-        The struct is updated here, at command time, so that the intermediates of the previous command are still
-        materialised with the values they were computed with."""
+        """`CudaModel.set_params` / `set_tensors` since this controller's last command: its plan takes the new values
+        (no re-plan).  The struct is updated here, at command time, so that the intermediates of the previous command are
+        still materialised with the values they were computed with."""
         self._leave_resident()          # a resident grid holds the parameters it was launched with
+        old = self._ext_arr[1]
         self._ext_arr = self._fill_model_params(self._p)
         self._model_version = self._model._param_version
         p = self._p
         _cabi.check(self._lib.mppi_plan_set_model_params(self._plan, p.model_params, p.model_params_ext, p.n_model_params_ext),
                     "mppi_plan_set_model_params")
+        if p.n_model_tensors:
+            _cabi.check(self._lib.mppi_plan_set_model_tensors(self._plan, p.model_tensors, p.n_model_tensors),
+                        "mppi_plan_set_model_tensors")
+            # a swapped-out tensor may still be read by commands already queued: its memory is not reused before they ran
+            stream = torch.cuda.current_stream(self.d)
+            for t in old[1] if old is not None else ():
+                if not any(t is n for n in self._ext_arr[1][1]):
+                    t.record_stream(stream)
 
     def _make_plan(self, p):
         """Freeze the launch state in the C library (`mppi_plan_create`): per command only the state,
