@@ -102,10 +102,15 @@ enum {
     MPPI_FLAG_WIDE_REGS = 1u << 10,       /* retired (accepted and ignored; the bit stays reserved): round 1's opt-in
                                              instantiation without the 64-register cap.  The split-cost kernels have the
                                              whole register file anyway, the single-loop kernels of large K need the cap. */
-    MPPI_FLAG_SPLIT_COST = 1u << 9        /* small problems (threads_per_sample > 1): the rollout thread runs the bare state
+    MPPI_FLAG_SPLIT_COST = 1u << 9,       /* small problems (threads_per_sample > 1): the rollout thread runs the bare state
                                              recurrence, the sample's helper threads evaluate the T running costs in
                                              parallel from the stored states, summed in the reference's order (same
                                              operations and rounding as the single-loop rollout; see mppi_fused.cuh)  */
+    MPPI_FLAG_GLOBAL_TILE = 1u << 11      /* keep the noise tiles (and KMPPI's W / Wshift) in a per-CTA slice of the
+                                             workspace instead of shared memory: horizons whose tile does not fit.  Read
+                                             by mppi_fused_query, mppi_plan_create, mppi_sample_perturb,
+                                             mppi_softmin_update and mppi_materialize; single-loop kernels (split-cost
+                                             off), one GPU, not for resident mode or the PendulumMLP models           */
 };
 
 /* One `command()` of a registered analytic model: replaces, in one launch,
@@ -230,6 +235,8 @@ typedef struct MppiLaunchInfo {
                                     in direct mode, 1 = the rank's combined record); 0 = not sharded       */
     int32_t ll_tail;             /* 1 if the command runs the split-cost kernel specialised for one GPU in LL mode (every
                                     cluster record through this GPU's own mailbox): its softmin tail is inlined   */
+    int32_t global_tile;         /* 1 if the plan keeps its tiles in the workspace (MPPI_FLAG_GLOBAL_TILE); fills the
+                                    struct's trailing padding, so sizeof stays 64                           */
 } MppiLaunchInfo;
 
 int mppi_b200_abi_version(void);
@@ -241,7 +248,9 @@ const char* mppi_status_string(int status);
 const char* mppi_last_cuda_error(void);
 
 /* Launch geometry / scratch needs for these parameters (no launch).  With model == 0 (no fused model: the per-step
- * entry points further down) only sm_count and workspace_bytes are filled in. */
+ * entry points further down) only sm_count, workspace_bytes, global_tile and smem_bytes are filled in: smem_bytes is the
+ * larger dynamic shared memory of the sampling and softmin kernels' plans, 0 if either does not fit (then only
+ * MPPI_FLAG_GLOBAL_TILE runs these dimensions). */
 int mppi_fused_query(const MppiFusedParams* p, MppiLaunchInfo* out);
 /* The fused command (see struct comment) as a one-shot plan: mppi_plan_create, one command with the struct's state /
  * state_dev / flags / seed / offset / z / action_out / host_mailbox, mppi_plan_destroy.  `stream` is a cudaStream_t. */

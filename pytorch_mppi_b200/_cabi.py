@@ -37,6 +37,7 @@ FLAG_NOMINAL_PADDED = 1 << 7
 FLAG_PDL = 1 << 8
 FLAG_SPLIT_COST = 1 << 9
 FLAG_WIDE_REGS = 1 << 10
+FLAG_GLOBAL_TILE = 1 << 11
 
 STATUS = {0: "ok", -1: "bad argument", -2: "unsupported", -3: "workspace too small", -4: "CUDA error",
           -5: "ABI mismatch", -6: "peer exchange timeout"}
@@ -145,6 +146,7 @@ class MppiLaunchInfo(C.Structure):
         ("cluster_size", C.c_int32),
         ("xchg_records", C.c_int32),
         ("ll_tail", C.c_int32),
+        ("global_tile", C.c_int32),
     ]
 
 

@@ -208,11 +208,28 @@ static_assert(MPPI_RES_CMD_SHIFT == (unsigned)RES_CMD_SHIFT && MPPI_RES_CMD_STOP
 static_assert((int)RES_ERR_BAD_ARG == (int)MPPI_ERR_BAD_ARG && (int)RES_ERR_TIMEOUT == (int)MPPI_ERR_TIMEOUT, "status codes of the protocol header");
 
 // ---- generic path: sample / softmin -------------------------------------------------------------
+// MPPI_FLAG_GLOBAL_TILE: the global-tile kernels, whose tile slices follow the record mailbox in the workspace
+inline bool gtile_of(const MppiFusedParams* p) { return (p->flags & MPPI_FLAG_GLOBAL_TILE) != 0; }
+inline int check_gtile_workspace(const MppiFusedParams* p, const Geometry& g, int rows2) {
+    const uint64_t need = ws_bytes(g.nb, rows_of(p)) + ws_gtile_plan_bytes(p, g.nb, g.BS, rows2);
+    if (p->workspace == nullptr || p->workspace_bytes < need) return MPPI_ERR_WORKSPACE;
+    if (p->n_env > 1 && (p->env_ws_stride < need || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env)) return MPPI_ERR_WORKSPACE;
+    return MPPI_OK;
+}
+
+template <typename real, int V, int NU>
+int plan_sample(const MppiFusedParams* p, Geometry& g) {
+    if (!gtile_of(p)) return plan_geometry<real>(sample_kernel<real, V, NU>, p, V == V_KMPPI, false, g);
+    if (const char* why = gtile_refusal(nullptr, p)) return UNSUPPORTED(why);
+    int rc = plan_geometry<real>(sample_kernel_gtile<real, V, NU>, p, V == V_KMPPI, false, g, 0, true);
+    return rc ? rc : check_gtile_workspace(p, g, V == V_KMPPI);
+}
+
 template <typename real, int V, int NU>
 int run_sample(const MppiFusedParams* p, KArgs<real>& a_extra, cudaStream_t stream) {
-    auto kernel = sample_kernel<real, V, NU>;
+    auto kernel = gtile_of(p) ? sample_kernel_gtile<real, V, NU> : sample_kernel<real, V, NU>;
     Geometry g;
-    int rc = plan_geometry<real>(kernel, p, V == V_KMPPI, false, g);
+    int rc = plan_sample<real, V, NU>(p, g);
     if (rc) return rc;
     KArgs<real> a;
     fill_kargs<real>(p, a, g.BS, g.nb, g.tps);
@@ -265,17 +282,31 @@ int run_sample_any(const MppiFusedParams* p, void* pa, void* noise, void* noise_
     return MPPI_ERR_BAD_ARG;
 }
 
+// check_ws = false: the geometry alone (mppi_fused_query asks before the caller has a workspace)
 template <typename real, int V, int NU>
-int run_softmin(const MppiFusedParams* p, const void* cost, const void* eps, cudaStream_t stream) {
-    auto kernel = softmin_update_kernel<real, V, NU>;
+int plan_softmin(const MppiFusedParams* p, Geometry& g, bool check_ws = true) {
     // the warp-fold tail without clusters, one record per rank: its layout as softmin_update_kernel builds it
     const int xst = fused_xstage_doubles(sharded_in_kernel(p), p->world, 1, rows_of(p));
-    Geometry g;
-    int rc = plan_geometry<real>(kernel, p, layout_extra(0, 0, 1, xst), true, g, p->n_env > 1 ? (int)sizeof(KArgs<real>) : 0);
-    if (rc) return rc;
+    const int env_bytes = p->n_env > 1 ? (int)sizeof(KArgs<real>) : 0;
+    if (gtile_of(p)) {
+        if (const char* why = gtile_refusal(nullptr, p)) return UNSUPPORTED(why);
+        int rc = plan_geometry<real>(softmin_update_kernel_gtile<real, V, NU>, p, layout_extra(0, 0, 1, xst), true, g, env_bytes, true);
+        return rc ? rc : check_gtile_workspace(p, g, 0);
+    }
+    int rc = plan_geometry<real>(softmin_update_kernel<real, V, NU>, p, layout_extra(0, 0, 1, xst), true, g, env_bytes);
+    if (rc || !check_ws) return rc;
     const uint64_t need_ws = ws_bytes(g.nb, rows_of(p));
     if (p->workspace == nullptr || p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
     if (p->n_env > 1 && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env)) return MPPI_ERR_WORKSPACE;
+    return MPPI_OK;
+}
+
+template <typename real, int V, int NU>
+int run_softmin(const MppiFusedParams* p, const void* cost, const void* eps, cudaStream_t stream) {
+    auto kernel = gtile_of(p) ? softmin_update_kernel_gtile<real, V, NU> : softmin_update_kernel<real, V, NU>;
+    Geometry g;
+    int rc = plan_softmin<real, V, NU>(p, g);
+    if (rc) return rc;
     KArgs<real> a;
     fill_kargs<real>(p, a, g.BS, g.nb, g.tps);
     a.in_cost = (const real*)cost;
@@ -300,6 +331,30 @@ template <typename real> int run_softmin_any(const MppiFusedParams* p, const voi
         case MPPI_VARIANT_KMPPI: return run_softmin_nu<real, V_KMPPI>(p, c, e, s);
     }
     return MPPI_ERR_BAD_ARG;
+}
+
+// the larger dynamic shared memory of the sampling and softmin plans of these dimensions (mppi_fused_query, model == 0);
+// 0 if either does not fit
+template <typename real, int V, int NU> int stepped_smem(const MppiFusedParams* p) {
+    Geometry gs, gu;
+    if (plan_sample<real, V, NU>(p, gs) != MPPI_OK) return 0;
+    if (plan_softmin<real, V, NU>(p, gu, false) != MPPI_OK) return 0;
+    return gs.smem > gu.smem ? gs.smem : gu.smem;
+}
+template <typename real> int stepped_smem_any(const MppiFusedParams* p) {
+    const int V = p->variant, nu = p->nu;
+#define MPPI_STEPPED_SMEM_NU(VV)                                      \
+    switch (nu) {                                                      \
+        case 1: return stepped_smem<real, VV, 1>(p);                   \
+        case 2: return stepped_smem<real, VV, 2>(p);                   \
+        case 3: return stepped_smem<real, VV, 3>(p);                   \
+        case 4: return stepped_smem<real, VV, 4>(p);                   \
+    }
+    if (V == V_MPPI) { MPPI_STEPPED_SMEM_NU(V_MPPI) }
+    else if (V == V_SMPPI) { MPPI_STEPPED_SMEM_NU(V_SMPPI) }
+    else { MPPI_STEPPED_SMEM_NU(V_KMPPI) }
+#undef MPPI_STEPPED_SMEM_NU
+    return 0;
 }
 
 template <typename real, int V>
@@ -356,10 +411,18 @@ int mppi_fused_query(const MppiFusedParams* p, MppiLaunchInfo* out) {
     int rc = validate(p);
     if (rc) return rc;
     if (p->model == 0) {      // the per-step entry points: only the workspace mppi_softmin_update needs
+        if (gtile_of(p))
+            if (const char* why = gtile_refusal(nullptr, p)) return UNSUPPORTED(why);
         DevInfo di;
         if ((rc = get_dev_info(di)) != MPPI_OK) return rc;
         out->sm_count = di.sm_count;
         out->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p));
+        if (gtile_of(p)) {
+            out->workspace_bytes += ws_gtile_bytes(p, di.sm_count);
+            out->global_tile = 1;
+        } else {
+            out->smem_bytes = p->dtype == MPPI_F32 ? stepped_smem_any<float>(p) : stepped_smem_any<double>(p);
+        }
         return MPPI_OK;
     }
     if ((rc = validate(p, true)) != MPPI_OK) return rc;
@@ -486,6 +549,8 @@ int mppi_resident_start(void* plan, void* host_box, void* board_dev, void* actio
     Plan* pl = reinterpret_cast<Plan*>(plan);
     if (pl == nullptr || host_box == nullptr || board_dev == nullptr || action_out_dev == nullptr || idle_us == 0)
         return MPPI_ERR_BAD_ARG;
+    if (pl->p.flags & MPPI_FLAG_GLOBAL_TILE)
+        return UNSUPPORTED("resident mode keeps its tiles in shared memory: not available on a global-tile plan (tile_memory)");
     if (pl->res_kernel == nullptr)
         return UNSUPPORTED("resident mode needs a plan on the split-cost rollout (one tile per SM, one environment, single GPU)");
     if (pl->p.z_out != nullptr) return UNSUPPORTED("resident mode does not record the noise it draws (z_out)");
@@ -584,6 +649,20 @@ int mppi_user_model_register(const void* cubin, uint64_t cubin_bytes, int32_t nx
             return cuda_fail(e, "mppi_user_fused_command_kernel_ll");
         }
         mk.split_ll[variant] = (const void*)k;
+    }
+    // its global-tile kernels, exported under fixed names (MPPI_USER_KERNEL_GTILE / _BATCHED in mppi_fused.cuh)
+    const char* gnames[2] = {"mppi_user_fused_command_kernel_gtile", mk.batched != nullptr ? "mppi_user_fused_command_kernel_gtile_batched" : nullptr};
+    const void** gslots[2] = {&mk.gtile[variant], &mk.gtile_batched};
+    for (int i = 0; i < 2; ++i) {
+        if (gnames[i] == nullptr) continue;
+        cudaKernel_t k = nullptr;
+        cudaError_t e = cudaLibraryGetKernel(&k, lib, gnames[i]);
+        if (e != cudaSuccess) {
+            cudaLibraryUnload(lib);
+            delete h;
+            return cuda_fail(e, gnames[i]);
+        }
+        *gslots[i] = (const void*)k;
     }
     if (mk.fused[variant] == nullptr || mk.states == nullptr) {
         cudaLibraryUnload(lib);

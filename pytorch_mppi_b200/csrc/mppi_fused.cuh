@@ -127,8 +127,11 @@ __host__ __device__ inline int align_up(int x, int a) { return (x + a - 1) / a *
 // BD = threads per CTA, BS = samples per tile (BD / threads-per-sample)
 // `extra`: bit 0 = rows2 needed; bits 8.. = nx of the split-cost rollout's per-step state buffer xs[T*nx][BS]
 // (0 = none; see fused_command_kernel<..., SPLIT>)
+// gtile: the global-tile kernels (fused_command_kernel_gtile, sample_kernel_gtile, softmin_update_kernel_gtile) keep
+// the K-proportional buffers — rows, rows2 and KMPPI's W / Wshift — out of shared memory (gtile_bind)
 template <typename real>
-__host__ __device__ inline SmemLayout make_layout(int variant, int T, int nu, int S, int R, int BD, int BS, int nb, int extra) {
+__host__ __device__ inline SmemLayout make_layout(int variant, int T, int nu, int S, int R, int BD, int BS, int nb, int extra,
+                                                  bool gtile = false) {
     SmemLayout L;
     const int need_rows2 = extra & 1, nx_split = (extra >> 8) & 0xff, cluster = (extra >> 16) & 0xf, xstage = (extra >> 20) * 16;
     const int es = (int)sizeof(real);
@@ -140,11 +143,11 @@ __host__ __device__ inline SmemLayout make_layout(int variant, int T, int nu, in
     L.off_us = o; o = align_up(o + TN * es, 16);
     L.off_as = o; o = align_up(o + (variant == V_SMPPI ? TN : 0) * es, 16);
     L.off_ths = o; o = align_up(o + (variant == V_KMPPI ? SN : 0) * es, 16);
-    L.off_w = o; o = align_up(o + (variant == V_KMPPI ? T * S : 0) * es, 16);
-    L.off_wsh = o; o = align_up(o + (variant == V_KMPPI ? S * S : 0) * es, 16);
-    L.LD = BS + 1;
-    L.off_rows = o; o = align_up(o + R * L.LD * es, 16);
-    L.off_rows2 = o; o = align_up(o + (need_rows2 ? TN * L.LD : 0) * es, 16);
+    L.off_w = o; o = align_up(o + (variant == V_KMPPI && !gtile ? T * S : 0) * es, 16);
+    L.off_wsh = o; o = align_up(o + (variant == V_KMPPI && !gtile ? S * S : 0) * es, 16);
+    L.LD = gtile ? BS : BS + 1;      // (the +1 column staggers shared-memory banks; in global memory rows stay aligned)
+    L.off_rows = o; o = align_up(o + (gtile ? 0 : R * L.LD) * es, 16);
+    L.off_rows2 = o; o = align_up(o + (need_rows2 && !gtile ? TN * L.LD : 0) * es, 16);
     L.off_part2 = o; o = align_up(o + nw * R * 8, 16);
     L.off_numd = o; o = align_up(o + (R + 2) * 8, 16);
     L.off_xs = o; o = align_up(o + T * nx_split * BS * es, 16);
@@ -165,6 +168,15 @@ __host__ __device__ inline SmemLayout make_layout(int variant, int T, int nu, in
 }
 
 #define MPPI_XCHG_MAX_R 1024
+#define MPPI_LL_STAGE_BYTES 49152                          // finisher staging budget: LL mode needs xw x clusters x (R+2) x 8 <= this
+#define MPPI_LL_LOCAL_WORDS (2 * MPPI_LL_STAGE_BYTES / 8)  // words per parity of this GPU's own record mailbox (2 words per double)
+
+// ---- global-tile kernels: every CTA's tiles in the workspace ------------------------------------------------------------
+// The workspace is [ticket | cluster records | this GPU's record mailbox (two parities) | tile slices].  CTA b owns slice
+// b — rows (R x BS elements), then rows2 (TN x BS) where the kernel has one — and reuses it across its grid-stride tiles.
+__host__ __device__ inline long long gtile_slice_bytes(int R, int TN, int rows2, int BS, int es) {
+    return ((long long)(R + (rows2 ? TN : 0)) * BS * es + 255) / 256 * 256;
+}
 
 #if defined(__CUDACC__)
 
@@ -249,6 +261,20 @@ template <typename real> struct Smem {
     }
 };
 
+// global-tile kernels: point the tiles at this CTA's workspace slice (behind the record mailbox a.peers[0], which fill_kargs
+// and make_env_args place in this environment's workspace) and KMPPI's matrices at their global copies, read in place.
+// Only plain loads and stores reach the slice: it is written and read within the kernel, so never through ld.global.nc.
+template <typename real>
+__device__ __forceinline__ void gtile_bind(const KArgs<real>& a, Smem<real>& sm, int rows2) {
+    const int BS = blockDim.x / a.tps;
+    unsigned char* region = reinterpret_cast<unsigned char*>(a.peers[0]) + 2ull * MPPI_LL_LOCAL_WORDS * 8;
+    real* base = reinterpret_cast<real*>(region + (size_t)blockIdx.x * gtile_slice_bytes(a.R, a.TN, rows2, BS, (int)sizeof(real)));
+    sm.rows = base;
+    sm.rows2 = base + (size_t)a.R * BS;
+    sm.Ws = const_cast<real*>(a.W);
+    sm.Wsh = const_cast<real*>(a.Wshift);
+}
+
 // ---- stage 0: nominal sequence(s) into shared memory, shift folded in ----------------------------
 // stage_issue starts the (asynchronous) TMA bulk copy; stage_finish waits for it and builds the
 // shifted nominal.  The first tile's Philox draws run in between, hiding the global-memory latency.
@@ -277,6 +303,30 @@ __device__ void stage_issue(const KArgs<real>& a, Smem<real>& sm) {
         if (a.shift)
             for (int j = tid; j < S * S; j += BD) sm.Wsh[j] = a.Wshift[j];
     }
+}
+
+// stage_issue of the global-tile kernels: KMPPI's W / Wshift are read in place (gtile_bind), not staged
+template <typename real, int VARIANT, int NU>
+__device__ void stage_issue_gtile(const KArgs<real>& a, Smem<real>& sm) {
+    const int tid = threadIdx.x, BD = blockDim.x;
+    const int R = a.R, TN = a.TN;
+    if (tid == 0) mbar_init(sm.bar, 1);
+    __syncthreads();
+    if (a.tma_ok) {
+        if (tid == 0) {
+            const uint32_t bytes = (uint32_t)align_up(TN * (int)sizeof(real), 16);
+            mbar_expect_tx(sm.bar, VARIANT == V_SMPPI ? 2 * bytes : bytes);
+            tma_bulk_g2s(sm.Uraw, a.U, bytes, sm.bar);
+            if (VARIANT == V_SMPPI) tma_bulk_g2s(sm.Araw, a.A, bytes, sm.bar);
+        }
+    } else {
+        for (int j = tid; j < TN; j += BD) {
+            sm.Uraw[j] = a.U[j];
+            if (VARIANT == V_SMPPI) sm.Araw[j] = a.A[j];
+        }
+    }
+    if (VARIANT == V_KMPPI)
+        for (int j = tid; j < R; j += BD) sm.thraw[j] = a.theta[j];
 }
 
 template <typename real, int VARIANT, int NU>
@@ -317,7 +367,9 @@ __device__ void stage_nominal(const KArgs<real>& a, Smem<real>& sm) {
 // Philox chunks)
 // the rarely-taken sources of normals, out of line so that they do not sit in the hot path's instruction stream:
 // injected z (parity tests), the torch-compatible stream (one Philox call per element), recording of the draws (z_out)
-template <typename real>
+// G: instantiated separately for the global-tile kernels (their tile is in global memory): a shared copy of an out-of-line
+// function would lose the shared-memory stores the compiler gives it when every caller passes a shared-memory tile
+template <typename real, bool G = false>
 __device__ __noinline__ void fill_normals_rare(const KArgs<real>& a, real* rows, int LD, int tile, bool active, unsigned long long kg, int nvalid) {
     const int tid = threadIdx.x, BD = blockDim.x, R = a.R;
     const int BS = BD / a.tps, s_ = tid % BS, g_ = tid / BS;
@@ -342,7 +394,7 @@ __device__ __noinline__ void fill_normals_rare(const KArgs<real>& a, real* rows,
         }
     }
 }
-template <typename real>
+template <typename real, bool G = false>
 __device__ __noinline__ void record_normals(const KArgs<real>& a, const real* rows, int LD, int tile, int nvalid) {
     const int tid = threadIdx.x, BD = blockDim.x, R = a.R, BS = BD / a.tps;
     __syncthreads();
@@ -355,12 +407,12 @@ __device__ __noinline__ void record_normals(const KArgs<real>& a, const real* ro
     __syncthreads();
 }
 
-template <typename real>
+template <typename real, bool GTILE = false>
 __device__ void fill_normals(const KArgs<real>& a, Smem<real>& sm, int tile, bool active, unsigned long long kg, int nvalid) {
     const int tid = threadIdx.x, BD = blockDim.x, R = a.R, LD = sm.LD;
     const int BS = BD / a.tps, s_ = tid % BS, g_ = tid / BS;
     if (a.z != nullptr || a.torch_total > 0) {
-        fill_normals_rare<real>(a, sm.rows, LD, tile, active, kg, nvalid);
+        fill_normals_rare<real, GTILE>(a, sm.rows, LD, tile, active, kg, nvalid);
     } else if (active) {
         constexpr int PER = Normals<real>::PER_CALL;
         real* col = sm.rows + s_;
@@ -373,7 +425,7 @@ __device__ void fill_normals(const KArgs<real>& a, Smem<real>& sm, int tile, boo
                 if (c * PER + q < R) col[(c * PER + q) * LD] = tmp[q];
         }
     }
-    if (a.z_out != nullptr) record_normals<real>(a, sm.rows, LD, tile, nvalid);
+    if (a.z_out != nullptr) record_normals<real, GTILE>(a, sm.rows, LD, tile, nvalid);
 }
 
 // value that overrides the sampled action before the clamp: null action (mppi.py:390-392) or a
@@ -1317,7 +1369,7 @@ MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
 }
 
 // single_loop on the exact step and cost, out of line (as split_recurrence_rare)
-template <class Model, typename real, int VARIANT>
+template <class Model, typename real, int VARIANT, bool G = false>      // G: as fill_normals_rare
 __device__ __noinline__ RolloutCarry<real, Model::NX> single_loop_rare(const KArgs<real>& a, const typename Model::template P<real>& mp,
                                                                        const RolloutTiles<real> tiles, unsigned long long kg,
                                                                        RolloutCarry<real, Model::NX> c) {
@@ -1326,7 +1378,7 @@ __device__ __noinline__ RolloutCarry<real, Model::NX> single_loop_rare(const KAr
 }
 
 // the single-loop rollout of a model with a fast range: stores cost_total[k] and returns it
-template <class Model, typename real, int VARIANT>
+template <class Model, typename real, int VARIANT, bool GTILE = false>
 __device__ __forceinline__ real single_loop_rollout_fast(const KArgs<real>& a, const typename Model::template P<real>& mp,
                                                          const Smem<real>& sm, int k, unsigned long long kg) {
     typedef Ops<real> O;
@@ -1336,7 +1388,7 @@ __device__ __forceinline__ real single_loop_rollout_fast(const KArgs<real>& a, c
     c.pert = (real)0;
     c.smooth = (real)0;
     if (Model::template in_fast_range<real>(mp, c.x, a.T)) single_loop<Model, real, VARIANT, true>(a, mp, sm, kg, c);
-    else c = single_loop_rare<Model, real, VARIANT>(a, mp, RolloutTiles<real>(sm), kg, c);
+    else c = single_loop_rare<Model, real, VARIANT, GTILE>(a, mp, RolloutTiles<real>(sm), kg, c);
     if (Model::template has_terminal<real>(mp)) c.roll = O::add(c.roll, Model::template terminal<real>(mp, c.x));
     real c_tot = O::add(c.roll, c.pert);                                              // mppi.py:416
     if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(c.smooth, a.nm.w_smooth));  // mppi.py:562,569
@@ -1573,8 +1625,10 @@ template <class Model> struct FusedMinBlocks {
 template <> struct FusedMinBlocks<PendulumMLPModel> { static constexpr int value = 1; };
 
 // LL1: the tail of warp_tail<..., LL1 = true> (fused_command_kernel_ll below)
-template <class Model, typename real, int VARIANT, bool BATCHED, bool SPLIT, bool LL1>
+// GTILE: the tiles in this CTA's workspace slice (fused_command_kernel_gtile below; single loop only)
+template <class Model, typename real, int VARIANT, bool BATCHED, bool SPLIT, bool LL1, bool GTILE = false>
 __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, const typename Model::template P<real>& mp) {
+    static_assert(!(GTILE && (SPLIT || LL1)), "the global-tile kernel runs the single-loop rollout");
     typedef Ops<real> O;
     constexpr int NX = Model::NX, NU = Model::NU;
     extern __shared__ __align__(16) unsigned char smem[];
@@ -1586,8 +1640,9 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
     const int xst = fused_xstage_doubles(a.world > 1 && !a.export_partial, a.world, a.xchg_npub, a.R);
     const int cs_ = (int)cluster_nctarank(), NC_ = (int)gridDim.x / cs_;
     const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BS, fused_layout_nb(NC_, a.xchg_npub),
-                                           layout_extra(VARIANT != V_MPPI, SPLIT ? NX : 0, cs_, xst));
+                                           layout_extra(VARIANT != V_MPPI, SPLIT ? NX : 0, cs_, xst), GTILE);
     Smem<real> sm(smem, L);
+    if (GTILE) gtile_bind<real>(a, sm, VARIANT != V_MPPI);
     const NoiseModel<real>& nm = a.nm;
     const int T = a.T;
     warp_records_init<real>(a, sm);      // published by the barrier in stage_issue
@@ -1599,14 +1654,17 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
     // Programmatic dependent launch: this grid may be resident while the previous kernel on the stream is
     // still finishing.  Let our own successor start early too, draw the first tile's normals (pure
     // compute into shared memory), and only then wait for the predecessor's memory to be visible.
-    const bool early_fill = a.pdl && a.z == nullptr && a.z_out == nullptr && blockIdx.x < a.n_tiles;
+    // (GTILE: the first tile is global memory that the previous command's CTAs may still be folding from — nothing is
+    // written before the wait)
+    const bool early_fill = !GTILE && a.pdl && a.z == nullptr && a.z_out == nullptr && blockIdx.x < a.n_tiles;
     if (a.pdl) asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     if (early_fill) {
         const int k0 = blockIdx.x * BS + (tid % BS);
-        fill_normals<real>(a, sm, blockIdx.x, k0 < a.K, (unsigned long long)(a.k_offset + k0), min(BS, a.K - blockIdx.x * BS));
+        fill_normals<real, GTILE>(a, sm, blockIdx.x, k0 < a.K, (unsigned long long)(a.k_offset + k0), min(BS, a.K - blockIdx.x * BS));
     }
     if (a.pdl) asm volatile("griddepcontrol.wait;" ::: "memory");
-    stage_issue<real, VARIANT, NU>(a, sm);
+    if constexpr (GTILE) stage_issue_gtile<real, VARIANT, NU>(a, sm);
+    else stage_issue<real, VARIANT, NU>(a, sm);
     stamp(a.dbg, 1);
     bool staged = false;
 
@@ -1617,7 +1675,7 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
         const int nvalid = min(BS, a.K - tile * BS);
         const unsigned long long kg = (unsigned long long)(a.k_offset + k);
 
-        if (!(early_fill && tile == blockIdx.x)) fill_normals<real>(a, sm, tile, in_range, kg, nvalid);
+        if (!(early_fill && tile == blockIdx.x)) fill_normals<real, GTILE>(a, sm, tile, in_range, kg, nvalid);
         if (!staged) {   // the nominal sequence is first needed now; its TMA copy flew during the draws
             stage_finish<real, VARIANT, NU>(a, sm);
             staged = true;
@@ -1641,7 +1699,7 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
             // C''. M copies of the sample's rollout, interleaved in registers
             if (active) c_tot = copies_rollout<Model, real, VARIANT>(a, mp, sm, k, kg);
         } else if constexpr (FastRange<Model, real>::value) {
-            if (active) c_tot = single_loop_rollout_fast<Model, real, VARIANT>(a, mp, sm, k, kg);
+            if (active) c_tot = single_loop_rollout_fast<Model, real, VARIANT, GTILE>(a, mp, sm, k, kg);
         } else if (active) {
 
             // C. rollout (mppi.py:297-332) + action cost (mppi.py:409,415) [+ smoothness :559-562]
@@ -1727,6 +1785,14 @@ __global__ void __launch_bounds__(512, 1) fused_command_kernel_ll(const __grid_c
     fused_command_body<Model, real, VARIANT, false, true, true>(a_in, mp);
 }
 
+// The single-loop kernel with its tiles in the workspace (MPPI_FLAG_GLOBAL_TILE): horizons whose R x (BS+1) tile does not
+// fit in shared memory.  Same stages, same functions, same order of operations — only the tile pointers differ.
+template <class Model, typename real, int VARIANT, bool BATCHED>
+__global__ void __launch_bounds__(512, FusedMinBlocks<Model>::value) fused_command_kernel_gtile(
+    const __grid_constant__ KArgs<real> a_in, const __grid_constant__ typename Model::template P<real> mp) {
+    fused_command_body<Model, real, VARIANT, BATCHED, false, false, true>(a_in, mp);
+}
+
 #ifdef __CUDACC_RTC__
 // A user model (NVRTC, one module per dtype and controller variant) exports its fused_command_kernel_ll under one unmangled
 // name, which mppi_user_model_register looks up beside the kernels it is given by name.
@@ -1735,14 +1801,28 @@ __global__ void __launch_bounds__(512, 1) fused_command_kernel_ll(const __grid_c
         const __grid_constant__ mppi::KArgs<real> a_in, const __grid_constant__ Model::P<real> mp) {                         \
         mppi::fused_command_body<Model, real, VARIANT, false, true, true>(a_in, mp);                                         \
     }
+// ... and its global-tile kernels (mppi_user_model_register looks them up by these names): the single-loop kernel, and for
+// MPPI_Batched (MPPI variant, one copy) the batched one
+#define MPPI_USER_KERNEL_GTILE(Model, real, VARIANT)                                                                         \
+    extern "C" __global__ void __launch_bounds__(512, mppi::FusedMinBlocks<Model>::value) mppi_user_fused_command_kernel_gtile( \
+        const __grid_constant__ mppi::KArgs<real> a_in, const __grid_constant__ Model::P<real> mp) {                         \
+        mppi::fused_command_body<Model, real, VARIANT, false, false, false, true>(a_in, mp);                                 \
+    }
+#define MPPI_USER_KERNEL_GTILE_BATCHED(Model, real)                                                                          \
+    extern "C" __global__ void __launch_bounds__(512, mppi::FusedMinBlocks<Model>::value)                                    \
+        mppi_user_fused_command_kernel_gtile_batched(const __grid_constant__ mppi::KArgs<real> a_in,                         \
+                                                     const __grid_constant__ Model::P<real> mp) {                            \
+        mppi::fused_command_body<Model, real, mppi::V_MPPI, true, false, false, true>(a_in, mp);                             \
+    }
 #endif
 
 // =================================================================================================
 // Generic path, part 1: sample + perturb with coalesced write-out (mppi.py:375-385, 409, 415;
 // SMPPI :539-562; KMPPI :657-670).  Also used to materialise noise/perturbed_action lazily.
 // =================================================================================================
-template <typename real, int VARIANT, int NU>
-__global__ void __launch_bounds__(512) sample_kernel(const __grid_constant__ KArgs<real> a_in) {
+// GTILE: the tiles in this CTA's workspace slice (sample_kernel_gtile)
+template <typename real, int VARIANT, int NU, bool GTILE>
+__device__ __forceinline__ void sample_body(const KArgs<real>& a_in) {
     typedef Ops<real> O;
     extern __shared__ __align__(16) unsigned char smem[];
     const int tid = threadIdx.x, BD = blockDim.x;
@@ -1750,12 +1830,18 @@ __global__ void __launch_bounds__(512) sample_kernel(const __grid_constant__ KAr
     if (a_in.n_env > 1) make_env_args<real, 0, NU>(a_in, reinterpret_cast<KArgs<real>*>(a_env_raw));
     const KArgs<real>& a = a_in.n_env > 1 ? *reinterpret_cast<const KArgs<real>*>(a_env_raw) : a_in;
     const int BS = BD / a.tps;
-    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BS, 1, VARIANT == V_KMPPI);
+    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BS, 1, VARIANT == V_KMPPI, GTILE);
     Smem<real> sm(smem, L);
+    if (GTILE) gtile_bind<real>(a, sm, VARIANT == V_KMPPI);
     const NoiseModel<real>& nm = a.nm;
     const int T = a.T, R = a.R, TN = a.TN, LD = sm.LD;
 
-    stage_nominal<real, VARIANT, NU>(a, sm);
+    if constexpr (GTILE) {
+        stage_issue_gtile<real, VARIANT, NU>(a, sm);
+        stage_finish<real, VARIANT, NU>(a, sm);
+    } else {
+        stage_nominal<real, VARIANT, NU>(a, sm);
+    }
     if (blockIdx.x == 0 && a.nominal_used != nullptr) {
         for (int j = tid; j < TN; j += BD) {
             a.nominal_used[j] = sm.Us[j];
@@ -1771,7 +1857,7 @@ __global__ void __launch_bounds__(512) sample_kernel(const __grid_constant__ KAr
         const bool active = in_range && tid < BS;
         const int nvalid = min(BS, a.K - tile * BS);
         const unsigned long long kg = (unsigned long long)(a.k_offset + k);
-        fill_normals<real>(a, sm, tile, in_range, kg, nvalid);
+        fill_normals<real, GTILE>(a, sm, tile, in_range, kg, nvalid);
         if (a.tps > 1) __syncthreads();
         if (in_range) transform_column<real, VARIANT, NU>(a, sm, kg);
         if (a.tps > 1) __syncthreads();
@@ -1836,6 +1922,14 @@ __global__ void __launch_bounds__(512) sample_kernel(const __grid_constant__ KAr
         __syncthreads();
     }
 }
+template <typename real, int VARIANT, int NU>
+__global__ void __launch_bounds__(512) sample_kernel(const __grid_constant__ KArgs<real> a_in) {
+    sample_body<real, VARIANT, NU, false>(a_in);
+}
+template <typename real, int VARIANT, int NU>
+__global__ void __launch_bounds__(512) sample_kernel_gtile(const __grid_constant__ KArgs<real> a_in) {
+    sample_body<real, VARIANT, NU, true>(a_in);
+}
 
 // states along the rollout of given perturbed actions (mppi.py:307-322), for registered models.
 // pa_stride = elements between consecutive samples' action sequences: T*nu for a (K,T,nu) tensor, 0 when every
@@ -1887,21 +1981,23 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
 // GPU, rank-record mode on a sharded controller.  Never LL mode: a single-GPU stepped command does not advance the
 // record epoch, and CUDA-graph replays repeat one, so LL records of the previous command would pass for this one's.
 // =================================================================================================
-template <typename real, int VARIANT, int NU>
-__global__ void __launch_bounds__(512) softmin_update_kernel(const __grid_constant__ KArgs<real> a_in) {
+// GTILE: the tile in this CTA's workspace slice (softmin_update_kernel_gtile)
+template <typename real, int VARIANT, int NU, bool GTILE>
+__device__ __forceinline__ void softmin_update_body(const KArgs<real>& a_in) {
     typedef Ops<real> O;
     extern __shared__ __align__(16) unsigned char smem[];
     const int tid = threadIdx.x, BD = blockDim.x;
     const int BS = BD / a_in.tps;
     const int xst = fused_xstage_doubles(a_in.world > 1 && !a_in.export_partial, a_in.world, 1, a_in.R);
     const SmemLayout L = make_layout<real>(VARIANT, a_in.T, NU, a_in.S, a_in.R, BD, BS, fused_layout_nb(gridDim.x, 1),
-                                           layout_extra(0, 0, 1, xst));
+                                           layout_extra(0, 0, 1, xst), GTILE);
     // batched environments: the per-environment argument view sits behind the layout (the host adds its size), so that
     // one environment pays no shared memory for it and this kernel plans every horizon the fused kernel does
     KArgs<real>* a_env = reinterpret_cast<KArgs<real>*>(smem + L.total);
     if (a_in.n_env > 1) make_env_args<real, 0, NU>(a_in, a_env);
     const KArgs<real>& a = a_in.n_env > 1 ? *a_env : a_in;
     Smem<real> sm(smem, L);
+    if (GTILE) gtile_bind<real>(a, sm, 0);
     const int R = a.R, TN = a.TN, LD = sm.LD;
     warp_records_init<real>(a, sm);
     // post-shift nominal comes from nominal_used (written by sample_kernel)
@@ -1911,7 +2007,8 @@ __global__ void __launch_bounds__(512) softmin_update_kernel(const __grid_consta
     }
     if (VARIANT == V_KMPPI) {
         for (int j = tid; j < R; j += BD) sm.ths[j] = a.nominal_used[2 * TN + j];
-        for (int j = tid; j < a.T * a.S; j += BD) sm.Ws[j] = a.W[j];
+        if (!GTILE)
+            for (int j = tid; j < a.T * a.S; j += BD) sm.Ws[j] = a.W[j];
     }
     for (int tile = blockIdx.x; tile < a.n_tiles; tile += gridDim.x) {
         const int k = tile * BS + tid;
@@ -1929,6 +2026,14 @@ __global__ void __launch_bounds__(512) softmin_update_kernel(const __grid_consta
         if (tid < BS) warp_fold<real, VARIANT, false, true>(a, sm, c, active, nvalid);
     }
     warp_tail<real, VARIANT, NU>(a, sm);
+}
+template <typename real, int VARIANT, int NU>
+__global__ void __launch_bounds__(512) softmin_update_kernel(const __grid_constant__ KArgs<real> a_in) {
+    softmin_update_body<real, VARIANT, NU, false>(a_in);
+}
+template <typename real, int VARIANT, int NU>
+__global__ void __launch_bounds__(512) softmin_update_kernel_gtile(const __grid_constant__ KArgs<real> a_in) {
+    softmin_update_body<real, VARIANT, NU, true>(a_in);
 }
 
 // omega_k = exp(-(c_k - beta)/lambda) / eta from the stats a command left behind (mppi.py:256-258)

@@ -43,12 +43,25 @@ inline bool select_tensor_core_route(const ModelKernels* mk, const MppiFusedPara
 //              their staging (world x clusters x (R+2) doubles) is small (direct mode), else its one combined record
 //   ll         split-cost plans of one GPU whose clusters all publish to its own mailbox (LL mode) run
 //              fused_command_kernel_ll, the instantiation whose tail is that one path, inlined (mppi_fused.cuh, warp_tail)
+//   gtile      MPPI_FLAG_GLOBAL_TILE: fused_command_kernel_gtile, tiles in per-CTA workspace slices — single loop, one GPU,
+//              no clusters (the padded grid of a cluster would outgrow the slices ws_gtile_bytes sizes), and ticket mode
+//              where the finisher's LL staging does not fit next to the (R+2)-sized records
 struct FusedChoice {
     const void* kernel;
     Geometry g;
     int split;
     int ll;
+    int gtile;
 };
+
+// the reasons a global-tile plan is refused, before any CUDA call (nullptr: none)
+inline const char* gtile_refusal(const ModelKernels* mk, const MppiFusedParams* p) {
+    if (mk != nullptr && mk->is_mlp)
+        return "global-tile plans: the PendulumMLP kernels fix their own tiles (tile_memory='shared' only)";
+    if (p->world > 1 || (p->flags & MPPI_FLAG_EXPORT_PARTIAL))
+        return "global-tile plans: not available on sharded controllers (the peer mailbox caps T*nu at 1024)";
+    return nullptr;
+}
 
 // the rank records of a command are exchanged with peers inside the kernel (else they stay in this GPU's own mailbox)
 inline bool sharded_in_kernel(const MppiFusedParams* p) {
@@ -63,9 +76,13 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     const int V = p->variant;
     const bool batched = p->n_env > 1;
     if (batched && (V != V_MPPI || p->world > 1)) return UNSUPPORTED("batched environments: MPPI variant, single GPU only");
-    const void* kernel = batched ? mk->batched : mk->fused[V];
+    const bool gtile = (p->flags & MPPI_FLAG_GLOBAL_TILE) != 0;
+    if (gtile) {
+        if (const char* why = gtile_refusal(mk, p)) return UNSUPPORTED(why);
+    }
+    const void* kernel = gtile ? (batched ? mk->gtile_batched : mk->gtile[V]) : (batched ? mk->batched : mk->fused[V]);
     if (kernel == nullptr) return UNSUPPORTED("this model was built without the kernel of this controller variant");
-    const bool tc_route = select_tensor_core_route(mk, p, p_tc, kernel);
+    const bool tc_route = !gtile && select_tensor_core_route(mk, p, p_tc, kernel);
     if (tc_route) p = &p_tc;
     const int R = rows_of(p);
     const int world = p->world <= 0 ? 1 : p->world;
@@ -79,10 +96,10 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     const int tile2 = V != V_MPPI && !tc_route;
     // the ensemble's tensor-core kernel keeps every copy's network and step buffers behind the layout
     const int ens_bytes = tc_route && mk->is_mlp == 2 ? PendulumMLPEnsembleModel::tc_smem_bytes(p->rollout_samples) : 0;
-    rc = plan_geometry<real>(kernel, &pg, layout_extra(tile2, 0, 1, xst1), false, g, ens_bytes);
+    rc = plan_geometry<real>(kernel, &pg, layout_extra(tile2, 0, 1, xst1), false, g, ens_bytes, gtile);
     if (rc) return rc;
     int split = 0;
-    if (mk->split[V] != nullptr) {      // (the MLP has none: its step is the network, the cost is nothing)
+    if (mk->split[V] != nullptr && !gtile) {      // (the MLP has none: its step is the network, the cost is nothing)
         if (!batched && (p->flags & MPPI_FLAG_SPLIT_COST) && g.tps > 1) {
             const void* k2 = mk->split[V];
             MppiFusedParams p2 = pg;
@@ -113,6 +130,7 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
     g.npub = 1;
     for (int cs = 8; cs >= 1; cs >>= 1) {
         if (cs > want && cs > 1) continue;
+        if (gtile && cs > 1) continue;
         const int nbp = (g.nb + cs - 1) / cs * cs;
         if (cs > 2 && nbp > di.sm_count) continue;                        // 8 / 4: one wave of at most one CTA per SM (pairs pack anywhere)
         if (cs > 1 && (g.nb < 2 || nbp > di.sm_count * g.occ)) continue;
@@ -123,13 +141,19 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
         if (NC > 1 && (long long)xw * NC * (R + 2) * 8 <= MPPI_LL_STAGE_BYTES) npub = NC;
         if (const char* e = getenv("MPPI_B200_XCHG_DIRECT"))
             if (atoi(e) == 0) npub = 1;
-        const int xst = fused_xstage_doubles(sharded, world, npub, R);
+        int xst = fused_xstage_doubles(sharded, world, npub, R);
         const void* kc = may_ll && NC > 1 && npub == NC ? mk->split_ll[V] : kernel;
         CK(cudaFuncGetAttributes(&fa, kc));
         const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;
         if (kc != kernel) CK(cudaFuncSetAttribute(kc, cudaFuncAttributeMaxDynamicSharedMemorySize, dyn_limit));
-        const int smem = make_layout<real>(p->variant, p->T, p->nu, p->S, R, g.BD, g.BS, fused_layout_nb(NC, npub),
-                                           layout_extra(tile2, split ? mk->nx : 0, cs, xst)).total + ens_bytes;
+        int smem = make_layout<real>(p->variant, p->T, p->nu, p->S, R, g.BD, g.BS, fused_layout_nb(NC, npub),
+                                     layout_extra(tile2, split ? mk->nx : 0, cs, xst), gtile).total + ens_bytes;
+        if (gtile && smem > dyn_limit && npub > 1) {       // ticket mode: the cluster records stay in the L2 workspace
+            npub = 1;
+            xst = fused_xstage_doubles(sharded, world, npub, R);
+            smem = make_layout<real>(p->variant, p->T, p->nu, p->S, R, g.BD, g.BS, fused_layout_nb(NC, npub),
+                                     layout_extra(tile2, 0, cs, xst), true).total;
+        }
         if (smem > dyn_limit) continue;
         if (cs > 1) {
             cudaLaunchConfig_t cfg;
@@ -152,8 +176,10 @@ int choose_fused(const ModelKernels* mk, const MppiFusedParams*& p, MppiFusedPar
         chosen = kc;
         break;
     }
-    if (g.cluster == 0) return UNSUPPORTED("shared-memory tile does not fit");
-    c = FusedChoice{chosen, g, split, chosen != kernel};
+    if (g.cluster == 0)
+        return gtile ? UNSUPPORTED("global-tile plan: the per-CTA vectors (nominal sequence, softmin records) do not fit in shared memory")
+                     : UNSUPPORTED("shared-memory tile does not fit");
+    c = FusedChoice{chosen, g, split, chosen != kernel, gtile ? 1 : 0};
     return MPPI_OK;
 }
 
@@ -180,12 +206,13 @@ template <typename real> int query_fused(const ModelKernels* mk, const MppiFused
     info->regs_per_thread = g.regs;
     info->max_blocks_per_sm = g.occ;
     info->sm_count = di.sm_count;
-    info->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p));
+    info->workspace_bytes = ws_bytes(max_planned_grid(p, di.sm_count), rows_of(p)) + (c.gtile ? ws_gtile_bytes(p, di.sm_count) : 0);
     info->tma_staging = a.tma_ok;
     info->split_cost = c.split;
     info->cluster_size = g.cluster;
     info->xchg_records = g.npub;
     info->ll_tail = c.ll;
+    info->global_tile = c.gtile;
     return MPPI_OK;
 }
 
@@ -200,7 +227,7 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
     pl->g = c.g;
     if (p->U == nullptr || p->cost_total == nullptr || p->nominal_used == nullptr || p->stats == nullptr || p->workspace == nullptr)
         return MPPI_ERR_BAD_ARG;
-    const uint64_t need_ws = ws_bytes(pl->g.nb, rows_of(p));
+    const uint64_t need_ws = ws_bytes(pl->g.nb, rows_of(p)) + (c.gtile ? ws_gtile_plan_bytes(p, pl->g.nb, pl->g.BS, V != V_MPPI) : 0);
     if (p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
     if (batched && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env ||
                     p->env_u_stride < p->T * p->nu))

@@ -79,6 +79,8 @@ struct ModelKernels {
     const void* resident[3];         // resident_command_kernel<Model, real, V> (nullptr: not available)
     const void* resident_stamped;    // the one instantiation with %globaltimer stamps, or nullptr
     const void* states;              // states_kernel<Model, real>
+    const void* gtile[3];            // fused_command_kernel_gtile<Model, real, V, false> (nullptr: not available)
+    const void* gtile_batched;       // fused_command_kernel_gtile<Model, real, V_MPPI, true>
     const void* tc[3][2][2];         // mlp_tc_command_kernel<V, SPLIT = 2 - mode, FAST>, [V][mode - 1][fast]; fp32 MLP only
                                      // (the ensemble: mlp_ens_tc_command_kernel)
     void* library;                   // run-time user models: the cudaLibrary_t that owns the kernels
@@ -188,8 +190,8 @@ template <typename real> void fill_noise_model(const MppiFusedParams* p, NoiseMo
 
 // ticket + the records of the warp-fold tail's ticket mode: one of (R + 2) doubles per cluster (at most one per CTA)
 // ... followed by this GPU's own record mailbox (single-GPU LL mode): two epoch parities of MPPI_LL_LOCAL_WORDS flagged words
-#define MPPI_LL_STAGE_BYTES 49152                          // finisher staging budget: LL mode needs xw x clusters x (R+2) x 8 <= this
-#define MPPI_LL_LOCAL_WORDS (2 * MPPI_LL_STAGE_BYTES / 8)  // words per parity of the local mailbox (2 words per double)
+// (MPPI_LL_STAGE_BYTES / MPPI_LL_LOCAL_WORDS: mppi_fused.cuh)
+// ... followed, for the global-tile kernels, by one tile slice per CTA (gtile_slice_bytes; ws_gtile_bytes below)
 inline uint64_t ws_partials_bytes(int nb, int R) { return (16 + (uint64_t)nb * (uint64_t)(R + 2) * 8 + 255) / 256 * 256; }
 inline uint64_t ws_bytes(int nb, int R) { return ws_partials_bytes(nb, R) + 2ull * MPPI_LL_LOCAL_WORDS * 8; }
 
@@ -202,6 +204,29 @@ inline int max_planned_grid(const MppiFusedParams* p, int sm_count) {
     const long long tiles = (K + 31) / 32, cap = (long long)sm_count * MPPI_MAX_CTAS_PER_SM;
     const long long nb = tiles < cap ? tiles : cap;
     return (int)((nb + 7) / 8 * 8);
+}
+
+// Global-tile plans: the samples whose tiles are in flight at once (grid x samples per tile) are capped at
+// MPPI_GTILE_SAMPLES_PER_SM per SM, so the tile slices stay bounded at large K (a grid-stride CTA reuses its slice).
+#define MPPI_GTILE_SAMPLES_PER_SM 128
+inline int gtile_grid_cap(int sm_count, int BS) {
+    const int nb = sm_count * MPPI_GTILE_SAMPLES_PER_SM / BS;
+    return nb > 1 ? nb : 1;
+}
+// The tile slices of any global-tile plan of these dimensions (per environment): at most min(K + 511, cap) samples in
+// flight, one slice per CTA of at least 32 samples.  rows2 (T*nu per sample) only where a kernel of the variant has it:
+// SMPPI (fused) and KMPPI (fused and sampling); MPPI's slices hold `rows` alone.
+inline uint64_t ws_gtile_bytes(const MppiFusedParams* p, int sm_count) {
+    const long long K = p->K_geom > p->K ? p->K_geom : p->K;
+    long long n = (long long)sm_count * MPPI_GTILE_SAMPLES_PER_SM;
+    if (K + 511 < n) n = K + 511;
+    const int es = p->dtype == MPPI_F64 ? 8 : 4;
+    const long long per_sample = rows_of(p) + (p->variant != MPPI_VARIANT_MPPI ? (long long)p->T * p->nu : 0);
+    return (uint64_t)n * (uint64_t)per_sample * es + (uint64_t)(n / 32 + 1) * 256;
+}
+// ... and the slices of a planned grid
+inline uint64_t ws_gtile_plan_bytes(const MppiFusedParams* p, int nb, int BS, int rows2) {
+    return (uint64_t)nb * (uint64_t)gtile_slice_bytes(rows_of(p), p->T * p->nu, rows2, BS, p->dtype == MPPI_F64 ? 8 : 4);
 }
 
 inline unsigned long long xchg_timeout_ns() {
@@ -359,9 +384,10 @@ struct GeomKey {
 // grid_records: the kernel's finisher rescales one record per CTA of the grid (the warp-fold tail in ticket mode without
 // clusters: softmin_update_kernel), so the layout grows with the grid; the fused routes size their final layout themselves.
 // extra_bytes: dynamic shared memory the kernel uses behind the layout (the ensemble wgmma kernel's per-copy tiles).
+// gtile: a global-tile kernel (layout without the tiles, grid capped by gtile_grid_cap)
 template <typename real, typename KernelT>
 int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool grid_records, Geometry& g,
-                  int extra_bytes = 0) {
+                  int extra_bytes = 0, bool gtile = false) {
     static thread_local GeomKey keys[8];
     static thread_local Geometry vals[8];
     static thread_local int n_cached = 0, next_slot = 0;
@@ -402,7 +428,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         // shared memory (the R x (BS+1) noise tile of long horizons at nu = 3..4), so no geometry that fits changes
         auto next_bs = [&](int bs) { return bs == 32 ? 0 : bs < 512 ? bs + (bs < 128 ? 64 : 32) : (best_load < 0 ? 32 : 0); };
         for (int bs = 64; bs != 0; bs = next_bs(bs)) {
-            SmemLayout Lc = make_layout<real>(p->variant, p->T, p->nu, p->S, R, bs, bs, grid_records ? di.sm_count * 4 : 1, need_rows2);
+            SmemLayout Lc = make_layout<real>(p->variant, p->T, p->nu, p->S, R, bs, bs, grid_records ? di.sm_count * 4 : 1, need_rows2, gtile);
             Lc.total += extra_bytes;
             if (Lc.total > dyn0) continue;
             int occ_c = 0;
@@ -410,7 +436,8 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
             if (occ_c < 1) continue;
             const int nt = (p->K + bs - 1) / bs;
             for (int j = 1; j <= occ_c && j <= 8; ++j) {
-                const int nbc = nt < di.sm_count * j ? nt : di.sm_count * j;
+                int nbc = nt < di.sm_count * j ? nt : di.sm_count * j;
+                if (gtile && nbc > gtile_grid_cap(di.sm_count, bs)) nbc = gtile_grid_cap(di.sm_count, bs);   // as below
                 const int passes = (nt + nbc - 1) / nbc;
                 const int bps = (nbc + di.sm_count - 1) / di.sm_count;
                 long long load = (long long)bps * passes * bs;
@@ -431,12 +458,13 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
     }
     if (BS % 32 != 0 || BS < 32 || BS > 512) return MPPI_ERR_BAD_ARG;
     const int n_tiles = (p->K + BS - 1) / BS;
-    const int cap = di.sm_count * MPPI_MAX_CTAS_PER_SM;     // workspaces are sized for it: max_planned_grid
+    int cap = di.sm_count * MPPI_MAX_CTAS_PER_SM;     // workspaces are sized for it: max_planned_grid
     cudaFuncAttributes fa;
     CK(cudaFuncGetAttributes(&fa, kernel));
     const int dyn_limit = di.max_smem_optin - (int)fa.sharedSizeBytes;   // static + dynamic <= opt-in maximum
     // The layout may depend on the grid (grid_records: one rescale factor per CTA in shared memory) and the
     // grid on the occupancy the layout allows: iterate from an optimistic guess to a fixed point.
+    if (gtile && gtile_grid_cap(di.sm_count, BS) < cap) cap = gtile_grid_cap(di.sm_count, BS);
     int nb = n_tiles < cap ? n_tiles : cap;
     if (tps <= 0) {
         // helper threads only pay off while an SM hosts a single small CTA
@@ -446,7 +474,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         // each helper thread's warp adds per-warp partial rows to the tile: fewer helpers where all of them do not fit
         // (the optimistic grid's layout is the largest of the fixed-point iteration below)
         while (tps > 1 && BS * tps > 64 && make_layout<real>(p->variant, p->T, p->nu, p->S, R, BS * tps, BS,
-                                                             grid_records ? nb : 1, need_rows2).total + extra_bytes > dyn_limit)
+                                                             grid_records ? nb : 1, need_rows2, gtile).total + extra_bytes > dyn_limit)
             tps >>= 1;
     }
     while (tps > 1 && BS * tps > 512) tps >>= 1;
@@ -461,9 +489,11 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
     int occ = 0;
     SmemLayout L;
     for (int it = 0; it < 4; ++it) {
-        L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, grid_records ? nb : 1, need_rows2);
+        L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, grid_records ? nb : 1, need_rows2, gtile);
         L.total += extra_bytes;
-        if (L.total > dyn_limit) return UNSUPPORTED("shared-memory tile does not fit");
+        if (L.total > dyn_limit)
+            return gtile ? UNSUPPORTED("global-tile plan: the per-CTA vectors (nominal sequence, softmin records) do not fit in shared memory")
+                         : UNSUPPORTED("shared-memory tile does not fit");
         CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, BD, L.total));
         if (occ < 1) return UNSUPPORTED("kernel does not fit on an SM with this block size");
         int nb2 = n_tiles < di.sm_count * occ ? n_tiles : di.sm_count * occ;
@@ -473,7 +503,7 @@ int plan_geometry(KernelT kernel, const MppiFusedParams* p, int need_rows2, bool
         if (nb2 == nb) break;
         nb = nb2;
     }
-    L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, grid_records ? nb : 1, need_rows2);
+    L = make_layout<real>(p->variant, p->T, p->nu, p->S, R, BD, BS, grid_records ? nb : 1, need_rows2, gtile);
     L.total += extra_bytes;
     g.BS = BS;
     g.tps = tps;

@@ -76,6 +76,15 @@ const void* stamped_resident_kernel() {
     if constexpr (MPPI_TU_MODEL == 1 && !MPPI_TU_F64) return (const void*)resident_command_kernel<TuModel, TuReal, V_MPPI, true>;
     else return nullptr;
 }
+// global-tile kernels (MPPI_FLAG_GLOBAL_TILE): not for the MLP models, whose kernels fix their own tiles
+template <int V> const void* gtile_kernel() {
+    if constexpr (kIsMlp || kIsEnsemble) return nullptr;
+    else return (const void*)fused_command_kernel_gtile<TuModel, TuReal, V, false>;
+}
+const void* gtile_batched_kernel() {
+    if constexpr (kIsMlp || kIsEnsemble) return nullptr;
+    else return (const void*)fused_command_kernel_gtile<TuModel, TuReal, V_MPPI, true>;
+}
 template <int V, int SPLIT, int FAST> const void* tc_kernel() {
     if constexpr (kIsMlp && !MPPI_TU_F64) return (const void*)mlp_tc_command_kernel<V, SPLIT, FAST>;
     else if constexpr (kIsEnsemble && !MPPI_TU_F64) return (const void*)mlp_ens_tc_command_kernel<V, SPLIT, FAST>;
@@ -92,6 +101,8 @@ const ModelKernels g_kernels = {
     {resident_kernel<V_MPPI>(), resident_kernel<V_SMPPI>(), resident_kernel<V_KMPPI>()},
     stamped_resident_kernel(),
     (const void*)states_kernel<TuModel, TuReal>,
+    {gtile_kernel<V_MPPI>(), gtile_kernel<V_SMPPI>(), gtile_kernel<V_KMPPI>()},
+    gtile_batched_kernel(),
     {{{tc_kernel<V_MPPI, 1, 0>(), tc_kernel<V_MPPI, 1, 1>()}, {tc_kernel<V_MPPI, 0, 0>(), tc_kernel<V_MPPI, 0, 1>()}},
      {{tc_kernel<V_SMPPI, 1, 0>(), tc_kernel<V_SMPPI, 1, 1>()}, {tc_kernel<V_SMPPI, 0, 0>(), tc_kernel<V_SMPPI, 0, 1>()}},
      {{tc_kernel<V_KMPPI, 1, 0>(), tc_kernel<V_KMPPI, 1, 1>()}, {tc_kernel<V_KMPPI, 0, 0>(), tc_kernel<V_KMPPI, 0, 1>()}}},

@@ -34,6 +34,7 @@ logger = logging.getLogger(__name__)
 
 _DT = {torch.float32: _cabi.F32, torch.float64: _cabi.F64}
 _ES = {torch.float32: 4, torch.float64: 8}
+_TILE_MEMORY = ("shared", "global", "auto")
 
 
 class SpecificActionSampler:
@@ -126,7 +127,10 @@ class MPPI:
                  block_threads: int = 0,
                  threads_per_sample: int = 0,
                  process_group=None,
-                 exchange: str = "p2p"):
+                 exchange: str = "p2p",
+                 tile_memory: str = "shared"):
+        if tile_memory not in _TILE_MEMORY:
+            raise ValueError(f"tile_memory must be one of {_TILE_MEMORY}, got {tile_memory!r}")
         self._lib = _cabi.load()          # raises if the CUDA library is not built
         self.d = torch.device(device)
         if self.d.type != "cuda":
@@ -200,6 +204,16 @@ class MPPI:
         if rng not in ("philox", "torch"):
             raise ValueError("rng must be 'philox' (one subsequence per sample) or 'torch' (the stream torch.randn draws on CUDA)")
         self._rng_mode = rng
+        # where the noise tiles live: "shared" (shared memory; horizons up to its edge), "global" (a per-CTA slice of the
+        # workspace, any horizon up to T*nu = 2048), "auto" (shared wherever it fits, else global)
+        self._tile_memory = tile_memory
+        if tile_memory != "shared":
+            if process_group is not None:
+                raise ValueError("tile_memory='global' / 'auto' is not available on sharded controllers "
+                                 "(the peer mailbox caps T*nu at 1024)")
+            if self._model is not None and self._model.model_id in (_cabi.MODEL_PENDULUM_MLP, _cabi.MODEL_PENDULUM_MLP_ENSEMBLE):
+                raise ValueError("tile_memory='global' / 'auto' is not available for the PendulumMLP models "
+                                 "(their kernels fix their own tiles)")
         self._block_threads = int(block_threads)
         self._pdl = os.environ.get("MPPI_B200_PDL", "1") != "0"
         # split-cost rollout for problems that run with helper threads: measured 17.1 -> 14.8 us per command back to
@@ -478,6 +492,8 @@ class MPPI:
                 self._xchg_status_word = C.c_longlong.from_address(self._xchg_status.data_ptr())
             p.xchg_status_host = self._xchg_status.data_ptr()
         self._variant_pack(p)
+        if self._tile_memory == "global" or (self._tile_memory == "auto" and not self._shared_tile_fits(p)):
+            self._base_flags |= _cabi.FLAG_GLOBAL_TILE
         # the library sizes the workspace for any geometry of these dimensions, per environment
         info = _cabi.MppiLaunchInfo()
         p.flags = self._base_flags
@@ -499,6 +515,22 @@ class MPPI:
         self._dirty = False
         if self._model is not None:
             self._make_plan(p)
+
+    def _shared_tile_fits(self, p):
+        """tile_memory='auto': whether today's shared-memory plan serves these dimensions (no launch).  The fused route
+        asks the planner; the stepped route, the sampling and softmin kernels' plans (mppi_fused_query, model == 0)."""
+        p.flags = self._base_flags
+        info = _cabi.MppiLaunchInfo()
+        if self._model is None:
+            _cabi.check(self._lib.mppi_fused_query(C.byref(p), C.byref(info)), "mppi_fused_query")
+            return info.smem_bytes > 0
+        try:
+            _cabi.check(self._lib.mppi_fused_query(C.byref(p), C.byref(info)), "mppi_fused_query")
+        except _cabi.MppiLibraryError as e:
+            if "shared-memory tile does not fit" in str(e):
+                return False
+            raise
+        return True
 
     def _fill_model_params(self, p):
         """The model's current parameters and device tensors into `p`; returns what `p` points to — the host array of
@@ -670,6 +702,9 @@ class MPPI:
             self._take_model_params()
         if self._z_out is not None:
             raise _cabi.MppiLibraryError("resident mode does not record noise; call record_noise(False) first")
+        if self.launch_info.global_tile:
+            raise _cabi.MppiLibraryError("resident mode keeps its tiles in shared memory: not available on a global-tile plan "
+                                         "(tile_memory)")
         words = 64 + self.u_per_command * self.nu * (2 if self.dtype == torch.float64 else 1)
         if getattr(self, "_res_box", None) is None or self._res_box.numel() != words:
             self._res_box = torch.zeros(words, dtype=torch.int64).pin_memory()
@@ -1555,12 +1590,14 @@ class MPPI_Batched(MPPI):
 
     def __init__(self, dynamics, running_cost, nx, noise_sigma, num_envs, num_samples=100, horizon=15, device="cuda",
                  lambda_=1., noise_mu=None, u_min=None, u_max=None, u_init=None, u_scale=1, u_per_command=1,
-                 step_dependent_dynamics=False, noise_abs_cost=False, *, rng_seed=None, block_threads=0):
+                 step_dependent_dynamics=False, noise_abs_cost=False, *, rng_seed=None, block_threads=0,
+                 tile_memory="shared"):
         self.N = int(num_envs)
         super().__init__(dynamics, running_cost, nx, noise_sigma, num_samples=num_samples, horizon=horizon, device=device,
                          lambda_=lambda_, noise_mu=noise_mu, u_min=u_min, u_max=u_max, u_init=u_init, u_scale=u_scale,
                          u_per_command=u_per_command, step_dependent_dynamics=step_dependent_dynamics,
-                         noise_abs_cost=noise_abs_cost, rng_seed=rng_seed, block_threads=block_threads, threads_per_sample=0)
+                         noise_abs_cost=noise_abs_cost, rng_seed=rng_seed, block_threads=block_threads, threads_per_sample=0,
+                         tile_memory=tile_memory)
 
     # ---- (N, ...) buffers ------------------------------------------------------------------------
     def _alloc_nominal(self, U_init):

@@ -77,7 +77,8 @@ def kernel_names(real: str, variant: int, copies: int = 1):
     fused, split-cost, batched (MPPI variant only), resident, states.  A model with copies > 1 has only the fused
     (single-loop) and states kernels: the split-cost rollout and the kernels built on it roll out one copy per sample,
     and MPPI_Batched has no rollout_samples.  A module with the split-cost kernel also exports its single-GPU LL form
-    under a fixed unmangled name (MPPI_USER_KERNEL_LL, added by compile_user_model)."""
+    under a fixed unmangled name (MPPI_USER_KERNEL_LL, added by compile_user_model), and every module its global-tile kernels
+    (MPPI_USER_KERNEL_GTILE, and MPPI_USER_KERNEL_GTILE_BATCHED where the batched kernel exists)."""
     m = "mppi::UserModel"
     one = copies == 1
     return [f"&mppi::fused_command_kernel<{m}, {real}, {variant}, false, false>",
@@ -99,6 +100,10 @@ def compile_user_model(header_text: str, real: str, variant: int, copies: int = 
     src = '#include "mppi_fused.cuh"\n#include "mppi_resident.cuh"\n' + header_text + "\n"
     if copies == 1:   # the split-cost kernel's single-GPU LL form, under the name mppi_user_model_register looks up
         src += f"MPPI_USER_KERNEL_LL(mppi::UserModel, {real}, {variant})\n"
+    # the global-tile kernels (tile_memory='global' / 'auto' past the shared-memory edge), also under fixed names
+    src += f"MPPI_USER_KERNEL_GTILE(mppi::UserModel, {real}, {variant})\n"
+    if variant == 0 and copies == 1:
+        src += f"MPPI_USER_KERNEL_GTILE_BATCHED(mppi::UserModel, {real})\n"
     prog = C.c_void_p()
     if lib.nvrtcCreateProgram(C.byref(prog), src.encode(), b"mppi_user_model.cu", 0, None, None) != 0:
         raise RtcError("nvrtcCreateProgram failed")
