@@ -242,7 +242,8 @@ typedef struct MppiLaunchInfo {
 int mppi_b200_abi_version(void);
 /* Layout probe for foreign-language mirrors of MppiFusedParams: which=0 sizeof, 1 offsetof(seed),
  * 2 offsetof(state), 3 offsetof(U), 4 offsetof(rank), 5 offsetof(partial_out), 6 sizeof(MppiLaunchInfo),
- * 7 offsetof(model_weights), 8 offsetof(model_tensors). */
+ * 7 offsetof(model_weights), 8 offsetof(model_tensors); and of MppiClosedLoop: 9 sizeof, 10 offsetof(states),
+ * 11 offsetof(plant_params), 12 offsetof(plant_blocks). */
 uint64_t mppi_abi_layout(int which);
 const char* mppi_status_string(int status);
 const char* mppi_last_cuda_error(void);
@@ -292,6 +293,40 @@ int mppi_plan_set_model_params(void* plan, const double* model_params, const dou
  * mppi_user_model_set_tensors).  MPPI_ERR_UNSUPPORTED while a resident grid is armed. */
 int mppi_plan_set_model_tensors(void* plan, const MppiTensorRef* refs, int32_t n);
 
+/* ---- Closed-loop episodes: the receding-horizon loop without returning to the host -----------------
+ * `steps` control steps of a plan's controller against a plant, enqueued on the stream in one call.  Step s is the plan's
+ * command (mppi_plan_command with flags SHIFT | STATE_DEVICE, state_dev = states row s, action_out = actions row s, Philox
+ * (seed, offset + s * offset_stride)), then one plant step on that action: states row s + 1 = the model's step of row s
+ * under u_scale * action — what mppi_rollout_states replays for a one-row sequence — plus disturbance row s, and costs
+ * row s = the model's running cost of row s + 1 with that action (t = 0).  The plant is the plan's model (copy 0 of a model
+ * with copies) with its own parameter block per environment.  Both launches of every step use programmatic dependent
+ * launch where the plan does (MPPI_FLAG_PDL).  The plan's epochs advance once per command, as through mppi_plan_command.
+ * All buffers are device memory of the controller dtype, n_env = 1 for a single-environment plan. */
+typedef struct MppiClosedLoop {
+    uint32_t struct_size;                   /* sizeof(MppiClosedLoop), ABI check                                       */
+    int32_t steps;                          /* >= 1                                                                    */
+    uint64_t seed, offset, offset_stride;   /* command s draws (seed, offset + s * offset_stride)                      */
+    void* states;                           /* (steps+1, n_env, nx): row 0 read, rows 1..steps written                 */
+    void* actions;                          /* (steps, n_env, nu) written                                              */
+    void* costs;                            /* (steps, n_env) written, or NULL                                         */
+    const void* disturbance;                /* (steps, n_env, nx) or NULL                                              */
+    const double* plant_params;             /* HOST (n_plant, n_plant_params) doubles in the model's own layout (model_params
+                                               followed by model_params_ext), or NULL = the plan's parameters          */
+    int32_t n_plant, n_plant_params;        /* n_plant: 1 or n_env                                                     */
+    void* plant_blocks;                     /* caller-owned DEVICE scratch, n_plant * mppi_plan_model_block_bytes(plan)
+                                               bytes, 16-byte aligned; written once per call (stream-ordered)          */
+} MppiClosedLoop;
+/* Bytes one packed model parameter block takes in MppiClosedLoop.plant_blocks (a multiple of 16); 0 for a null plan. */
+uint64_t mppi_plan_model_block_bytes(void* plan);
+/* A plant row's first MPPI_MODEL_PARAM_DOUBLES doubles are its model_params (zero-padded), the rest its model_params_ext;
+ * a user model's plant reads the plan's device tensors.
+ * MPPI_ERR_ABI: struct_size.  MPPI_ERR_BAD_ARG: null plan / cl / states / actions / plant_blocks, steps < 1, n_plant not 1
+ * or n_env, n_plant_params < 0, plant_params NULL with n_plant > 1.
+ * MPPI_ERR_UNSUPPORTED: models without a plant step (PENDULUM_MLP / _ENSEMBLE, step-dependent user models),
+ * u_per_command != 1, sharded plans (world > 1 or EXPORT_PARTIAL), plans that record their noise (z_out) or draw it from a
+ * device counter (offset_dev), a resident grid armed.  All checked before any CUDA call. */
+int mppi_plan_closed_loop(void* plan, const MppiClosedLoop* cl, void* stream);
+
 /* ---- Resident mode: command() without a kernel launch ---------------------------------------------
  * For a host control loop (mppi.py:240-252 called once per control step).  One cooperative launch leaves the
  * command's grid on the SMs; each following command is a record (flags, Philox counter, start state) written into
@@ -337,8 +372,9 @@ int mppi_apply_partials(const MppiFusedParams* p, const void* partials, void* st
  * [0] fused_command_kernel<UserModel, real, variant, false, false>   [1] ... split-cost (or NULL)
  * [2] ... batched, MPPI variant (or NULL)   [3] resident_command_kernel<UserModel, real, variant> (or NULL)
  * [4] states_kernel<UserModel, real>.  A module with a split-cost kernel also exports its single-GPU LL form as
- * `mppi_user_fused_command_kernel_ll` (MPPI_USER_KERNEL_LL).  The handle goes into MppiFusedParams.user_model with
- * model = MPPI_MODEL_USER. */
+ * `mppi_user_fused_command_kernel_ll` (MPPI_USER_KERNEL_LL).  A module may export its closed-loop plant step as
+ * `mppi_user_plant_step_kernel` (MPPI_USER_KERNEL_PLANT; without it mppi_plan_closed_loop is unsupported for the model).
+ * The handle goes into MppiFusedParams.user_model with model = MPPI_MODEL_USER. */
 int mppi_user_model_register(const void* cubin, uint64_t cubin_bytes, int32_t nx, int32_t nu, int32_t n_params, int32_t dtype,
                              int32_t variant, const char* const* names, void** handle_out);
 int mppi_user_model_release(void* handle);

@@ -150,6 +150,25 @@ class MppiLaunchInfo(C.Structure):
     ]
 
 
+class MppiClosedLoop(C.Structure):
+    """Mirror of `struct MppiClosedLoop`: one closed-loop episode of a plan (mppi_plan_closed_loop)."""
+    _fields_ = [
+        ("struct_size", C.c_uint32),
+        ("steps", C.c_int32),
+        ("seed", C.c_uint64),
+        ("offset", C.c_uint64),
+        ("offset_stride", C.c_uint64),
+        ("states", C.c_void_p),
+        ("actions", C.c_void_p),
+        ("costs", C.c_void_p),
+        ("disturbance", C.c_void_p),
+        ("plant_params", C.c_void_p),
+        ("n_plant", C.c_int32),
+        ("n_plant_params", C.c_int32),
+        ("plant_blocks", C.c_void_p),
+    ]
+
+
 # every symbol include/mppi_b200.h declares: (name, restype, argtypes)
 _P = C.POINTER(MppiFusedParams)
 SYMBOLS = [
@@ -167,6 +186,8 @@ SYMBOLS = [
                                          C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mppi_plan_set_model_params", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),
     ("mppi_plan_set_model_tensors", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
+    ("mppi_plan_model_block_bytes", C.c_uint64, [C.c_void_p]),
+    ("mppi_plan_closed_loop", C.c_int, [C.c_void_p, C.POINTER(MppiClosedLoop), C.c_void_p]),
     ("mppi_resident_start", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     ("mppi_resident_command", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]),
     ("mppi_resident_sync", C.c_int, [C.c_void_p]),

@@ -131,6 +131,85 @@ int plan_command(Plan* pl, const double* state, const void* state_dev, uint32_t 
     return plan_launch(pl, stream);
 }
 
+// ---- closed-loop episodes (mppi_plan_closed_loop) -------------------------------------------------------
+// one packed parameter block in the plant scratch: the model's block rounded up to 16 bytes (alignment of every block)
+inline uint64_t plant_block_bytes(const Plan* pl) { return ((uint64_t)pl->mk->param_bytes + 15) / 16 * 16; }
+
+// the reasons a closed loop is refused, before any CUDA call (MPPI_OK: none)
+int check_closed_loop(const Plan* pl, const MppiClosedLoop* cl) {
+    if (pl == nullptr || cl == nullptr) return MPPI_ERR_BAD_ARG;
+    if (cl->struct_size != sizeof(MppiClosedLoop)) return MPPI_ERR_ABI;
+    const int n_env = pl->p.n_env > 1 ? pl->p.n_env : 1;
+    if (cl->steps < 1 || cl->states == nullptr || cl->actions == nullptr || cl->plant_blocks == nullptr) return MPPI_ERR_BAD_ARG;
+    if ((uintptr_t)cl->plant_blocks % 16 != 0 || cl->n_plant_params < 0) return MPPI_ERR_BAD_ARG;
+    if (cl->n_plant != 1 && cl->n_plant != n_env) return MPPI_ERR_BAD_ARG;
+    if (cl->plant_params == nullptr && cl->n_plant != 1) return MPPI_ERR_BAD_ARG;
+    if (pl->mk->plant == nullptr)
+        return UNSUPPORTED("closed loop: this model has no plant step (the PendulumMLP models, step-dependent user models)");
+    if (pl->p.u_per_command != 1) return UNSUPPORTED("closed loop: u_per_command must be 1 (the plant applies one action per command)");
+    if (pl->p.world > 1 || (pl->p.flags & MPPI_FLAG_EXPORT_PARTIAL)) return UNSUPPORTED("closed loop: not available on sharded controllers");
+    if (pl->p.z_out != nullptr) return UNSUPPORTED("closed loop: the plan records the noise it draws (z_out)");
+    if (pl->p.offset_dev != nullptr) return UNSUPPORTED("closed loop: the plan reads its Philox counter from the device (offset_dev)");
+    if (pl->res.armed) return UNSUPPORTED("closed loop: a resident grid is armed on this plan (mppi_resident_stop first)");
+    return MPPI_OK;
+}
+
+template <typename real>
+int closed_loop_t(Plan* pl, const MppiClosedLoop* cl, cudaStream_t stream) {
+    const ModelKernels* mk = pl->mk;
+    const int n_env = pl->p.n_env > 1 ? pl->p.n_env : 1;
+    const int nx = mk->nx, nu = mk->nu;
+    const uint64_t bb = plant_block_bytes(pl);
+    // the plant blocks, packed once per call with the model's loader (a user model's views: the plan's tensors)
+    unsigned char* host = new (std::nothrow) unsigned char[bb * cl->n_plant];
+    if (host == nullptr) return MPPI_ERR_BAD_ARG;
+    memset(host, 0, bb * cl->n_plant);
+    if (cl->plant_params == nullptr) {
+        memcpy(host, pl->mparams, mk->param_bytes);
+    } else {
+        MppiFusedParams pp = pl->p;
+        const int n = cl->n_plant_params;
+        for (int i = 0; i < cl->n_plant; ++i) {
+            const double* row = cl->plant_params + (size_t)i * n;
+            for (int j = 0; j < MPPI_MODEL_PARAM_DOUBLES; ++j) pp.model_params[j] = j < n ? row[j] : 0.0;
+            pp.model_params_ext = n > MPPI_MODEL_PARAM_DOUBLES ? row + MPPI_MODEL_PARAM_DOUBLES : nullptr;
+            pp.n_model_params_ext = n > MPPI_MODEL_PARAM_DOUBLES ? n - MPPI_MODEL_PARAM_DOUBLES : 0;
+            load_model_params(mk, &pp, host + (size_t)i * bb);
+        }
+    }
+    // pageable source: the copy has taken the data when the call returns
+    const cudaError_t ce = cudaMemcpyAsync(cl->plant_blocks, host, bb * cl->n_plant, cudaMemcpyHostToDevice, stream);
+    delete[] host;
+    if (ce != cudaSuccess) return cuda_fail(ce, "closed loop: plant block copy");
+    PlantStepArgs<real> ps;
+    ps.plants = (const unsigned char*)cl->plant_blocks;
+    ps.plant_stride = (long long)bb;
+    ps.n_env = n_env;
+    ps.n_plant = cl->n_plant;
+    ps.u_scale = reinterpret_cast<const KArgs<real>*>(pl->kargs)->nm.u_scale;      // get_rollouts' u_scale (mppi.py:445)
+    void* argv[1] = {(void*)&ps};
+    real* states = (real*)cl->states;
+    real* actions = (real*)cl->actions;
+    const real* w = (const real*)cl->disturbance;
+    const size_t xrow = (size_t)n_env * nx, urow = (size_t)n_env * nu;
+    for (int s = 0; s < cl->steps; ++s) {
+        real* xs = states + (size_t)s * xrow;
+        real* us = actions + (size_t)s * urow;
+        plan_update<real>(pl, nullptr, xs, MPPI_FLAG_SHIFT | MPPI_FLAG_STATE_DEVICE, cl->seed, cl->offset + (uint64_t)s * cl->offset_stride,
+                          nullptr, us, nullptr);
+        int rc = plan_launch(pl, stream);
+        if (rc) return rc;
+        ps.x = xs;
+        ps.x_next = xs + xrow;
+        ps.u = us;
+        ps.w = w != nullptr ? w + (size_t)s * xrow : nullptr;
+        ps.cost = cl->costs != nullptr ? (real*)cl->costs + (size_t)s * n_env : nullptr;
+        const cudaError_t e = launch_raw(mk->plant, (n_env + 127) / 128, 128, 0, stream, argv, pl->pdl != 0);
+        if (e != cudaSuccess) return cuda_fail(e, "closed loop: plant step launch");
+    }
+    return MPPI_OK;
+}
+
 // ---- resident mode: the device backend of csrc/mppi_resident_host.h ---------------------------------
 template <typename real>
 int resident_launch_t(Plan* pl, uint64_t seed, uint64_t offset_pred, int shift_pred, uint64_t seq_start, uint32_t gen) {
@@ -386,6 +465,10 @@ uint64_t mppi_abi_layout(int which) {
         case 6: return sizeof(MppiLaunchInfo);
         case 7: return offsetof(MppiFusedParams, model_weights);
         case 8: return offsetof(MppiFusedParams, model_tensors);
+        case 9: return sizeof(MppiClosedLoop);
+        case 10: return offsetof(MppiClosedLoop, states);
+        case 11: return offsetof(MppiClosedLoop, plant_params);
+        case 12: return offsetof(MppiClosedLoop, plant_blocks);
     }
     return 0;
 }
@@ -504,6 +587,18 @@ int mppi_plan_set_model_tensors(void* plan, const MppiTensorRef* refs, int32_t n
     return MPPI_OK;
 }
 
+uint64_t mppi_plan_model_block_bytes(void* plan) {
+    const Plan* pl = reinterpret_cast<const Plan*>(plan);
+    return pl == nullptr ? 0 : plant_block_bytes(pl);
+}
+
+int mppi_plan_closed_loop(void* plan, const MppiClosedLoop* cl, void* stream) {
+    Plan* pl = reinterpret_cast<Plan*>(plan);
+    const int rc = check_closed_loop(pl, cl);
+    if (rc) return rc;
+    return pl->is_double ? closed_loop_t<double>(pl, cl, (cudaStream_t)stream) : closed_loop_t<float>(pl, cl, (cudaStream_t)stream);
+}
+
 int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint64_t seed, uint64_t offset, const void* z,
                            void* action_out_dev, void* host_mailbox, void* action_host_out, void* stream) {
     Plan* pl = reinterpret_cast<Plan*>(plan);
@@ -596,6 +691,7 @@ int mppi_resident_stop(void* plan) {
 // toolkit) into a cubin and hands it over with the lowered names of the kernels; they are loaded as a cudaLibrary_t and
 // wrapped in a ModelKernels table exactly like a registry unit's.  `names`: 5 entries, nullptr = not built:
 //   [0] fused (this variant)  [1] split-cost  [2] batched (MPPI variant only)  [3] resident  [4] states
+// and the kernels a module exports under fixed names (LL, global-tile, plant step)
 namespace {
 void user_load(const ModelKernels* mk, void* dst, const double* blob, const double* ext, int n_ext) {
     for (int i = 0; i < mk->np; ++i) {
@@ -663,6 +759,12 @@ int mppi_user_model_register(const void* cubin, uint64_t cubin_bytes, int32_t nx
             return cuda_fail(e, gnames[i]);
         }
         *gslots[i] = (const void*)k;
+    }
+    // its closed-loop plant step, where the module has one (MPPI_USER_KERNEL_PLANT; none for step-dependent models)
+    {
+        cudaKernel_t k = nullptr;
+        if (cudaLibraryGetKernel(&k, lib, "mppi_user_plant_step_kernel") == cudaSuccess) mk.plant = (const void*)k;
+        else cudaGetLastError();      // absent: closed loops of this model are refused
     }
     if (mk.fused[variant] == nullptr || mk.states == nullptr) {
         cudaLibraryUnload(lib);

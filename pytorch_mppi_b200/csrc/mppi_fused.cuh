@@ -1931,6 +1931,17 @@ __global__ void __launch_bounds__(512) sample_kernel_gtile(const __grid_constant
     sample_body<real, VARIANT, NU, true>(a_in);
 }
 
+// Step t of an open-loop replay of the action rows pa: u = u_scale * pa[t] (mppi.py:313 / :445), then the model's step — FAST: its
+// fast form, which a replay takes throughout when in_fast_range holds for its start state and length, as the command's
+// rollouts do.  The states kernel (get_rollouts, the states along a command's rollouts) and the plant step of a closed
+// loop (a one-row replay) both step through here, so a closed loop's plant is get_rollouts(x, U=u[None]) bit for bit.
+template <class Model, typename real, bool FAST>
+__device__ __forceinline__ void replay_step(const typename Model::template P<real>& mp, real* x, real* u, const real* pa,
+                                            real u_scale, int t, int m) {
+    for (int n = 0; n < Model::NU; ++n) u[n] = Ops<real>::mul(u_scale, pa[t * Model::NU + n]);   // mppi.py:313 / :445
+    model_step<Model, real, FAST>(mp, x, u, t, m);
+}
+
 // states along the rollout of given perturbed actions (mppi.py:307-322), for registered models.
 // pa_stride = elements between consecutive samples' action sequences: T*nu for a (K,T,nu) tensor, 0 when every
 // sample replays the SAME (T,nu) sequence (get_rollouts, mppi.py:425-448).
@@ -1938,7 +1949,6 @@ __global__ void __launch_bounds__(512) sample_kernel_gtile(const __grid_constant
 template <class Model, typename real>
 __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ states, const KArgs<real> a,
                               const typename Model::template P<real> mp, long long pa_stride) {
-    typedef Ops<real> O;
     constexpr int NX = Model::NX, NU = Model::NU;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.K) return;
@@ -1959,8 +1969,7 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
         if (Model::template in_fast_range<real>(mp, x, a.T)) {
             for (int t = 0; t < a.T; ++t) {
                 real u[NU];
-                for (int n = 0; n < NU; ++n) u[n] = O::mul(a.nm.u_scale, pa[t * NU + n]);         // mppi.py:313 / :445
-                model_step<Model, real, true>(mp, x, u, t);
+                replay_step<Model, real, true>(mp, x, u, pa, a.nm.u_scale, t, 0);
                 for (int i = 0; i < NX; ++i) states[((size_t)k * a.T + t) * NX + i] = x[i];
             }
             return;
@@ -1968,11 +1977,74 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
     }
     for (int t = 0; t < a.T; ++t) {
         real u[NU];
-        for (int n = 0; n < NU; ++n) u[n] = O::mul(a.nm.u_scale, pa[t * NU + n]);                 // mppi.py:313 / :445
-        model_step<Model, real>(mp, x, u, t, m);
+        replay_step<Model, real, false>(mp, x, u, pa, a.nm.u_scale, t, m);
         for (int i = 0; i < NX; ++i) states[((size_t)k * a.T + t) * NX + i] = x[i];
     }
 }
+
+// One plant step of a closed-loop episode (mppi_plan_closed_loop), one thread per environment: after the command of
+// control step s wrote its action row, x_{s+1} = step(x_s, u_scale * u_s) with the environment's plant parameter block
+// (the replay of get_rollouts(x_s, U=u_s[None])), plus the disturbance row; the running cost of the reached state with
+// the same (scaled) action, t = 0, as a rollout scores its first step (mppi.py:313-319).
+template <typename real> struct PlantStepArgs {
+    const real* x;                  // (n_env, nx) state row s
+    real* x_next;                   // (n_env, nx) state row s + 1
+    const real* u;                  // (n_env, nu) action row s (the command's action_out)
+    const real* w;                  // (n_env, nx) disturbance row s, or nullptr
+    real* cost;                     // (n_env) cost row s, or nullptr
+    const unsigned char* plants;    // n_plant parameter blocks (Model::P<real>), plant_stride bytes apart
+    long long plant_stride;
+    int n_env, n_plant;
+    real u_scale;
+};
+// x_{s+1} and the cost of environment e, on the model's fast step or not (the caller's in_fast_range choice)
+template <class Model, typename real, bool FAST>
+__device__ __forceinline__ void plant_step_env(const PlantStepArgs<real>& a, const typename Model::template P<real>& mp, real* x, int e) {
+    typedef Ops<real> O;
+    constexpr int NX = Model::NX, NU = Model::NU;
+    real u[NU];
+    replay_step<Model, real, FAST>(mp, x, u, a.u + (size_t)e * NU, a.u_scale, 0, 0);
+    if (a.w != nullptr)
+        for (int i = 0; i < NX; ++i) x[i] = O::add(x[i], a.w[(size_t)e * NX + i]);
+    for (int i = 0; i < NX; ++i) a.x_next[(size_t)e * NX + i] = x[i];
+    // the cost of the state reached, disturbance included: on the model's general form (its fast form is bit-identical
+    // only inside the range in_fast_range vouched for, which a disturbance may leave)
+    if (a.cost != nullptr) a.cost[e] = model_cost<Model, real>(mp, x, u, 0);                  // mppi.py:318, t = 0
+}
+template <class Model, typename real>
+__device__ __forceinline__ void plant_step_body(const PlantStepArgs<real>& a) {
+    constexpr int NX = Model::NX;
+    // launched behind the command (programmatic dependent launch): let the next command start drawing its noise, then
+    // wait until this command's action row is written.  Without the launch attribute both are no-ops.
+    asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+    asm volatile("griddepcontrol.wait;" ::: "memory");
+    const int e = blockIdx.x * blockDim.x + threadIdx.x;
+    if (e >= a.n_env) return;
+    const typename Model::template P<real>& mp = *reinterpret_cast<const typename Model::template P<real>*>(
+        a.plants + (size_t)(a.n_plant > 1 ? e : 0) * (size_t)a.plant_stride);
+    real x[NX];
+    for (int i = 0; i < NX; ++i) x[i] = a.x[(size_t)e * NX + i];
+    if constexpr (FastRange<Model, real>::value) {      // as the states kernel chooses for a one-row replay
+        if (Model::template in_fast_range<real>(mp, x, 1)) {
+            plant_step_env<Model, real, true>(a, mp, x, e);
+            return;
+        }
+    }
+    plant_step_env<Model, real, false>(a, mp, x, e);
+}
+template <class Model, typename real>
+__global__ void __launch_bounds__(128) plant_step_kernel(const PlantStepArgs<real> a) {
+    plant_step_body<Model, real>(a);
+}
+
+#ifdef __CUDACC_RTC__
+// A user model exports its plant step under one unmangled name, which mppi_user_model_register looks up (step-dependent
+// models have none: a per-step schedule has no step index in a closed loop)
+#define MPPI_USER_KERNEL_PLANT(Model, real)                                                                                  \
+    extern "C" __global__ void __launch_bounds__(128) mppi_user_plant_step_kernel(const mppi::PlantStepArgs<real> a) {       \
+        mppi::plant_step_body<Model, real>(a);                                                                               \
+    }
+#endif
 
 // =================================================================================================
 // Generic path, part 2: softmin + weighted update from materialised cost_total (K) and eps (K,R)

@@ -87,6 +87,8 @@ struct ModelKernels {
     int copies;                      // run-time user models: the COPIES their kernels were compiled with (0 or 1: none)
     int n_tensors;                   // run-time user models: device tensor views behind the parameters (mppi_model_tensors.h)
     int32_t tensor_dtype[MPPI_MAX_MODEL_TENSORS], tensor_ndim[MPPI_MAX_MODEL_TENSORS];
+    const void* plant;               // plant_step_kernel<Model, real>: closed-loop episodes (nullptr: the PendulumMLP models,
+                                     // step-dependent user models)
 };
 }  // namespace mppi_host
 

@@ -1,6 +1,6 @@
 // mppi_model_tu.cu — one translation unit per (registered model, dtype): the fused command kernels
-// (fused_command_kernel<Model, real, V, ...>, all variants and instantiations), the resident command kernels and the
-// states kernel of that model — and, for the fp32 MLP, the wgmma kernels.  The unit contains no launch logic: it
+// (fused_command_kernel<Model, real, V, ...>, all variants and instantiations), the resident command kernels, the
+// states kernel and the closed-loop plant step of that model — and, for the fp32 MLP, the wgmma kernels.  The unit contains no launch logic: it
 // exports ONE symbol, mppi_host::model_kernels_<model>_<dtype>(), a table of kernel handles plus the parameter packer,
 // which the generic host code in mppi_b200.cu (mppi_fused_host.cuh) works on.
 //
@@ -85,6 +85,11 @@ const void* gtile_batched_kernel() {
     if constexpr (kIsMlp || kIsEnsemble) return nullptr;
     else return (const void*)fused_command_kernel_gtile<TuModel, TuReal, V_MPPI, true>;
 }
+// the plant step of closed-loop episodes: not for the MLP models (a learned model is not the plant it approximates)
+const void* plant_kernel() {
+    if constexpr (kIsMlp || kIsEnsemble) return nullptr;
+    else return (const void*)plant_step_kernel<TuModel, TuReal>;
+}
 template <int V, int SPLIT, int FAST> const void* tc_kernel() {
     if constexpr (kIsMlp && !MPPI_TU_F64) return (const void*)mlp_tc_command_kernel<V, SPLIT, FAST>;
     else if constexpr (kIsEnsemble && !MPPI_TU_F64) return (const void*)mlp_ens_tc_command_kernel<V, SPLIT, FAST>;
@@ -106,7 +111,8 @@ const ModelKernels g_kernels = {
     {{{tc_kernel<V_MPPI, 1, 0>(), tc_kernel<V_MPPI, 1, 1>()}, {tc_kernel<V_MPPI, 0, 0>(), tc_kernel<V_MPPI, 0, 1>()}},
      {{tc_kernel<V_SMPPI, 1, 0>(), tc_kernel<V_SMPPI, 1, 1>()}, {tc_kernel<V_SMPPI, 0, 0>(), tc_kernel<V_SMPPI, 0, 1>()}},
      {{tc_kernel<V_KMPPI, 1, 0>(), tc_kernel<V_KMPPI, 1, 1>()}, {tc_kernel<V_KMPPI, 0, 0>(), tc_kernel<V_KMPPI, 0, 1>()}}},
-    nullptr,
+    nullptr, 0, 0, {}, {},
+    plant_kernel(),
 };
 
 }  // namespace

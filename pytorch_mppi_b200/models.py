@@ -478,7 +478,7 @@ struct UserModel {{
         (0 MPPI / 1 SMPPI / 2 KMPPI): NVRTC, cached on disk.  Needs no GPU."""
         from . import rtc
         return rtc.compile_user_model(self.header_text(), "float" if dtype == torch.float32 else "double", int(variant),
-                                      self.copies)
+                                      self.copies, plant=not self.step_dependent)
 
     def rtc_handle(self, lib, dtype, variant):
         """The handle `MppiFusedParams.user_model` takes: the compiled kernels registered with the C library on the

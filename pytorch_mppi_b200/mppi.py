@@ -69,6 +69,13 @@ def _vec(x, n, name):
     return t.tolist()
 
 
+class ClosedLoopResult(typing.NamedTuple):
+    """What `run_closed_loop` returns: device tensors of the controller dtype (MPPI_Batched: an N axis after the first)."""
+    states: torch.Tensor     # (steps+1, [N,] nx): row 0 the start state, row s+1 the plant's step from row s
+    actions: torch.Tensor    # (steps, [N,] nu): the action of each command
+    costs: torch.Tensor      # (steps, [N]): the running cost of each reached state with its action, t = 0
+
+
 def _pad16(n_elems, es):
     return (n_elems * es + 15) // 16 * 16 // es
 
@@ -628,29 +635,35 @@ class MPPI:
         """(seed, counter base) for this command; the counter advances by the Philox calls one
         sample makes.  With rng_seed=None the stream is the torch CUDA generator's
         (torch.manual_seed reseeds it), consumed with the same (seed, offset) protocol ATen ops use."""
+        seed, base, _ = self._rng_block(1)
+        return seed, base
+
+    def _rng_block(self, n):
+        """(seed, counter base, per-command stride) of the next `n` commands, advancing the stream past all of them:
+        command i draws (seed, base + i * stride), exactly what `n` calls of `_next_rng` return."""
         per = 4 if self.dtype == torch.float32 else 2
         chunks = (self._noise_rows() + per - 1) // per
         if self._rng_mode == "torch":      # consume the torch CUDA generator exactly as torch.randn(K,T,nu) would
             gen = torch.cuda.default_generators[self.d.index]
             seed = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF
             off = gen.get_offset()
-            gen.set_offset(off + self._torch_counter_offset)
-            return seed, off // 4
+            gen.set_offset(off + n * self._torch_counter_offset)
+            return seed, off // 4, self._torch_counter_offset // 4
         if self._rng_seed is not None:
             base = self._rng_counter
-            self._rng_counter += chunks
-            return self._rng_seed, base
+            self._rng_counter += n * chunks
+            return self._rng_seed, base, chunks
         gen = torch.cuda.default_generators[self.d.index]
         seed = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF
         try:
             off = gen.get_offset()
-            gen.set_offset(off + 4 * chunks)
+            gen.set_offset(off + 4 * chunks * n)
         except (AttributeError, RuntimeError):   # very old torch: private counter keyed by the seed
             if getattr(self, "_rng_last_seed", None) != seed:
                 self._rng_last_seed, self._rng_counter = seed, 0
             off = 4 * self._rng_counter
-            self._rng_counter += chunks
-        return seed, off // 4
+            self._rng_counter += n * chunks
+        return seed, off // 4, chunks
 
     def refresh(self):
         """Re-read everything that feeds kernel constants (e.g. after retraining a PendulumMLP's network)."""
@@ -1346,6 +1359,106 @@ class MPPI:
             states[:, t + 1] = nxt[:, :self.nx]
         return states[:, 1:]
 
+    # ------------------------------------------------------------------------------------------
+    # closed-loop episodes on the device (mppi_plan_closed_loop)
+    # ------------------------------------------------------------------------------------------
+    def run_closed_loop(self, state, steps, *, plant_params=None, disturbance=None):
+        """The receding-horizon loop — command, apply the first action to the plant, repeat — for `steps` control steps,
+        enqueued in one call and run back to back on the GPU.  Step s is exactly ``command(x_s)`` with the device state
+        x_s, followed by ``x_{s+1} = get_rollouts(x_s, U=u_s[None])[0, 0] + disturbance[s]``; afterwards the controller
+        (nominal sequence, cost_total, beta / eta, noise / perturbed_action of the last command, RNG position, `state`)
+        is where those `steps` commands leave it.
+
+        state         (nx,) device tensor of the controller dtype
+        plant_params  None: the plant is the controller's model with its current parameters.  Else the plant's parameters
+                      in the model's own layout, ``param_blob() + param_blob_ext()`` (a CudaModel: its `params`), e.g.
+                      ``Pendulum(m=1.3).param_blob()``; a CudaModel's tensors are shared with the plant
+        disturbance   None, or a (steps, nx) device tensor of the controller dtype added to each reached state
+        Returns a ClosedLoopResult of device tensors: states (steps+1, nx) (row 0 = state), actions (steps, nu), costs
+        (steps,) — the model's running cost of each reached state with its action, cost(x_{s+1}, u_s) at t = 0, under
+        the plant's parameters.  Available on the fused route (registered and CudaModel models, not the PendulumMLP
+        models or step-dependent ones) with u_per_command = 1 on one GPU."""
+        return self._closed_loop(state, steps, plant_params, disturbance, None)
+
+    def _closed_loop(self, state, steps, plant_params, disturbance, N):
+        """run_closed_loop of one environment (N None) or of MPPI_Batched's N."""
+        n_env = 1 if N is None else N
+        lead = () if N is None else (N,)
+        m = self._model
+        # ---- refusals, before anything is launched -------------------------------------------------------------------
+        if isinstance(steps, bool) or not isinstance(steps, int) or steps < 1:
+            raise ValueError(f"steps must be an integer >= 1, got {steps!r}")
+        if m is None:
+            raise ValueError("run_closed_loop runs on the fused route: the dynamics and running cost must be a registered "
+                             "model's or a CudaModel's (arbitrary callables take the stepped route)")
+        if m.model_id in (_cabi.MODEL_PENDULUM_MLP, _cabi.MODEL_PENDULUM_MLP_ENSEMBLE):
+            raise ValueError("run_closed_loop: a learned PendulumMLP model is not a plant (it approximates one)")
+        if m.step_dependent:
+            raise ValueError("run_closed_loop: step-dependent models have no per-step schedule in a closed loop")
+        if self.u_per_command != 1:
+            raise ValueError("run_closed_loop needs u_per_command = 1 (the plant applies one action per command)")
+        if self._world > 1:
+            raise ValueError("run_closed_loop is not available on sharded controllers")
+        if self._z_inject is not None:
+            raise ValueError("run_closed_loop draws its noise from the RNG stream: a noise tensor is injected (inject_noise)")
+        if self._z_out is not None:
+            raise ValueError("run_closed_loop does not record the noise it draws: call record_noise(False) first")
+        if getattr(self, "_offset_dev", None) is not None:
+            raise ValueError("run_closed_loop: this controller's Philox counter lives on the device (compile() captured a "
+                             "CUDA graph); build a controller without compile() for closed loops")
+        if not torch.is_tensor(state) or state.dtype != self.dtype or state.device != self.d or \
+                tuple(state.shape) != lead + (self.nx,):
+            raise ValueError(f"state must be a {tuple(lead + (self.nx,))} tensor of {self.dtype} on {self.d}, got "
+                             + (f"{tuple(state.shape)} {state.dtype} on {state.device}" if torch.is_tensor(state) else repr(type(state))))
+        if disturbance is not None:
+            if not torch.is_tensor(disturbance) or disturbance.dtype != self.dtype or disturbance.device != self.d or \
+                    tuple(disturbance.shape) != (steps,) + lead + (self.nx,):
+                raise ValueError(f"disturbance must be a {(steps,) + lead + (self.nx,)} tensor of {self.dtype} on {self.d}")
+            disturbance = disturbance.contiguous()
+        n_params = len(m.param_blob()) + len(m.param_blob_ext())
+        plant = None
+        if plant_params is not None:
+            pt = plant_params if torch.is_tensor(plant_params) else torch.as_tensor(plant_params, dtype=torch.float64)
+            if not pt.is_floating_point() or pt.device not in (torch.device("cpu"), self.d):
+                raise ValueError(f"plant_params must be floating point, on the CPU or {self.d}; got {pt.dtype} on {pt.device}")
+            shapes = [(n_params,)] + ([(n_env, n_params)] if N is not None else [])
+            if tuple(pt.shape) not in shapes:
+                raise ValueError(f"plant_params must have shape {' or '.join(map(str, shapes))} (the model's "
+                                 f"param_blob() + param_blob_ext()), got {tuple(pt.shape)}")
+            plant = pt.detach().to("cpu", torch.float64).reshape(-1, n_params).contiguous()
+        # ---- the controller as command() leaves it for a launch --------------------------------------------------------
+        self._leave_resident()
+        if self._dirty:
+            self._pack()
+        if getattr(m, "_param_version", 0) != self._model_version:
+            self._take_model_params()
+        lib = self._lib
+        seed, base, stride = self._rng_block(steps)
+        states = torch.empty((steps + 1,) + lead + (self.nx,), device=self.d, dtype=self.dtype)
+        states[0].copy_(state)
+        actions = torch.empty((steps,) + lead + (self.nu,), device=self.d, dtype=self.dtype)
+        costs = torch.empty((steps,) + lead, device=self.d, dtype=self.dtype)
+        n_plant = 1 if plant is None else plant.shape[0]
+        blocks = torch.empty(n_plant * int(lib.mppi_plan_model_block_bytes(self._plan)), device=self.d, dtype=torch.uint8)
+        cl = _cabi.MppiClosedLoop(struct_size=C.sizeof(_cabi.MppiClosedLoop), steps=steps, seed=seed, offset=base,
+                                  offset_stride=stride, states=states.data_ptr(), actions=actions.data_ptr(),
+                                  costs=costs.data_ptr(), disturbance=None if disturbance is None else disturbance.data_ptr(),
+                                  plant_params=None if plant is None else plant.data_ptr(), n_plant=n_plant,
+                                  n_plant_params=n_params if plant is not None else 0, plant_blocks=blocks.data_ptr())
+        stream = torch._C._cuda_getCurrentRawStream(self.d.index)
+        _cabi.check(lib.mppi_plan_closed_loop(self._plan, C.byref(cl), stream), "mppi_plan_closed_loop")
+        # ---- bookkeeping of the last command (lazy noise / perturbed_action, materialised from its state row) ----------
+        self._cmd_count += steps
+        self._z_keep = None
+        last = states[steps - 1]
+        self.state = last                  # keeps the rows the last command read alive for materialisation
+        self._last = (self._base_flags | _cabi.FLAG_STATE_DEVICE | _cabi.FLAG_SHIFT, seed, base + (steps - 1) * stride, None,
+                      last.data_ptr())
+        self.cost_total = self._cost_buf
+        self._states = None
+        self._actions = None
+        return ClosedLoopResult(states, actions, costs)
+
 
 class SMPPI(MPPI):
     """Smooth MPPI: noise is sampled on the control derivative, actions are its integral, and the
@@ -1692,6 +1805,12 @@ class MPPI_Batched(MPPI):
                         "mppi_softmin_update")
         self.cost_total = self._cost_buf
         return action[:, 0] if self.u_per_command == 1 else action                               # mppi.py:870-873
+
+    def run_closed_loop(self, states, steps, *, plant_params=None, disturbance=None):
+        """`MPPI.run_closed_loop` for the N environments: states (N, nx); plant_params (n_params,) for one plant or
+        (N, n_params), one plant per environment (domain randomisation); disturbance (steps, N, nx).  Returns states
+        (steps+1, N, nx), actions (steps, N, nu) and costs (steps, N)."""
+        return self._closed_loop(states, steps, plant_params, disturbance, self.N)
 
     # per-environment intermediates are not materialised lazily for the batched controller
     noise = property(lambda self: None)

@@ -88,15 +88,9 @@ def kernel_names(real: str, variant: int, copies: int = 1):
             f"&mppi::states_kernel<{m}, {real}>"]
 
 
-def compile_user_model(header_text: str, real: str, variant: int, copies: int = 1):
-    """-> (cubin bytes, [lowered kernel name or None] x 5).  Cached on disk."""
-    tag = hashlib.sha1(f"{header_text}|{real}|{variant}|{copies}|{_sources_hash()}".encode()).hexdigest()[:20]
-    cubin_path = os.path.join(CACHE, f"rtc_{tag}.cubin")
-    names_path = os.path.join(CACHE, f"rtc_{tag}.json")
-    if os.path.exists(cubin_path) and os.path.exists(names_path):
-        with open(cubin_path, "rb") as f, open(names_path) as g:
-            return f.read(), json.load(g)
-    lib = _load_nvrtc()
+def compile_user_model(header_text: str, real: str, variant: int, copies: int = 1, plant: bool = True):
+    """-> (cubin bytes, [lowered kernel name or None] x 5).  Cached on disk.  `plant`: also export the closed-loop plant
+    step (MPPI_USER_KERNEL_PLANT; step-dependent models have none)."""
     src = '#include "mppi_fused.cuh"\n#include "mppi_resident.cuh"\n' + header_text + "\n"
     if copies == 1:   # the split-cost kernel's single-GPU LL form, under the name mppi_user_model_register looks up
         src += f"MPPI_USER_KERNEL_LL(mppi::UserModel, {real}, {variant})\n"
@@ -104,6 +98,17 @@ def compile_user_model(header_text: str, real: str, variant: int, copies: int = 
     src += f"MPPI_USER_KERNEL_GTILE(mppi::UserModel, {real}, {variant})\n"
     if variant == 0 and copies == 1:
         src += f"MPPI_USER_KERNEL_GTILE_BATCHED(mppi::UserModel, {real})\n"
+    if plant:         # the plant step of closed-loop episodes (run_closed_loop)
+        src += f"MPPI_USER_KERNEL_PLANT(mppi::UserModel, {real})\n"
+    # keyed by the whole program (model, exported kernels) and the kernel headers it includes: a module built before a
+    # kernel was added is never reused
+    tag = hashlib.sha1(f"{src}|{real}|{variant}|{copies}|{_sources_hash()}".encode()).hexdigest()[:20]
+    cubin_path = os.path.join(CACHE, f"rtc_{tag}.cubin")
+    names_path = os.path.join(CACHE, f"rtc_{tag}.json")
+    if os.path.exists(cubin_path) and os.path.exists(names_path):
+        with open(cubin_path, "rb") as f, open(names_path) as g:
+            return f.read(), json.load(g)
+    lib = _load_nvrtc()
     prog = C.c_void_p()
     if lib.nvrtcCreateProgram(C.byref(prog), src.encode(), b"mppi_user_model.cu", 0, None, None) != 0:
         raise RtcError("nvrtcCreateProgram failed")
