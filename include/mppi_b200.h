@@ -243,7 +243,8 @@ int mppi_b200_abi_version(void);
 /* Layout probe for foreign-language mirrors of MppiFusedParams: which=0 sizeof, 1 offsetof(seed),
  * 2 offsetof(state), 3 offsetof(U), 4 offsetof(rank), 5 offsetof(partial_out), 6 sizeof(MppiLaunchInfo),
  * 7 offsetof(model_weights), 8 offsetof(model_tensors); and of MppiClosedLoop: 9 sizeof, 10 offsetof(states),
- * 11 offsetof(plant_params), 12 offsetof(plant_blocks). */
+ * 11 offsetof(plant_params), 12 offsetof(plant_blocks); and of MppiEnvParams: 13 sizeof, 14 offsetof(chol),
+ * 15 offsetof(model_params), 16 offsetof(scratch). */
 uint64_t mppi_abi_layout(int which);
 const char* mppi_status_string(int status);
 const char* mppi_last_cuda_error(void);
@@ -326,6 +327,44 @@ uint64_t mppi_plan_model_block_bytes(void* plan);
  * u_per_command != 1, sharded plans (world > 1 or EXPORT_PARTIAL), plans that record their noise (z_out) or draw it from a
  * device counter (offset_dev), a resident grid armed.  All checked before any CUDA call. */
 int mppi_plan_closed_loop(void* plan, const MppiClosedLoop* cl, void* stream);
+
+/* ---- Per-environment settings of a batched plan (n_env > 1) ---------------------------------------
+ * Environment e of a batched plan may have its own temperature, noise covariance, noise mean and model parameters; the
+ * K standard normals stay shared.  Every array is optional (NULL: the plan's value applies to every environment) and
+ * HOST memory, read during the call.  Each environment's noise model is built exactly as the plan's: the plan's parameters
+ * with that environment's values substituted.  An environment's covariance counts as diagonal (MPPI_FLAG_DIAG_SIGMA)
+ * when its Cholesky factor is: a diagonal factor is the one of a diagonal covariance, so diagonal and full covariances
+ * may be mixed.  The packed blocks go to `scratch` with one stream-ordered copy; commands enqueued before the call keep the
+ * values they were launched with, the following commands (and mppi_plan_closed_loop, whose plants with plant_params NULL
+ * are then the per-environment models) use the new ones.  No new plan: kernel and geometry stay; with model parameters
+ * the plan runs the batched kernel that reads one parameter block per environment.  All pointers NULL: back to the plan's
+ * shared values. */
+typedef struct MppiEnvParams {
+    uint32_t struct_size;                   /* sizeof(MppiEnvParams), ABI check                                        */
+    int32_t n_env;                          /* the plan's n_env                                                        */
+    const double* lambda_;                  /* (n_env) temperatures > 0, or NULL                                       */
+    const double* chol;                     /* (n_env, MPPI_MAX_NU, MPPI_MAX_NU) lower Cholesky factors of the noise
+                                               covariances, as MppiFusedParams.chol (diagonal: sqrt on the diagonal); NULL
+                                               or set together with sigma_inv                                          */
+    const double* sigma_inv;                /* (n_env, MPPI_MAX_NU, MPPI_MAX_NU) inverse covariances, or NULL           */
+    const double* noise_mu;                 /* (n_env, MPPI_MAX_NU) noise means, or NULL                               */
+    const double* model_params;             /* (n_env, n_model_params) in the model's own layout (model_params followed
+                                               by model_params_ext, as MppiClosedLoop.plant_params), or NULL; a user
+                                               model's blocks read the plan's device tensors                           */
+    int32_t n_model_params;
+    int32_t reserved;                       /* 0                                                                       */
+    void* scratch;                          /* caller-owned DEVICE memory, mppi_plan_env_scratch_bytes(plan) bytes,
+                                               16-byte aligned, kept for as long as the plan runs with these settings;
+                                               NULL when every array is NULL                                           */
+    uint64_t scratch_bytes;
+} MppiEnvParams;
+/* Bytes of MppiEnvParams.scratch for this plan (n_env parameter blocks and noise models); 0 for a null plan. */
+uint64_t mppi_plan_env_scratch_bytes(void* plan);
+/* MPPI_ERR_ABI: struct_size.  MPPI_ERR_BAD_ARG: null plan / ep, n_env not the plan's, a temperature <= 0 or not finite,
+ * only one of chol / sigma_inv, n_model_params < 0, reserved != 0, scratch NULL / misaligned / smaller than
+ * mppi_plan_env_scratch_bytes.  MPPI_ERR_UNSUPPORTED: single-environment plans, sharded plans, model parameters of the
+ * PENDULUM_MLP models (no per-environment kernel).  All checked before any CUDA call. */
+int mppi_plan_set_env_params(void* plan, const MppiEnvParams* ep, void* stream);
 
 /* ---- Resident mode: command() without a kernel launch ---------------------------------------------
  * For a host control loop (mppi.py:240-252 called once per control step).  One cooperative launch leaves the

@@ -169,6 +169,23 @@ class MppiClosedLoop(C.Structure):
     ]
 
 
+class MppiEnvParams(C.Structure):
+    """Mirror of `struct MppiEnvParams`: per-environment settings of a batched plan (mppi_plan_set_env_params)."""
+    _fields_ = [
+        ("struct_size", C.c_uint32),
+        ("n_env", C.c_int32),
+        ("lambda_", C.c_void_p),
+        ("chol", C.c_void_p),
+        ("sigma_inv", C.c_void_p),
+        ("noise_mu", C.c_void_p),
+        ("model_params", C.c_void_p),
+        ("n_model_params", C.c_int32),
+        ("reserved", C.c_int32),
+        ("scratch", C.c_void_p),
+        ("scratch_bytes", C.c_uint64),
+    ]
+
+
 # every symbol include/mppi_b200.h declares: (name, restype, argtypes)
 _P = C.POINTER(MppiFusedParams)
 SYMBOLS = [
@@ -188,6 +205,8 @@ SYMBOLS = [
     ("mppi_plan_set_model_tensors", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     ("mppi_plan_model_block_bytes", C.c_uint64, [C.c_void_p]),
     ("mppi_plan_closed_loop", C.c_int, [C.c_void_p, C.POINTER(MppiClosedLoop), C.c_void_p]),
+    ("mppi_plan_env_scratch_bytes", C.c_uint64, [C.c_void_p]),
+    ("mppi_plan_set_env_params", C.c_int, [C.c_void_p, C.POINTER(MppiEnvParams), C.c_void_p]),
     ("mppi_resident_start", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     ("mppi_resident_command", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]),
     ("mppi_resident_sync", C.c_int, [C.c_void_p]),

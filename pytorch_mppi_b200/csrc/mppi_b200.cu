@@ -109,8 +109,14 @@ inline void plan_update(Plan* pl, const double* state, const void* state_dev, ui
 inline int plan_launch(Plan* pl, cudaStream_t stream) {
     int rc = refuse_capture(stream, pl->g);
     if (rc) return rc;
-    void* argv[2] = {(void*)pl->kargs, (void*)pl->mparams};
-    cudaError_t e = launch_raw(pl->kernel, pl->g.nb, pl->g.BD, pl->g.smem, stream, argv, pl->pdl != 0, pl->p.n_env > 1 ? pl->p.n_env : 1,
+    void* argv[3] = {(void*)pl->kargs, (void*)pl->mparams, nullptr};
+    const void* kernel = pl->kernel;
+    if (pl->env_kernel != nullptr) {      // per-environment parameter blocks in place of the plan's one
+        kernel = pl->env_kernel;
+        argv[1] = (void*)&pl->env_mp;
+        argv[2] = (void*)&pl->env_stride;
+    }
+    cudaError_t e = launch_raw(kernel, pl->g.nb, pl->g.BD, pl->g.smem, stream, argv, pl->pdl != 0, pl->p.n_env > 1 ? pl->p.n_env : 1,
                                pl->g.cluster);
     if (e != cudaSuccess) {
         snprintf(g_cuda_err, sizeof(g_cuda_err), "plan launch grid=%d block=%d smem=%d cluster=%d: %s (%s)", pl->g.nb, pl->g.BD, pl->g.smem, pl->g.cluster,
@@ -134,6 +140,20 @@ int plan_command(Plan* pl, const double* state, const void* state_dev, uint32_t 
 // ---- closed-loop episodes (mppi_plan_closed_loop) -------------------------------------------------------
 // one packed parameter block in the plant scratch: the model's block rounded up to 16 bytes (alignment of every block)
 inline uint64_t plant_block_bytes(const Plan* pl) { return ((uint64_t)pl->mk->param_bytes + 15) / 16 * 16; }
+
+// n rows of n_params doubles in the model's own layout (the first MPPI_MODEL_PARAM_DOUBLES are its model_params,
+// zero-padded, the rest its model_params_ext), packed with the model's loader into n blocks plant_block_bytes apart
+void pack_param_rows(const Plan* pl, const double* rows, int n, int n_params, unsigned char* dst) {
+    MppiFusedParams pp = pl->p;
+    const uint64_t bb = plant_block_bytes(pl);
+    for (int i = 0; i < n; ++i) {
+        const double* row = rows + (size_t)i * n_params;
+        for (int j = 0; j < MPPI_MODEL_PARAM_DOUBLES; ++j) pp.model_params[j] = j < n_params ? row[j] : 0.0;
+        pp.model_params_ext = n_params > MPPI_MODEL_PARAM_DOUBLES ? row + MPPI_MODEL_PARAM_DOUBLES : nullptr;
+        pp.n_model_params_ext = n_params > MPPI_MODEL_PARAM_DOUBLES ? n_params - MPPI_MODEL_PARAM_DOUBLES : 0;
+        load_model_params(pl->mk, &pp, dst + (size_t)i * bb);
+    }
+}
 
 // the reasons a closed loop is refused, before any CUDA call (MPPI_OK: none)
 int check_closed_loop(const Plan* pl, const MppiClosedLoop* cl) {
@@ -160,32 +180,27 @@ int closed_loop_t(Plan* pl, const MppiClosedLoop* cl, cudaStream_t stream) {
     const int n_env = pl->p.n_env > 1 ? pl->p.n_env : 1;
     const int nx = mk->nx, nu = mk->nu;
     const uint64_t bb = plant_block_bytes(pl);
-    // the plant blocks, packed once per call with the model's loader (a user model's views: the plan's tensors)
-    unsigned char* host = new (std::nothrow) unsigned char[bb * cl->n_plant];
-    if (host == nullptr) return MPPI_ERR_BAD_ARG;
-    memset(host, 0, bb * cl->n_plant);
-    if (cl->plant_params == nullptr) {
-        memcpy(host, pl->mparams, mk->param_bytes);
-    } else {
-        MppiFusedParams pp = pl->p;
-        const int n = cl->n_plant_params;
-        for (int i = 0; i < cl->n_plant; ++i) {
-            const double* row = cl->plant_params + (size_t)i * n;
-            for (int j = 0; j < MPPI_MODEL_PARAM_DOUBLES; ++j) pp.model_params[j] = j < n ? row[j] : 0.0;
-            pp.model_params_ext = n > MPPI_MODEL_PARAM_DOUBLES ? row + MPPI_MODEL_PARAM_DOUBLES : nullptr;
-            pp.n_model_params_ext = n > MPPI_MODEL_PARAM_DOUBLES ? n - MPPI_MODEL_PARAM_DOUBLES : 0;
-            load_model_params(mk, &pp, host + (size_t)i * bb);
-        }
-    }
-    // pageable source: the copy has taken the data when the call returns
-    const cudaError_t ce = cudaMemcpyAsync(cl->plant_blocks, host, bb * cl->n_plant, cudaMemcpyHostToDevice, stream);
-    delete[] host;
-    if (ce != cudaSuccess) return cuda_fail(ce, "closed loop: plant block copy");
     PlantStepArgs<real> ps;
     ps.plants = (const unsigned char*)cl->plant_blocks;
     ps.plant_stride = (long long)bb;
     ps.n_env = n_env;
     ps.n_plant = cl->n_plant;
+    if (cl->plant_params == nullptr && pl->env_kernel != nullptr) {
+        // per-environment model parameters: environment e's plant is its own model, the blocks its commands read
+        ps.plants = pl->env_mp;
+        ps.n_plant = n_env;
+    } else {
+        // the plant blocks, packed once per call with the model's loader (a user model's views: the plan's tensors)
+        unsigned char* host = new (std::nothrow) unsigned char[bb * cl->n_plant];
+        if (host == nullptr) return MPPI_ERR_BAD_ARG;
+        memset(host, 0, bb * cl->n_plant);
+        if (cl->plant_params == nullptr) memcpy(host, pl->mparams, mk->param_bytes);
+        else pack_param_rows(pl, cl->plant_params, cl->n_plant, cl->n_plant_params, host);
+        // pageable source: the copy has taken the data when the call returns
+        const cudaError_t ce = cudaMemcpyAsync(cl->plant_blocks, host, bb * cl->n_plant, cudaMemcpyHostToDevice, stream);
+        delete[] host;
+        if (ce != cudaSuccess) return cuda_fail(ce, "closed loop: plant block copy");
+    }
     ps.u_scale = reinterpret_cast<const KArgs<real>*>(pl->kargs)->nm.u_scale;      // get_rollouts' u_scale (mppi.py:445)
     void* argv[1] = {(void*)&ps};
     real* states = (real*)cl->states;
@@ -207,6 +222,103 @@ int closed_loop_t(Plan* pl, const MppiClosedLoop* cl, cudaStream_t stream) {
         const cudaError_t e = launch_raw(mk->plant, (n_env + 127) / 128, 128, 0, stream, argv, pl->pdl != 0);
         if (e != cudaSuccess) return cuda_fail(e, "closed loop: plant step launch");
     }
+    return MPPI_OK;
+}
+
+// ---- per-environment settings (mppi_plan_set_env_params) -------------------------------------------------
+// scratch: n_env parameter blocks (plant_block_bytes apart), then n_env noise models
+inline uint64_t env_nm_bytes(const Plan* pl) {
+    return pl->is_double ? sizeof(NoiseModel<double>) : sizeof(NoiseModel<float>);
+}
+inline uint64_t env_scratch_bytes(const Plan* pl) {
+    return (uint64_t)pl->p.n_env * (plant_block_bytes(pl) + env_nm_bytes(pl));
+}
+
+// the reasons the settings are refused, before any CUDA call (MPPI_OK: none)
+int check_env_params(const Plan* pl, const MppiEnvParams* ep) {
+    if (pl == nullptr || ep == nullptr) return MPPI_ERR_BAD_ARG;
+    if (ep->struct_size != sizeof(MppiEnvParams)) return MPPI_ERR_ABI;
+    if (pl->p.n_env <= 1) return UNSUPPORTED("per-environment settings: the plan has one environment (MPPI_Batched only)");
+    if (pl->p.world > 1 || (pl->p.flags & MPPI_FLAG_EXPORT_PARTIAL))
+        return UNSUPPORTED("per-environment settings: not available on sharded controllers");
+    if (ep->n_env != pl->p.n_env || ep->n_model_params < 0 || ep->reserved != 0) return MPPI_ERR_BAD_ARG;
+    if ((ep->chol == nullptr) != (ep->sigma_inv == nullptr)) return MPPI_ERR_BAD_ARG;
+    if (ep->lambda_ != nullptr)
+        for (int e = 0; e < ep->n_env; ++e)
+            if (!(ep->lambda_[e] > 0.0) || !isfinite(ep->lambda_[e])) return MPPI_ERR_BAD_ARG;
+    if (ep->model_params != nullptr) {
+        const bool gtile = (pl->p.flags & MPPI_FLAG_GLOBAL_TILE) != 0;
+        if ((gtile ? pl->mk->env_gtile_batched : pl->mk->env_batched) == nullptr)
+            return UNSUPPORTED("per-environment model parameters: this model has no per-environment kernel (the PendulumMLP models)");
+    }
+    const bool any = ep->lambda_ || ep->chol || ep->noise_mu || ep->model_params;
+    if (any && (ep->scratch == nullptr || (uintptr_t)ep->scratch % 16 != 0 || ep->scratch_bytes < env_scratch_bytes(pl)))
+        return MPPI_ERR_BAD_ARG;
+    return MPPI_OK;
+}
+
+template <typename real>
+int set_env_params_t(Plan* pl, const MppiEnvParams* ep, cudaStream_t stream) {
+    KArgs<real>* a = reinterpret_cast<KArgs<real>*>(pl->kargs);
+    const bool has_nm = ep->lambda_ || ep->chol || ep->noise_mu;
+    if (!has_nm && ep->model_params == nullptr) {      // back to the plan's shared values
+        a->env_nm = nullptr;
+        pl->env_kernel = nullptr;
+        pl->env_mp = nullptr;
+        return MPPI_OK;
+    }
+    const int n_env = pl->p.n_env;
+    const uint64_t bb = plant_block_bytes(pl), mp_bytes = (uint64_t)n_env * bb;
+    const void* env_kernel = nullptr;
+    if (ep->model_params != nullptr) {
+        // the per-environment kernel runs the plan's geometry (same tiles, grid and clusters, so the same reduction order):
+        // its shared-memory limit is raised as the plan's kernel's was.  Its registers are not capped for two 512-thread
+        // CTAs per SM (the cap spills); fewer resident CTAs than the plan counted on cost time, not correctness: only an
+        // environment's finisher waits, for CTAs of its own environment dispatched before it.
+        env_kernel = (pl->p.flags & MPPI_FLAG_GLOBAL_TILE) ? pl->mk->env_gtile_batched : pl->mk->env_batched;
+        DevInfo di;
+        int rc = get_dev_info(di);
+        if (rc) return rc;
+        cudaFuncAttributes fa;
+        CK(cudaFuncGetAttributes(&fa, env_kernel));
+        CK(cudaFuncSetAttribute(env_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, di.max_smem_optin - (int)fa.sharedSizeBytes));
+        int occ = 0;
+        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, env_kernel, pl->g.BD, pl->g.smem));
+        if (occ < 1) return UNSUPPORTED("per-environment model parameters: the per-environment kernel does not fit the plan's CTA");
+    }
+    unsigned char* host = new (std::nothrow) unsigned char[env_scratch_bytes(pl)];
+    if (host == nullptr) return MPPI_ERR_BAD_ARG;
+    memset(host, 0, env_scratch_bytes(pl));
+    if (ep->model_params != nullptr) pack_param_rows(pl, ep->model_params, n_env, ep->n_model_params, host);
+    NoiseModel<real>* nms = reinterpret_cast<NoiseModel<real>*>(host + mp_bytes);
+    if (has_nm) {
+        // environment e's noise model: the plan's parameters with e's values, through the plan's own fill_noise_model
+        MppiFusedParams pe = pl->p;
+        for (int e = 0; e < n_env; ++e) {
+            if (ep->lambda_ != nullptr) pe.lambda_ = ep->lambda_[e];
+            if (ep->noise_mu != nullptr) memcpy(pe.noise_mu, ep->noise_mu + (size_t)e * MPPI_MAX_NU, sizeof(pe.noise_mu));
+            if (ep->chol != nullptr) {
+                const size_t nn = MPPI_MAX_NU * MPPI_MAX_NU;
+                memcpy(pe.chol, ep->chol + (size_t)e * nn, sizeof(pe.chol));
+                memcpy(pe.sigma_inv, ep->sigma_inv + (size_t)e * nn, sizeof(pe.sigma_inv));
+                bool diag = true;
+                for (int i = 0; i < MPPI_MAX_NU; ++i)
+                    for (int j = 0; j < MPPI_MAX_NU; ++j) diag = diag && (i == j || pe.chol[i * MPPI_MAX_NU + j] == 0.0);
+                pe.flags = diag ? (pe.flags | MPPI_FLAG_DIAG_SIGMA) : (pe.flags & ~(uint32_t)MPPI_FLAG_DIAG_SIGMA);
+            }
+            fill_noise_model<real>(&pe, nms[e]);
+        }
+    }
+    // pageable source: the copy has taken the data when the call returns; commands enqueued before it have read the old
+    // blocks by the time it lands (stream order)
+    const cudaError_t ce = cudaMemcpyAsync(ep->scratch, host, env_scratch_bytes(pl), cudaMemcpyHostToDevice, stream);
+    delete[] host;
+    if (ce != cudaSuccess) return cuda_fail(ce, "per-environment settings: block copy");
+    const unsigned char* scratch = (const unsigned char*)ep->scratch;
+    a->env_nm = has_nm ? reinterpret_cast<const NoiseModel<real>*>(scratch + mp_bytes) : nullptr;
+    pl->env_kernel = env_kernel;
+    pl->env_mp = env_kernel != nullptr ? scratch : nullptr;
+    pl->env_stride = (long long)bb;
     return MPPI_OK;
 }
 
@@ -469,6 +581,10 @@ uint64_t mppi_abi_layout(int which) {
         case 10: return offsetof(MppiClosedLoop, states);
         case 11: return offsetof(MppiClosedLoop, plant_params);
         case 12: return offsetof(MppiClosedLoop, plant_blocks);
+        case 13: return sizeof(MppiEnvParams);
+        case 14: return offsetof(MppiEnvParams, chol);
+        case 15: return offsetof(MppiEnvParams, model_params);
+        case 16: return offsetof(MppiEnvParams, scratch);
     }
     return 0;
 }
@@ -597,6 +713,18 @@ int mppi_plan_closed_loop(void* plan, const MppiClosedLoop* cl, void* stream) {
     const int rc = check_closed_loop(pl, cl);
     if (rc) return rc;
     return pl->is_double ? closed_loop_t<double>(pl, cl, (cudaStream_t)stream) : closed_loop_t<float>(pl, cl, (cudaStream_t)stream);
+}
+
+uint64_t mppi_plan_env_scratch_bytes(void* plan) {
+    const Plan* pl = reinterpret_cast<const Plan*>(plan);
+    return pl == nullptr ? 0 : env_scratch_bytes(pl);
+}
+
+int mppi_plan_set_env_params(void* plan, const MppiEnvParams* ep, void* stream) {
+    Plan* pl = reinterpret_cast<Plan*>(plan);
+    const int rc = check_env_params(pl, ep);
+    if (rc) return rc;
+    return pl->is_double ? set_env_params_t<double>(pl, ep, (cudaStream_t)stream) : set_env_params_t<float>(pl, ep, (cudaStream_t)stream);
 }
 
 int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint64_t seed, uint64_t offset, const void* z,
@@ -746,10 +874,13 @@ int mppi_user_model_register(const void* cubin, uint64_t cubin_bytes, int32_t nx
         }
         mk.split_ll[variant] = (const void*)k;
     }
-    // its global-tile kernels, exported under fixed names (MPPI_USER_KERNEL_GTILE / _BATCHED in mppi_fused.cuh)
-    const char* gnames[2] = {"mppi_user_fused_command_kernel_gtile", mk.batched != nullptr ? "mppi_user_fused_command_kernel_gtile_batched" : nullptr};
-    const void** gslots[2] = {&mk.gtile[variant], &mk.gtile_batched};
-    for (int i = 0; i < 2; ++i) {
+    // its global-tile kernels, exported under fixed names (MPPI_USER_KERNEL_GTILE / _BATCHED in mppi_fused.cuh), and beside
+    // the batched kernel its per-environment forms (MPPI_USER_KERNEL_ENV_BATCHED)
+    const bool b = mk.batched != nullptr;
+    const char* gnames[4] = {"mppi_user_fused_command_kernel_gtile", b ? "mppi_user_fused_command_kernel_gtile_batched" : nullptr,
+                             b ? "mppi_user_fused_command_kernel_env" : nullptr, b ? "mppi_user_fused_command_kernel_env_gtile" : nullptr};
+    const void** gslots[4] = {&mk.gtile[variant], &mk.gtile_batched, &mk.env_batched, &mk.env_gtile_batched};
+    for (int i = 0; i < 4; ++i) {
         if (gnames[i] == nullptr) continue;
         cudaKernel_t k = nullptr;
         cudaError_t e = cudaLibraryGetKernel(&k, lib, gnames[i]);

@@ -93,7 +93,12 @@ template <typename real> struct KArgs {
     // generic-path extras (sample_kernel / softmin_update_kernel)
     real* out_pa;
     real* out_noise;
-    real* out_noise_theta;
+    // The batched fused kernels read no generic-path extras: their per-environment noise models (n_env of them, or
+    // nullptr: every environment takes `nm`) share the space of sample_kernel's KMPPI output, so KArgs keeps its size.
+    union {
+        real* out_noise_theta;            // sample_kernel (KMPPI)
+        const NoiseModel<real>* env_nm;   // batched fused kernels (mppi_plan_set_env_params)
+    };
     real* out_cost_init;
     const real* override_rows;
     int n_override, override_start;
@@ -1143,13 +1148,20 @@ __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
 // ---- per-environment view of the kernel arguments (batched launches) -------------------------------
 // The argument block lives in constant (parameter) space; a batched CTA needs its environment's
 // pointers, so it builds an adjusted copy in shared memory once and every stage reads that copy.
-template <typename real, int NXv, int NUv>
+// ENV_NM (the batched fused kernels): the environment's own noise model replaces `nm` where env_nm is set.
+template <typename real, int NXv, int NUv, bool ENV_NM = false>
 __device__ void make_env_args(const KArgs<real>& in, KArgs<real>* out) {
     const int tid = threadIdx.x, BD = blockDim.x;
     const uint32_t* src = reinterpret_cast<const uint32_t*>(&in);
     uint32_t* dst = reinterpret_cast<uint32_t*>(out);
     for (int i = tid; i < (int)(sizeof(KArgs<real>) / 4); i += BD) dst[i] = src[i];
     __syncthreads();
+    if (ENV_NM && in.env_nm != nullptr) {
+        static_assert(sizeof(NoiseModel<real>) % 4 == 0, "word copy of the noise model");
+        const uint32_t* nsrc = reinterpret_cast<const uint32_t*>(in.env_nm + blockIdx.y);
+        uint32_t* ndst = reinterpret_cast<uint32_t*>(&out->nm);
+        for (int i = tid; i < (int)(sizeof(NoiseModel<real>) / 4); i += BD) ndst[i] = nsrc[i];
+    }
     if (tid == 0) {
         const long long e = blockIdx.y;
         const long long K = in.K, TN = in.TN, R = in.R;
@@ -1634,7 +1646,7 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
     extern __shared__ __align__(16) unsigned char smem[];
     const int tid = threadIdx.x, BD = blockDim.x;
     __shared__ __align__(16) unsigned char a_env_raw[BATCHED ? sizeof(KArgs<real>) : 16];
-    if (BATCHED) make_env_args<real, NX, NU>(a_in, reinterpret_cast<KArgs<real>*>(a_env_raw));
+    if (BATCHED) make_env_args<real, NX, NU, true>(a_in, reinterpret_cast<KArgs<real>*>(a_env_raw));
     const KArgs<real>& a = BATCHED ? *reinterpret_cast<const KArgs<real>*>(a_env_raw) : a_in;
     const int BS = BD / a.tps;
     const int xst = fused_xstage_doubles(a.world > 1 && !a.export_partial, a.world, a.xchg_npub, a.R);
@@ -1793,6 +1805,23 @@ __global__ void __launch_bounds__(512, FusedMinBlocks<Model>::value) fused_comma
     fused_command_body<Model, real, VARIANT, BATCHED, false, false, true>(a_in, mp);
 }
 
+// Batched environments with their own model parameters (mppi_plan_set_env_params): environment blockIdx.y's parameter
+// block is read in place, through L1, from the n_env blocks packed env_stride bytes apart (16-byte aligned, as the plant
+// blocks of a closed loop) — in place of the one block the other kernels take as a __grid_constant__ argument.
+// GTILE: the global-tile form.
+template <class Model, typename real, bool GTILE>
+__device__ __forceinline__ void fused_command_env_body(const KArgs<real>& a_in, const unsigned char* __restrict__ env_mp,
+                                                       long long env_stride) {
+    typedef typename Model::template P<real> P;
+    const P& mp = *reinterpret_cast<const P*>(env_mp + (size_t)blockIdx.y * (size_t)env_stride);
+    fused_command_body<Model, real, V_MPPI, true, false, false, GTILE>(a_in, mp);
+}
+template <class Model, typename real, bool GTILE>
+__global__ void __launch_bounds__(512, 1) fused_command_kernel_env(
+    const __grid_constant__ KArgs<real> a_in, const unsigned char* __restrict__ env_mp, long long env_stride) {
+    fused_command_env_body<Model, real, GTILE>(a_in, env_mp, env_stride);
+}
+
 #ifdef __CUDACC_RTC__
 // A user model (NVRTC, one module per dtype and controller variant) exports its fused_command_kernel_ll under one unmangled
 // name, which mppi_user_model_register looks up beside the kernels it is given by name.
@@ -1813,6 +1842,18 @@ __global__ void __launch_bounds__(512, FusedMinBlocks<Model>::value) fused_comma
         mppi_user_fused_command_kernel_gtile_batched(const __grid_constant__ mppi::KArgs<real> a_in,                         \
                                                      const __grid_constant__ Model::P<real> mp) {                            \
         mppi::fused_command_body<Model, real, mppi::V_MPPI, true, false, false, true>(a_in, mp);                             \
+    }
+// ... and, for MPPI_Batched, the batched kernels with per-environment model parameters (fused_command_kernel_env)
+#define MPPI_USER_KERNEL_ENV_BATCHED(Model, real)                                                                            \
+    extern "C" __global__ void __launch_bounds__(512, 1)                                                                     \
+        mppi_user_fused_command_kernel_env(const __grid_constant__ mppi::KArgs<real> a_in,                                   \
+                                           const unsigned char* __restrict__ env_mp, long long env_stride) {                 \
+        mppi::fused_command_env_body<Model, real, false>(a_in, env_mp, env_stride);                                          \
+    }                                                                                                                        \
+    extern "C" __global__ void __launch_bounds__(512, 1)                                                                     \
+        mppi_user_fused_command_kernel_env_gtile(const __grid_constant__ mppi::KArgs<real> a_in,                             \
+                                                 const unsigned char* __restrict__ env_mp, long long env_stride) {           \
+        mppi::fused_command_env_body<Model, real, true>(a_in, env_mp, env_stride);                                           \
     }
 #endif
 

@@ -58,6 +58,11 @@ struct Plan {
     alignas(16) unsigned char kargs[sizeof(KArgs<double>)];
     alignas(16) unsigned char mparams[MPPI_MODEL_BLOCK_BYTES];
     MppiTensorRef tensors[MPPI_MAX_MODEL_TENSORS];   // the plan's copy of p.model_tensors (p.model_tensors points here)
+    // per-environment model parameters (mppi_plan_set_env_params): the kernel that reads them and the packed blocks in
+    // the caller's scratch (env_kernel nullptr: the plan's own block, `kernel`)
+    const void* env_kernel;
+    const unsigned char* env_mp;
+    long long env_stride;
 };
 
 // What one (model, dtype) pair contributes: its kernels (as launchable handles) and how to pack its parameter block.
@@ -89,6 +94,9 @@ struct ModelKernels {
     int32_t tensor_dtype[MPPI_MAX_MODEL_TENSORS], tensor_ndim[MPPI_MAX_MODEL_TENSORS];
     const void* plant;               // plant_step_kernel<Model, real>: closed-loop episodes (nullptr: the PendulumMLP models,
                                      // step-dependent user models)
+    const void* env_batched;         // fused_command_kernel_env<Model, real, false>: MPPI_Batched with per-environment model
+                                     // parameters (nullptr: the PendulumMLP models)
+    const void* env_gtile_batched;   // fused_command_kernel_env<Model, real, true>
 };
 }  // namespace mppi_host
 

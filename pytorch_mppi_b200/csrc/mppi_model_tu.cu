@@ -90,6 +90,11 @@ const void* plant_kernel() {
     if constexpr (kIsMlp || kIsEnsemble) return nullptr;
     else return (const void*)plant_step_kernel<TuModel, TuReal>;
 }
+// MPPI_Batched with per-environment model parameters: not for the MLP models (their 1,250-weight blocks)
+template <bool GTILE> const void* env_kernel() {
+    if constexpr (kIsMlp || kIsEnsemble) return nullptr;
+    else return (const void*)fused_command_kernel_env<TuModel, TuReal, GTILE>;
+}
 template <int V, int SPLIT, int FAST> const void* tc_kernel() {
     if constexpr (kIsMlp && !MPPI_TU_F64) return (const void*)mlp_tc_command_kernel<V, SPLIT, FAST>;
     else if constexpr (kIsEnsemble && !MPPI_TU_F64) return (const void*)mlp_ens_tc_command_kernel<V, SPLIT, FAST>;
@@ -113,6 +118,8 @@ const ModelKernels g_kernels = {
      {{tc_kernel<V_KMPPI, 1, 0>(), tc_kernel<V_KMPPI, 1, 1>()}, {tc_kernel<V_KMPPI, 0, 0>(), tc_kernel<V_KMPPI, 0, 1>()}}},
     nullptr, 0, 0, {}, {},
     plant_kernel(),
+    env_kernel<false>(),
+    env_kernel<true>(),
 };
 
 }  // namespace

@@ -80,6 +80,16 @@ def _pad16(n_elems, es):
     return (n_elems * es + 15) // 16 * 16 // es
 
 
+def _factor_sigma(sigma):
+    """The reference's factoring of a (nu, nu) noise covariance (mppi.py:131-139) -> (diagonal, Cholesky factor L,
+    inverse, sqrt of the diagonal or None): the diagonal test, then sqrt / 1/diag, or cholesky / inv."""
+    if bool(torch.equal(sigma, torch.diag(torch.diag(sigma)))):                               # mppi.py:131
+        diag = torch.diag(sigma)
+        sqrt_diag = torch.sqrt(diag)
+        return True, torch.diag(sqrt_diag), torch.diag(1.0 / diag), sqrt_diag
+    return False, torch.linalg.cholesky(sigma), torch.linalg.inv(sigma), None                 # mppi.py:138-139
+
+
 def fused_route_model(dynamics, running_cost, terminal_state_cost, nx, nu, rollout_samples, specific_action_sampler,
                       step_dependent_dynamics) -> typing.Optional[AnalyticModel]:
     """The registered model a controller with these arguments runs on the fused route, or None (stepped route).
@@ -279,16 +289,9 @@ class MPPI:
     # ------------------------------------------------------------------------------------------
     def _set_sigma(self, sigma):
         self._noise_sigma = sigma
-        self._diagonal_sigma = bool(torch.equal(sigma, torch.diag(torch.diag(sigma))))     # mppi.py:131
+        self._diagonal_sigma, self._chol, self._noise_sigma_inv, self._noise_sigma_sqrt_diag = _factor_sigma(sigma)
         if self._diagonal_sigma:
-            diag = torch.diag(sigma)
-            self._noise_sigma_inv_diag = 1.0 / diag
-            self._noise_sigma_sqrt_diag = torch.sqrt(diag)
-            self._noise_sigma_inv = torch.diag(self._noise_sigma_inv_diag)
-            self._chol = torch.diag(self._noise_sigma_sqrt_diag)
-        else:
-            self._noise_sigma_inv = torch.linalg.inv(sigma)                                  # mppi.py:138-139
-            self._chol = torch.linalg.cholesky(sigma)
+            self._noise_sigma_inv_diag = torch.diag(self._noise_sigma_inv)
         self._dirty = True
 
     noise_sigma = property(lambda self: self._noise_sigma, lambda self, v: self._set_sigma(torch.as_tensor(v).to(self.d, self.dtype).reshape(self.nu, self.nu)))
@@ -1706,6 +1709,10 @@ class MPPI_Batched(MPPI):
                  step_dependent_dynamics=False, noise_abs_cost=False, *, rng_seed=None, block_threads=0,
                  tile_memory="shared"):
         self.N = int(num_envs)
+        # per-environment settings (set_env_params): None = the controller's shared value
+        self._env_model_params = self._env_lambda = self._env_sigma = self._env_mu = None
+        self._env_factors = None          # (diagonal, L, inverse, sqrt-diagonal) per environment of _env_sigma
+        self._env_scratch = None          # device blocks the plan reads (mppi_plan_set_env_params)
         super().__init__(dynamics, running_cost, nx, noise_sigma, num_samples=num_samples, horizon=horizon, device=device,
                          lambda_=lambda_, noise_mu=noise_mu, u_min=u_min, u_max=u_max, u_init=u_init, u_scale=u_scale,
                          u_per_command=u_per_command, step_dependent_dynamics=step_dependent_dynamics,
@@ -1743,6 +1750,144 @@ class MPPI_Batched(MPPI):
     def reset(self):
         """mppi.py:819-820"""
         self.U = self._sample_noise((self.N, self.T))
+
+    def _sample_noise(self, shape):
+        """As MPPI's; with per-environment noise (set_env_params), environment e's rows are coloured with its own
+        N(mu_e, Sigma_e) from the same standard normals."""
+        if self._env_sigma is None and self._env_mu is None:
+            return super()._sample_noise(shape)
+        z = torch.randn(*shape, self.nu, device=self.d, dtype=self.dtype)
+        out = torch.empty_like(z)
+        for e in range(self.N):
+            diag, L, _, sqrt_diag = self._env_factors[e] if self._env_factors is not None else \
+                (self._diagonal_sigma, self._chol, None, self._noise_sigma_sqrt_diag)
+            mu = self._env_mu[e] if self._env_mu is not None else self._noise_mu
+            out[e] = z[e] * sqrt_diag + mu if diag else z[e] @ L.T + mu
+        return out
+
+    # ---- per-environment settings ------------------------------------------------------------------
+    def set_env_params(self, model_params=None, lambda_=None, noise_sigma=None, noise_mu=None):
+        """Give each environment its own model parameters, temperature and noise (registered models and CudaModels on
+        the fused route).  The K standard normals stay shared: environment e colours them with its own Sigma_e and
+        mu_e and weights them with its own lambda_e, so its command is the single-environment MPPI command with e's
+        settings on the same draws.
+
+        model_params  (N, n_params) floats in the model's own layout, ``param_blob() + param_blob_ext()`` (a CudaModel:
+                      its `params`; its device tensors stay shared), as run_closed_loop's plant_params
+        lambda_       (N,) temperatures > 0
+        noise_sigma   (N, nu, nu) symmetric positive definite covariances; each is factored as the reference factors
+                      one (diagonal: sqrt / 1/diag, else cholesky / inv), so diagonal and full ones may be mixed
+        noise_mu      (N, nu) noise means
+        An argument left None stays shared (the controller's own value applies to every environment);
+        ``set_env_params()`` returns to fully shared settings.  The values take effect at the next command, without a new
+        plan; commands already enqueued keep the values they were launched with.  With model parameters and
+        plant_params=None, run_closed_loop's plant of environment e is the model with e's parameters."""
+        N, nu = self.N, self.nu
+        given = [v is not None for v in (model_params, lambda_, noise_sigma, noise_mu)]
+        m = self._model
+        if any(given) and m is None:
+            raise ValueError("set_env_params: per-environment settings run on the fused route only (registered models and "
+                             "CudaModels); arbitrary dynamics / cost callables take the stepped route")
+
+        def host(v, name, shape):
+            t = v if torch.is_tensor(v) else torch.as_tensor(v, dtype=torch.float64)
+            if not t.is_floating_point() or t.dtype not in (torch.float32, torch.float64):
+                raise ValueError(f"set_env_params: {name} must be float32 or float64, got {t.dtype}")
+            if t.device not in (torch.device("cpu"), self.d):
+                raise ValueError(f"set_env_params: {name} must be on the CPU or {self.d}, got {t.device}")
+            if tuple(t.shape) != shape:
+                raise ValueError(f"set_env_params: {name} must have shape {shape}, got {tuple(t.shape)}")
+            if not bool(torch.isfinite(t).all()):
+                raise ValueError(f"set_env_params: {name} has non-finite values")
+            return t.detach()
+
+        mp = lam = sig = mu = factors = None
+        if model_params is not None:
+            if m.model_id in (_cabi.MODEL_PENDULUM_MLP, _cabi.MODEL_PENDULUM_MLP_ENSEMBLE):
+                raise ValueError("set_env_params: model_params are not available for the PendulumMLP models (their "
+                                 "1,250-weight blocks)")
+            n_params = len(m.param_blob()) + len(m.param_blob_ext())
+            mp = host(model_params, "model_params", (N, n_params)).to("cpu", torch.float64).contiguous()
+        if lambda_ is not None:
+            lam = host(lambda_, "lambda_", (N,)).to("cpu", torch.float64).contiguous()
+            if not bool((lam > 0).all()):
+                raise ValueError(f"set_env_params: every lambda_ must be > 0, got {lam.tolist()}")
+        if noise_sigma is not None:
+            sig = host(noise_sigma, "noise_sigma", (N, nu, nu)).to(self.d, self.dtype)
+            factors = []
+            for e in range(N):
+                s = sig[e]
+                if not torch.equal(s, s.T):
+                    raise ValueError(f"set_env_params: noise_sigma[{e}] is not symmetric")
+                try:
+                    f = _factor_sigma(s)
+                except RuntimeError as err:       # torch.linalg.cholesky: not positive definite
+                    raise ValueError(f"set_env_params: noise_sigma[{e}] is not positive definite") from err
+                if f[0] and not bool((torch.diag(s) > 0).all()):
+                    raise ValueError(f"set_env_params: noise_sigma[{e}] is not positive definite")
+                factors.append(f)
+        if noise_mu is not None:
+            mu = host(noise_mu, "noise_mu", (N, nu)).to(self.d, self.dtype)
+        self._env_model_params, self._env_lambda, self._env_sigma, self._env_mu = mp, lam, sig, mu
+        self._env_factors = factors
+        if self._plan is not None:
+            self._apply_env_params()
+
+    env_model_params = property(lambda self: self._env_model_params,
+                                doc="(N, n_params) float64 per-environment model parameters, or None (shared)")
+    env_lambda = property(lambda self: self._env_lambda, doc="(N,) float64 per-environment temperatures, or None (shared)")
+    env_noise_sigma = property(lambda self: self._env_sigma, doc="(N, nu, nu) per-environment covariances, or None (shared)")
+    env_noise_mu = property(lambda self: self._env_mu, doc="(N, nu) per-environment noise means, or None (shared)")
+
+    def _env_arrays(self):
+        """The host arrays of MppiEnvParams (None where shared), in the library's MPPI_MAX_NU layout."""
+        N, nu, MU = self.N, self.nu, _cabi.MPPI_MAX_NU
+
+        def arr(t):
+            t = t.detach().to("cpu", torch.float64).contiguous().reshape(-1)
+            return (C.c_double * t.numel())(*t.tolist())
+        lam = None if self._env_lambda is None else arr(self._env_lambda)
+        chol = sinv = mu = mp = None
+        if self._env_factors is not None:
+            L = torch.zeros(N, MU, MU, dtype=torch.float64)
+            Si = torch.zeros(N, MU, MU, dtype=torch.float64)
+            for e, (_, le, ie, _) in enumerate(self._env_factors):
+                L[e, :nu, :nu] = le.detach().to("cpu", torch.float64)
+                Si[e, :nu, :nu] = ie.detach().to("cpu", torch.float64)
+            chol, sinv = arr(L), arr(Si)
+        if self._env_mu is not None:
+            m = torch.zeros(N, MU, dtype=torch.float64)
+            m[:, :nu] = self._env_mu.detach().to("cpu", torch.float64)
+            mu = arr(m)
+        if self._env_model_params is not None:
+            mp = arr(self._env_model_params)
+        return lam, chol, sinv, mu, mp
+
+    def _apply_env_params(self):
+        """Hand the per-environment settings to the plan (mppi_plan_set_env_params): no new plan."""
+        lam, chol, sinv, mu, mp = self._env_arrays()
+        lib = self._lib
+        ptr = lambda a: None if a is None else C.cast(a, C.c_void_p)
+        ep = _cabi.MppiEnvParams(struct_size=C.sizeof(_cabi.MppiEnvParams), n_env=self.N, lambda_=ptr(lam), chol=ptr(chol),
+                                 sigma_inv=ptr(sinv), noise_mu=ptr(mu), model_params=ptr(mp),
+                                 n_model_params=0 if self._env_model_params is None else self._env_model_params.shape[1])
+        if any(a is not None for a in (lam, chol, mu, mp)):
+            need = int(lib.mppi_plan_env_scratch_bytes(self._plan))
+            if self._env_scratch is None or self._env_scratch.numel() < need:
+                self._env_scratch = torch.empty(need, device=self.d, dtype=torch.uint8)
+            ep.scratch, ep.scratch_bytes = self._env_scratch.data_ptr(), self._env_scratch.numel()
+        stream = torch._C._cuda_getCurrentRawStream(self.d.index)
+        _cabi.check(lib.mppi_plan_set_env_params(self._plan, C.byref(ep), stream), "mppi_plan_set_env_params")
+
+    def _make_plan(self, p):
+        super()._make_plan(p)
+        if any(v is not None for v in (self._env_model_params, self._env_lambda, self._env_sigma, self._env_mu)):
+            self._apply_env_params()
+
+    def _take_model_params(self):
+        super()._take_model_params()
+        if self._env_model_params is not None:      # the blocks carry the CudaModel's tensor views: re-pack them
+            self._apply_env_params()
 
     def shift_nominal_trajectory(self):
         U = torch.roll(self.U, -1, dims=1)
@@ -1824,6 +1969,9 @@ class MPPI_Batched(MPPI):
             return None
         beta = self._stats[:, 0:1].to(self.dtype)
         eta = self._stats[:, 1:2].to(self.dtype)
+        if self._env_lambda is not None:          # each environment's own temperature
+            f = (-(1.0 / self._env_lambda)).to(self.d, self.dtype).view(self.N, 1)
+            return torch.exp(f * (self.cost_total - beta)) / eta
         return torch.exp(-(1.0 / self._lambda) * (self.cost_total - beta)) / eta
 
 

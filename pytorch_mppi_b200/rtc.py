@@ -98,6 +98,8 @@ def compile_user_model(header_text: str, real: str, variant: int, copies: int = 
     src += f"MPPI_USER_KERNEL_GTILE(mppi::UserModel, {real}, {variant})\n"
     if variant == 0 and copies == 1:
         src += f"MPPI_USER_KERNEL_GTILE_BATCHED(mppi::UserModel, {real})\n"
+        # MPPI_Batched with per-environment model parameters (set_env_params)
+        src += f"MPPI_USER_KERNEL_ENV_BATCHED(mppi::UserModel, {real})\n"
     if plant:         # the plant step of closed-loop episodes (run_closed_loop)
         src += f"MPPI_USER_KERNEL_PLANT(mppi::UserModel, {real})\n"
     # keyed by the whole program (model, exported kernels) and the kernel headers it includes: a module built before a
