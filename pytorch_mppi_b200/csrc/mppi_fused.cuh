@@ -25,9 +25,6 @@
 #endif
 #include "mppi_math.cuh"
 
-#ifndef MPPI_ROLLOUT_PIPELINED
-#define MPPI_ROLLOUT_PIPELINED 0
-#endif
 #ifndef MPPI_ROLLOUT_UNROLL
 #define MPPI_ROLLOUT_UNROLL 2
 #endif
@@ -1187,10 +1184,9 @@ __device__ void make_env_args(const KArgs<real>& in, KArgs<real>* out) {
     __syncthreads();
 }
 
-// ---- Rollouts of models with a fast range (FastRange, mppi_math.cuh).  Every thread of a sample checks
-// in_fast_range on x_0; when it holds, the sample's rollout runs on the model's fast step and cost, inlined; when it
-// does not (a start far out, or a non-finite one), on the exact forms, out of line.  Models without a fast range keep
-// the rollouts below these (split_cost_rollout's own body and the kernel's single loop) as they are.
+// ---- Rollouts.  A model with a fast range (FastRange, mppi_math.cuh) checks in_fast_range on x_0; when it holds, the
+// sample's rollout runs on the model's fast step and cost, inlined; when it does not (a start far out, or a non-finite
+// one), on the exact forms, out of line.  Every other model runs the exact forms inline.
 
 // the rollout thread's state at t = 0 (mppi.py:303-305): the controller's state, or the sample's own (state_per_sample)
 template <typename real, int NX>
@@ -1212,15 +1208,44 @@ template <typename real, int NX> struct RolloutCarry {
     real roll, pert, smooth;
 };
 
+// step t's action cost (mppi.py:409, 415) added to pert and, for SMPPI, the step's smoothness (mppi.py:559-562) added to
+// smooth; vprev carries the previous perturbed action from step to step (zeros before t = 0)
+template <typename real, int VARIANT, int NU>
+__device__ __forceinline__ void action_terms(const NoiseModel<real>& nm, const real* us, int t, const real* v, const real* eps,
+                                             real& pert, real& smooth, real* vprev) {
+    typedef Ops<real> O;
+    pert = O::add(pert, action_cost_term<real, NU>(nm, eps, us));
+    if (VARIANT == V_SMPPI) {
+        if (t > 0) {
+#pragma unroll
+            for (int n = 0; n < NU; ++n) {
+                const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
+                smooth = O::add(smooth, O::mul(d, d));
+            }
+        }
+#pragma unroll
+        for (int n = 0; n < NU; ++n) vprev[n] = v[n];
+    }
+}
+
+// the sample's total cost from its rollout cost, action cost and SMPPI smoothness, stored to cost_total[k]
+template <typename real, int VARIANT>
+__device__ __forceinline__ real sample_total(const KArgs<real>& a, int k, real roll, real pert, real smooth) {
+    typedef Ops<real> O;
+    real c_tot = O::add(roll, pert);                                                  // mppi.py:416
+    if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, a.nm.w_smooth));    // mppi.py:562,569
+    a.cost_total[k] = c_tot;
+    return c_tot;
+}
+
 // the recurrence of the split-cost rollout on the sample's rollout thread: every x_t to the sample's column of xs, the
 // action cost (and SMPPI smoothness) accumulated alongside.  FAST: the model's fast step.
 template <class Model, typename real, int VARIANT, bool FAST>
 __device__ __forceinline__ void split_recurrence(const KArgs<real>& a, const typename Model::template P<real>& mp, const Smem<real>& sm,
-                                                 unsigned long long kg, real* xcol, RolloutCarry<real, Model::NX>& c) {
+                                                 unsigned long long kg, real* xcol, int BS, int T, real* x, real& pert, real& smooth) {
     typedef Ops<real> O;
     constexpr int NX = Model::NX, NU = Model::NU;
     const NoiseModel<real>& nm = a.nm;
-    const int BS = blockDim.x / a.tps, T = a.T;
     real vprev[NU];
 #pragma unroll
     for (int n = 0; n < NU; ++n) vprev[n] = (real)0;
@@ -1231,21 +1256,10 @@ MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
         noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
 #pragma unroll
         for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
-        model_step<Model, real, FAST>(mp, c.x, u, t);                             // mppi.py:314
+        model_step<Model, real, FAST>(mp, x, u, t);                               // mppi.py:314
 #pragma unroll
-        for (int i = 0; i < NX; ++i) xcol[(t * NX + i) * BS] = c.x[i];
-        c.pert = O::add(c.pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
-        if (VARIANT == V_SMPPI) {
-            if (t > 0) {
-#pragma unroll
-                for (int n = 0; n < NU; ++n) {
-                    const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
-                    c.smooth = O::add(c.smooth, O::mul(d, d));
-                }
-            }
-#pragma unroll
-            for (int n = 0; n < NU; ++n) vprev[n] = v[n];
-        }
+        for (int i = 0; i < NX; ++i) xcol[(t * NX + i) * BS] = x[i];
+        action_terms<real, VARIANT, NU>(nm, sm.Us + t * NU, t, v, eps, pert, smooth, vprev);
     }
 }
 
@@ -1271,17 +1285,16 @@ template <class Model, typename real, int VARIANT>
 __device__ __noinline__ RolloutCarry<real, Model::NX> split_recurrence_rare(const KArgs<real>& a, const typename Model::template P<real>& mp,
                                                                             const RolloutTiles<real> tiles, unsigned long long kg, real* xcol,
                                                                             RolloutCarry<real, Model::NX> c) {
-    split_recurrence<Model, real, VARIANT, false>(a, mp, tiles.smem(), kg, xcol, c);
+    split_recurrence<Model, real, VARIANT, false>(a, mp, tiles.smem(), kg, xcol, blockDim.x / a.tps, a.T, c.x, c.pert, c.smooth);
     return c;
 }
 
 // the T running costs of a split-cost rollout, spread over the sample's tps threads: cost_t overwrites x_t[0] in xs
 template <class Model, typename real, int VARIANT, bool FAST>
 __device__ __forceinline__ void split_costs(const KArgs<real>& a, const typename Model::template P<real>& mp, const Smem<real>& sm,
-                                            unsigned long long kg, real* xcol) {
+                                            unsigned long long kg, real* xcol, int tid, int BS, int T) {
     typedef Ops<real> O;
     constexpr int NX = Model::NX, NU = Model::NU;
-    const int tid = threadIdx.x, BS = blockDim.x / a.tps, T = a.T;
 MPPI_UNROLL_N(2)
     for (int t = tid / BS; t < T; t += a.tps) {      // independent across t: two in flight per thread
         real v[NU], u[NU], xt[NX];
@@ -1294,90 +1307,85 @@ MPPI_UNROLL_N(2)
     }
 }
 
-// split_cost_rollout of a model with a fast range
+// ---- stage C', split-cost rollout as a function: recurrence on the rollout thread | running costs on all tps
+// threads of the sample | ordered sum.  Returns the sample's total cost on its rollout thread (+inf elsewhere) and
+// stores it to cost_total[k].  Contains two CTA barriers: every thread must call it.
+// Shared by fused_command_kernel<..., SPLIT = true> and the resident kernel (mppi_resident.cuh).
+// A model with a fast range has every thread of the sample read x_0 and check in_fast_range, so that its running costs
+// take the form its recurrence took; other models read x_0 on the rollout thread only.
 template <class Model, typename real, int VARIANT>
-__device__ __forceinline__ real split_cost_rollout_fast(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
-                                                        int k, unsigned long long kg, bool in_range, bool active) {
+__device__ __forceinline__ real split_cost_rollout(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
+                                                   int k, unsigned long long kg, bool in_range, bool active) {
+    static_assert(ModelCopies<Model>::value == 1, "models with COPIES > 1 run the single-loop rollout (copies_rollout)");
     typedef Ops<real> O;
     constexpr int NX = Model::NX;
+    constexpr bool FR = FastRange<Model, real>::value;
     const int tid = threadIdx.x, BS = blockDim.x / a.tps, T = a.T;
     real c_tot = O::inf();
     real* xcol = sm.xs + (tid % BS);
     RolloutCarry<real, NX> c;
     c.pert = (real)0;
     c.smooth = (real)0;
-    bool fast = false;
-    if (in_range) {
-        initial_state<real, NX>(a, k, c.x);
-        fast = Model::template in_fast_range<real>(mp, c.x, T);
-    }
-    if (active) {
-        if (fast) split_recurrence<Model, real, VARIANT, true>(a, mp, sm, kg, xcol, c);
-        else c = split_recurrence_rare<Model, real, VARIANT>(a, mp, RolloutTiles<real>(sm), kg, xcol, c);
-    }
-    __syncthreads();
-    if (in_range) {
-        if (fast) split_costs<Model, real, VARIANT, true>(a, mp, sm, kg, xcol);
-        else split_costs<Model, real, VARIANT, false>(a, mp, sm, kg, xcol);
+    if constexpr (FR) {
+        // the fast path reads its sizes where it uses them, the form its kernels (C2, C5) are tuned in
+        bool fast = false;
+        if (in_range) {
+            initial_state<real, NX>(a, k, c.x);
+            fast = Model::template in_fast_range<real>(mp, c.x, T);
+        }
+        if (active) {
+            if (fast) split_recurrence<Model, real, VARIANT, true>(a, mp, sm, kg, xcol, blockDim.x / a.tps, a.T, c.x, c.pert, c.smooth);
+            else c = split_recurrence_rare<Model, real, VARIANT>(a, mp, RolloutTiles<real>(sm), kg, xcol, c);
+        }
+        __syncthreads();
+        if (in_range) {
+            const int tid_ = threadIdx.x, BS_ = blockDim.x / a.tps, T_ = a.T;
+            if (fast) split_costs<Model, real, VARIANT, true>(a, mp, sm, kg, xcol, tid_, BS_, T_);
+            else split_costs<Model, real, VARIANT, false>(a, mp, sm, kg, xcol, tid_, BS_, T_);
+        }
+    } else {
+        if (active) {
+            initial_state<real, NX>(a, k, c.x);
+            split_recurrence<Model, real, VARIANT, false>(a, mp, sm, kg, xcol, BS, T, c.x, c.pert, c.smooth);
+        }
+        __syncthreads();
+        if (in_range) split_costs<Model, real, VARIANT, false>(a, mp, sm, kg, xcol, tid, BS, T);
     }
     __syncthreads();
     if (active) {
         real roll = (real)0;
         for (int t = 0; t < T; ++t) roll = O::add(roll, xcol[(t * NX) * BS]);         // mppi.py:319, t = 0..T-1
         if (Model::template has_terminal<real>(mp)) roll = O::add(roll, Model::template terminal<real>(mp, c.x));
-        c_tot = O::add(roll, c.pert);                                                 // mppi.py:416
-        if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(c.smooth, a.nm.w_smooth));  // mppi.py:562,569
-        a.cost_total[k] = c_tot;
+        c_tot = sample_total<real, VARIANT>(a, k, roll, c.pert, c.smooth);
     }
     return c_tot;
 }
 
-// the single-loop rollout (the kernel's stage C) on the sample's rollout thread: dynamics, running cost, action cost
-// (and SMPPI smoothness) per step, as the kernel's own loop.  FAST: the model's fast step and cost.
+// the single-loop rollout on the sample's rollout thread: dynamics, running cost, action cost (and SMPPI smoothness)
+// per step.  FAST: the model's fast step and cost.
 template <class Model, typename real, int VARIANT, bool FAST>
 __device__ __forceinline__ void single_loop(const KArgs<real>& a, const typename Model::template P<real>& mp, const Smem<real>& sm,
-                                            unsigned long long kg, RolloutCarry<real, Model::NX>& c) {
+                                            unsigned long long kg, int T, real* x, real& roll, real& pert, real& smooth) {
     typedef Ops<real> O;
-    constexpr int NX = Model::NX, NU = Model::NU;
+    constexpr int NU = Model::NU;
     const NoiseModel<real>& nm = a.nm;
-    const int T = a.T;
-    real vprev[NU], uprev[NU];
+    real vprev[NU];
 #pragma unroll
-    for (int n = 0; n < NU; ++n) { vprev[n] = (real)0; uprev[n] = (real)0; }
+    for (int n = 0; n < NU; ++n) vprev[n] = (real)0;
+    // The running cost of the state reached at step t-1 and the dynamics of step t both depend only on x_t, so the
+    // unrolled loop issues them back to back: the single resident warp gets two independent dependency chains.  The
+    // arithmetic and the order of every accumulation are exactly the reference's (cost summed t = 0..T-1).
 MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
     for (int t = 0; t < T; ++t) {
-        real v[NU], u[NU], eps[NU], xs[NX];
+        real v[NU], u[NU], eps[NU];
         action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
         noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
 #pragma unroll
         for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
-#pragma unroll
-        for (int i = 0; i < NX; ++i) xs[i] = c.x[i];
-#if MPPI_ROLLOUT_PIPELINED
-        model_step<Model, real, FAST>(mp, c.x, u, t);                             // mppi.py:314
-        if (t > 0) c.roll = O::add(c.roll, model_cost<Model, real, FAST>(mp, xs, uprev, t - 1));   // mppi.py:318-319 (step t-1)
-#else
-        model_step<Model, real, FAST>(mp, c.x, u, t);                             // mppi.py:314
-        c.roll = O::add(c.roll, model_cost<Model, real, FAST>(mp, c.x, u, t));    // mppi.py:318-319
-#endif
-        c.pert = O::add(c.pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
-        if (VARIANT == V_SMPPI) {
-            if (t > 0) {
-#pragma unroll
-                for (int n = 0; n < NU; ++n) {
-                    const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
-                    c.smooth = O::add(c.smooth, O::mul(d, d));
-                }
-            }
-#pragma unroll
-            for (int n = 0; n < NU; ++n) vprev[n] = v[n];
-        }
-#pragma unroll
-        for (int n = 0; n < NU; ++n) uprev[n] = u[n];
+        model_step<Model, real, FAST>(mp, x, u, t);                               // mppi.py:314
+        roll = O::add(roll, model_cost<Model, real, FAST>(mp, x, u, t));          // mppi.py:318-319
+        action_terms<real, VARIANT, NU>(nm, sm.Us + t * NU, t, v, eps, pert, smooth, vprev);
     }
-#if MPPI_ROLLOUT_PIPELINED
-    c.roll = O::add(c.roll, model_cost<Model, real, FAST>(mp, c.x, uprev, T - 1));  // step T-1
-#endif
 }
 
 // single_loop on the exact step and cost, out of line (as split_recurrence_rare)
@@ -1385,107 +1393,30 @@ template <class Model, typename real, int VARIANT, bool G = false>      // G: as
 __device__ __noinline__ RolloutCarry<real, Model::NX> single_loop_rare(const KArgs<real>& a, const typename Model::template P<real>& mp,
                                                                        const RolloutTiles<real> tiles, unsigned long long kg,
                                                                        RolloutCarry<real, Model::NX> c) {
-    single_loop<Model, real, VARIANT, false>(a, mp, tiles.smem(), kg, c);
+    single_loop<Model, real, VARIANT, false>(a, mp, tiles.smem(), kg, a.T, c.x, c.roll, c.pert, c.smooth);
     return c;
 }
 
-// the single-loop rollout of a model with a fast range: stores cost_total[k] and returns it
+// ---- stage C, the single-loop rollout (mppi.py:297-332) + action cost (mppi.py:409,415) [+ smoothness :559-562] on the
+// sample's rollout thread: stores cost_total[k] and returns it.  T: the horizon as the kernel read it at entry; a model with
+// a fast range reads it here instead (the form its kernels are tuned in: scripts/sass_rollout_loop.py).
 template <class Model, typename real, int VARIANT, bool GTILE = false>
-__device__ __forceinline__ real single_loop_rollout_fast(const KArgs<real>& a, const typename Model::template P<real>& mp,
-                                                         const Smem<real>& sm, int k, unsigned long long kg) {
+__device__ __forceinline__ real single_loop_rollout(const KArgs<real>& a, const typename Model::template P<real>& mp,
+                                                    const Smem<real>& sm, int k, unsigned long long kg, int T) {
     typedef Ops<real> O;
     RolloutCarry<real, Model::NX> c;
     initial_state<real, Model::NX>(a, k, c.x);
     c.roll = (real)0;
     c.pert = (real)0;
     c.smooth = (real)0;
-    if (Model::template in_fast_range<real>(mp, c.x, a.T)) single_loop<Model, real, VARIANT, true>(a, mp, sm, kg, c);
-    else c = single_loop_rare<Model, real, VARIANT, GTILE>(a, mp, RolloutTiles<real>(sm), kg, c);
-    if (Model::template has_terminal<real>(mp)) c.roll = O::add(c.roll, Model::template terminal<real>(mp, c.x));
-    real c_tot = O::add(c.roll, c.pert);                                              // mppi.py:416
-    if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(c.smooth, a.nm.w_smooth));  // mppi.py:562,569
-    a.cost_total[k] = c_tot;
-    return c_tot;
-}
-
-// ---- stage C', split-cost rollout as a function: recurrence on the rollout thread | running costs on all tps
-// threads of the sample | ordered sum.  Returns the sample's total cost on its rollout thread (+inf elsewhere) and
-// stores it to cost_total[k].  Contains two CTA barriers: every thread must call it.
-// Shared by fused_command_kernel<..., SPLIT = true> and the resident kernel (mppi_resident.cuh).
-template <class Model, typename real, int VARIANT>
-__device__ __forceinline__ real split_cost_rollout(const KArgs<real>& a, const typename Model::template P<real>& mp, Smem<real>& sm,
-                                                   int k, unsigned long long kg, bool in_range, bool active) {
-    static_assert(ModelCopies<Model>::value == 1, "models with COPIES > 1 run the single-loop rollout (copies_rollout)");
-    if constexpr (FastRange<Model, real>::value) return split_cost_rollout_fast<Model, real, VARIANT>(a, mp, sm, k, kg, in_range, active);
-    else {
-        typedef Ops<real> O;
-        constexpr int NX = Model::NX, NU = Model::NU;
-        const NoiseModel<real>& nm = a.nm;
-        const int tid = threadIdx.x, BS = blockDim.x / a.tps, T = a.T;
-        real c_tot = O::inf();
-        real* xcol = sm.xs + (tid % BS);
-        real x[NX];
-        real pert = (real)0, smooth = (real)0;
-        if (active) {
-            if (a.state_dev != nullptr) {
-                const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
-#pragma unroll
-                for (int i = 0; i < NX; ++i) x[i] = sp[i];
-            } else {
-#pragma unroll
-                for (int i = 0; i < NX; ++i) x[i] = a.x0[i];
-            }
-            real vprev[NU];
-#pragma unroll
-            for (int n = 0; n < NU; ++n) vprev[n] = (real)0;
-MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
-            for (int t = 0; t < T; ++t) {
-                real v[NU], u[NU], eps[NU];
-                action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
-                noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
-#pragma unroll
-                for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
-                model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
-#pragma unroll
-                for (int i = 0; i < NX; ++i) xcol[(t * NX + i) * BS] = x[i];
-                pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
-                if (VARIANT == V_SMPPI) {
-                    if (t > 0) {
-#pragma unroll
-                        for (int n = 0; n < NU; ++n) {
-                            const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
-                            smooth = O::add(smooth, O::mul(d, d));
-                        }
-                    }
-#pragma unroll
-                    for (int n = 0; n < NU; ++n) vprev[n] = v[n];
-                }
-            }
-        }
-        __syncthreads();
-        if (in_range) {
-MPPI_UNROLL_N(2)
-            for (int t = tid / BS; t < T; t += a.tps) {      // independent across t: two in flight per thread
-                real v[NU], u[NU], xt[NX];
-                action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
-#pragma unroll
-                for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);
-#pragma unroll
-                for (int i = 0; i < NX; ++i) xt[i] = xcol[(t * NX + i) * BS];
-                xcol[(t * NX) * BS] = model_cost<Model, real>(mp, xt, u, t);              // mppi.py:318
-            }
-        }
-        __syncthreads();
-        if (active) {
-            real roll = (real)0;
-            for (int t = 0; t < T; ++t) roll = O::add(roll, xcol[(t * NX) * BS]);         // mppi.py:319, t = 0..T-1
-            if (Model::template has_terminal<real>(mp)) roll = O::add(roll, Model::template terminal<real>(mp, x));
-            c_tot = O::add(roll, pert);                                                   // mppi.py:416
-            if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));   // mppi.py:562,569
-            a.cost_total[k] = c_tot;
-        }
-        return c_tot;
+    if constexpr (FastRange<Model, real>::value) {
+        if (Model::template in_fast_range<real>(mp, c.x, a.T)) single_loop<Model, real, VARIANT, true>(a, mp, sm, kg, a.T, c.x, c.roll, c.pert, c.smooth);
+        else c = single_loop_rare<Model, real, VARIANT, GTILE>(a, mp, RolloutTiles<real>(sm), kg, c);
+    } else {
+        single_loop<Model, real, VARIANT, false>(a, mp, sm, kg, T, c.x, c.roll, c.pert, c.smooth);
     }
+    if (Model::template has_terminal<real>(mp)) c.roll = O::add(c.roll, Model::template terminal<real>(mp, c.x));
+    return sample_total<real, VARIANT>(a, k, c.roll, c.pert, c.smooth);
 }
 
 // one step's costs c[0..M-1] of the M copies (mppi.py:362-364): cs[m] += c[m], and var += var_m(c) * disc with the
@@ -1530,14 +1461,7 @@ __device__ __forceinline__ real copies_rollout(const KArgs<real>& a, const typen
     const NoiseModel<real>& nm = a.nm;
     const int T = a.T;
     real x[M][NX];
-    if (a.state_dev != nullptr) {
-        const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
-#pragma unroll
-        for (int i = 0; i < NX; ++i) x[0][i] = sp[i];
-    } else {
-#pragma unroll
-        for (int i = 0; i < NX; ++i) x[0][i] = a.x0[i];
-    }
+    initial_state<real, NX>(a, k, x[0]);
     real cs[M];
 #pragma unroll
     for (int m = 0; m < M; ++m) {
@@ -1546,57 +1470,23 @@ __device__ __forceinline__ real copies_rollout(const KArgs<real>& a, const typen
         for (int i = 0; i < NX; ++i) x[m][i] = x[0][i];
     }
     real var = (real)0, pert = (real)0, smooth = (real)0;
-    real vprev[NU], uprev[NU];
+    real vprev[NU];
 #pragma unroll
-    for (int n = 0; n < NU; ++n) { vprev[n] = (real)0; uprev[n] = (real)0; }
+    for (int n = 0; n < NU; ++n) vprev[n] = (real)0;
     for (int t = 0; t < T; ++t) {
         real v[NU], u[NU], eps[NU], c[M];
         action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
         noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
 #pragma unroll
         for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);                // mppi.py:355
-#if MPPI_ROLLOUT_PIPELINED
-        // step t-1's costs in iteration t, as the single loop of one copy: its variance takes disc[t-1]
-        MPPI_UNROLL_N(UNR)
-        for (int m = 0; m < mc; ++m) {
-            real xs[NX];
-#pragma unroll
-            for (int i = 0; i < NX; ++i) xs[i] = x[m][i];
-            model_step<Model, real>(mp, x[m], u, t, m);                                 // mppi.py:357
-            if (t > 0) c[m] = model_cost<Model, real>(mp, xs, uprev, t - 1, m);         // mppi.py:362 (step t-1)
-        }
-        if (t > 0) copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t - 1), mc);     // mppi.py:363-364
-#else
         MPPI_UNROLL_N(UNR)
         for (int m = 0; m < mc; ++m) {
             model_step<Model, real>(mp, x[m], u, t, m);                                 // mppi.py:357
             c[m] = model_cost<Model, real>(mp, x[m], u, t, m);                          // mppi.py:362
         }
         copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + t), mc);                     // mppi.py:363-364
-#endif
-        pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
-        if (VARIANT == V_SMPPI) {
-            if (t > 0) {
-#pragma unroll
-                for (int n = 0; n < NU; ++n) {
-                    const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));          // mppi.py:559
-                    smooth = O::add(smooth, O::mul(d, d));
-                }
-            }
-#pragma unroll
-            for (int n = 0; n < NU; ++n) vprev[n] = v[n];
-        }
-#pragma unroll
-        for (int n = 0; n < NU; ++n) uprev[n] = u[n];
+        action_terms<real, VARIANT, NU>(nm, sm.Us + t * NU, t, v, eps, pert, smooth, vprev);
     }
-#if MPPI_ROLLOUT_PIPELINED
-    {
-        real c[M];
-        MPPI_UNROLL_N(UNR)
-        for (int m = 0; m < mc; ++m) c[m] = model_cost<Model, real>(mp, x[m], uprev, T - 1, m);  // step T-1
-        copies_fold<real, M>(cs, var, c, __ldg(a.var_disc + T - 1), mc);
-    }
-#endif
     if (Model::template has_terminal<real>(mp)) {
         MPPI_UNROLL_N(UNR)
         for (int m = 0; m < mc; ++m) cs[m] = O::add(cs[m], model_terminal<Model, real>(mp, x[m], m));  // mppi.py:369-370
@@ -1606,10 +1496,7 @@ __device__ __forceinline__ real copies_rollout(const KArgs<real>& a, const typen
     for (int m = 1; m < M; ++m)
         if (m < mc) mean = O::add(mean, cs[m]);
     mean = O::div(mean, (real)mc);                                                        // mppi.py:371
-    real c_tot = O::add(O::add(mean, O::mul(var, a.var_cost)), pert);                     // mppi.py:372, 416
-    if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));           // mppi.py:562,569
-    a.cost_total[k] = c_tot;
-    return c_tot;
+    return sample_total<real, VARIANT>(a, k, O::add(mean, O::mul(var, a.var_cost)), pert, smooth);   // mppi.py:372
 }
 
 // =================================================================================================
@@ -1655,7 +1542,6 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
                                            layout_extra(VARIANT != V_MPPI, SPLIT ? NX : 0, cs_, xst), GTILE);
     Smem<real> sm(smem, L);
     if (GTILE) gtile_bind<real>(a, sm, VARIANT != V_MPPI);
-    const NoiseModel<real>& nm = a.nm;
     const int T = a.T;
     warp_records_init<real>(a, sm);      // published by the barrier in stage_issue
     // phase 0 of the cluster barrier: "this CTA has started" — the tail waits for it before the first store into the
@@ -1710,66 +1596,9 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
         } else if constexpr (ModelCopies<Model>::value > 1) {
             // C''. M copies of the sample's rollout, interleaved in registers
             if (active) c_tot = copies_rollout<Model, real, VARIANT>(a, mp, sm, k, kg);
-        } else if constexpr (FastRange<Model, real>::value) {
-            if (active) c_tot = single_loop_rollout_fast<Model, real, VARIANT, GTILE>(a, mp, sm, k, kg);
         } else if (active) {
-
-            // C. rollout (mppi.py:297-332) + action cost (mppi.py:409,415) [+ smoothness :559-562]
-            real x[NX];
-            if (a.state_dev != nullptr) {
-                const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
-#pragma unroll
-                for (int i = 0; i < NX; ++i) x[i] = sp[i];
-            } else {
-#pragma unroll
-                for (int i = 0; i < NX; ++i) x[i] = a.x0[i];
-            }
-            // Software-pipelined T-loop: the running cost of the state reached at step t-1 and the
-            // dynamics of step t both depend only on x_t, so issuing them back to back gives the
-            // single resident warp two independent dependency chains.  The arithmetic and the
-            // order of every accumulation are exactly the reference's (cost summed t = 0..T-1).
-            real roll = (real)0, pert = (real)0, smooth = (real)0;
-            real vprev[NU], uprev[NU];
-#pragma unroll
-            for (int n = 0; n < NU; ++n) { vprev[n] = (real)0; uprev[n] = (real)0; }
-MPPI_UNROLL_N(MPPI_ROLLOUT_UNROLL)
-            for (int t = 0; t < T; ++t) {
-                real v[NU], u[NU], eps[NU], xs[NX];
-                action_at<real, VARIANT, NU, true>(a, sm, kg, t, v);
-                noise_at<real, VARIANT, NU, true>(a, sm, t, v, eps);
-#pragma unroll
-                for (int n = 0; n < NU; ++n) u[n] = O::mul(nm.u_scale, v[n]);            // mppi.py:313
-#pragma unroll
-                for (int i = 0; i < NX; ++i) xs[i] = x[i];
-#if MPPI_ROLLOUT_PIPELINED
-                model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
-                if (t > 0) roll = O::add(roll, model_cost<Model, real>(mp, xs, uprev, t - 1));   // mppi.py:318-319 (step t-1)
-#else
-                model_step<Model, real>(mp, x, u, t);                                     // mppi.py:314
-                roll = O::add(roll, model_cost<Model, real>(mp, x, u, t));                // mppi.py:318-319
-#endif
-                pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
-                if (VARIANT == V_SMPPI) {
-                    if (t > 0) {
-#pragma unroll
-                        for (int n = 0; n < NU; ++n) {
-                            const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));    // mppi.py:559
-                            smooth = O::add(smooth, O::mul(d, d));
-                        }
-                    }
-#pragma unroll
-                    for (int n = 0; n < NU; ++n) vprev[n] = v[n];
-                }
-#pragma unroll
-                for (int n = 0; n < NU; ++n) uprev[n] = u[n];
-            }
-#if MPPI_ROLLOUT_PIPELINED
-            roll = O::add(roll, model_cost<Model, real>(mp, x, uprev, T - 1));            // step T-1
-#endif
-            if (Model::template has_terminal<real>(mp)) roll = O::add(roll, Model::template terminal<real>(mp, x));
-            c_tot = O::add(roll, pert);                                                   // mppi.py:416
-            if (VARIANT == V_SMPPI) c_tot = O::add(c_tot, O::mul(smooth, nm.w_smooth));   // mppi.py:562,569
-            a.cost_total[k] = c_tot;
+            // C. the single loop
+            c_tot = single_loop_rollout<Model, real, VARIANT, GTILE>(a, mp, sm, k, kg, T);
         }
         if (tile == blockIdx.x) stamp(a.dbg, 4);
         // D. every rollout warp folds its 32 samples into its own running record (no CTA barrier)
@@ -1911,21 +1740,10 @@ __device__ __forceinline__ void sample_body(const KArgs<real>& a_in) {
                 real v[NU], eps[NU];
                 action_at<real, VARIANT, NU>(a, sm, kg, t, v);
                 noise_at<real, VARIANT, NU>(a, sm, t, v, eps);
-                pert = O::add(pert, action_cost_term<real, NU>(nm, eps, sm.Us + t * NU));
+                action_terms<real, VARIANT, NU>(nm, sm.Us + t * NU, t, v, eps, pert, smooth, vprev);
                 if (VARIANT == V_KMPPI) {
 #pragma unroll
                     for (int n = 0; n < NU; ++n) sm.rows2[(t * NU + n) * LD + tid] = v[n];
-                }
-                if (VARIANT == V_SMPPI) {
-                    if (t > 0) {
-#pragma unroll
-                        for (int n = 0; n < NU; ++n) {
-                            const real d = O::mul(nm.u_scale, O::sub(v[n], vprev[n]));
-                            smooth = O::add(smooth, O::mul(d, d));
-                        }
-                    }
-#pragma unroll
-                    for (int n = 0; n < NU; ++n) vprev[n] = v[n];
                 }
             }
             if (a.out_cost_init != nullptr) {
@@ -1983,6 +1801,17 @@ __device__ __forceinline__ void replay_step(const typename Model::template P<rea
     model_step<Model, real, FAST>(mp, x, u, t, m);
 }
 
+// the states of sample k's replay from x, on the model's fast step (FAST) or not
+template <class Model, typename real, bool FAST>
+__device__ __forceinline__ void replay_states(const KArgs<real>& a, const typename Model::template P<real>& mp, real* x, const real* pa,
+                                              real* states, int k, int m) {
+    for (int t = 0; t < a.T; ++t) {
+        real u[Model::NU];
+        replay_step<Model, real, FAST>(mp, x, u, pa, a.nm.u_scale, t, m);
+        for (int i = 0; i < Model::NX; ++i) states[((size_t)k * a.T + t) * Model::NX + i] = x[i];
+    }
+}
+
 // states along the rollout of given perturbed actions (mppi.py:307-322), for registered models.
 // pa_stride = elements between consecutive samples' action sequences: T*nu for a (K,T,nu) tensor, 0 when every
 // sample replays the SAME (T,nu) sequence (get_rollouts, mppi.py:425-448).
@@ -1990,7 +1819,7 @@ __device__ __forceinline__ void replay_step(const typename Model::template P<rea
 template <class Model, typename real>
 __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ states, const KArgs<real> a,
                               const typename Model::template P<real> mp, long long pa_stride) {
-    constexpr int NX = Model::NX, NU = Model::NU;
+    constexpr int NX = Model::NX;
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= a.K) return;
     int m = 0;
@@ -2000,27 +1829,14 @@ __global__ void states_kernel(const real* __restrict__ pa, real* __restrict__ st
     }
     pa += (size_t)k * (size_t)pa_stride;
     real x[NX];
-    if (a.state_dev != nullptr) {
-        const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
-        for (int i = 0; i < NX; ++i) x[i] = sp[i];
-    } else {
-        for (int i = 0; i < NX; ++i) x[i] = a.x0[i];
-    }
+    initial_state<real, NX>(a, k, x);
     if constexpr (FastRange<Model, real>::value) {      // the fast step where the command's rollouts take it
         if (Model::template in_fast_range<real>(mp, x, a.T)) {
-            for (int t = 0; t < a.T; ++t) {
-                real u[NU];
-                replay_step<Model, real, true>(mp, x, u, pa, a.nm.u_scale, t, 0);
-                for (int i = 0; i < NX; ++i) states[((size_t)k * a.T + t) * NX + i] = x[i];
-            }
+            replay_states<Model, real, true>(a, mp, x, pa, states, k, 0);
             return;
         }
     }
-    for (int t = 0; t < a.T; ++t) {
-        real u[NU];
-        replay_step<Model, real, false>(mp, x, u, pa, a.nm.u_scale, t, m);
-        for (int i = 0; i < NX; ++i) states[((size_t)k * a.T + t) * NX + i] = x[i];
-    }
+    replay_states<Model, real, false>(a, mp, x, pa, states, k, m);
 }
 
 // One plant step of a closed-loop episode (mppi_plan_closed_loop), one thread per environment: after the command of

@@ -201,16 +201,7 @@ __global__ void __launch_bounds__(256, 2) mlp_tc_command_kernel(const __grid_con
 
         // ---- rollout: the MMAs are warpgroup-wide, so every thread keeps the step's two barriers ---------------------
         real x[NX] = {(real)0, (real)0};
-        if (active) {
-            if (a.state_dev != nullptr) {
-                const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
-                x[0] = sp[0];
-                x[1] = sp[1];
-            } else {
-                x[0] = a.x0[0];
-                x[1] = a.x0[1];
-            }
-        }
+        if (active) initial_state<real, NX>(a, k, x);
         real roll = (real)0, pert = (real)0, smooth = (real)0, vprev = (real)0, u_prev = (real)0;
         for (int t = 0; t < T; ++t) {
             real v[NU] = {(real)0}, eps[NU] = {(real)0};
@@ -426,20 +417,11 @@ __global__ void __launch_bounds__(256, 2) mlp_ens_tc_command_kernel(const __grid
         // copy-m state, read and updated there after the step's second barrier.
         auto xrow = [&](int m) -> float2& { return reinterpret_cast<float2*>(ens + m * Model::TC_COPY + Model::TC_X)[row]; };
         if (roller) {
-            real x0 = (real)0, x1 = (real)0;
-            if (active) {
-                if (a.state_dev != nullptr) {
-                    const real* sp = a.state_dev + (a.state_per_sample ? (size_t)k * NX : 0);
-                    x0 = sp[0];
-                    x1 = sp[1];
-                } else {
-                    x0 = a.x0[0];
-                    x1 = a.x0[1];
-                }
-            }
+            real x[NX] = {(real)0, (real)0};
+            if (active) initial_state<real, NX>(a, k, x);
 #pragma unroll
             for (int m = 0; m < MC; ++m)
-                if (m < M) xrow(m) = make_float2(x0, x1);
+                if (m < M) xrow(m) = make_float2(x[0], x[1]);
         }
         real cs[MC];
 #pragma unroll

@@ -90,14 +90,14 @@ def test_fp32_parity_with_oracle_north_star_shape():
 
 
 def test_single_loop_rollout_matches_oracle():
-    """K=131072: one thread per sample, the pipelined T-loop that evaluates step t-1's cost in iteration t (and step
-    T-1's after the loop).  An off-by-one in t there would miss by > 2e-4 (tests/test_step_dependent.py)."""
+    """K=131072: one thread per sample, the single T-loop that evaluates step t's cost in iteration t, after step t's
+    dynamics.  An off-by-one in t there would miss by > 2e-4 (tests/test_step_dependent.py)."""
     c = _closed_loop_vs_oracle("mppi", 131072, 15, torch.float64, 1e-9, steps=2)
     assert c.launch_info.split_cost == 0
 
 
 def test_split_cost_rollout_equals_single_loop_bit_for_bit(monkeypatch):
-    """The split-cost rollout (helper thread per t) and the single-loop kernel (step t-1's cost in iteration t) give the
+    """The split-cost rollout (helper thread per t) and the single-loop kernel (step t's cost in iteration t) give the
     same per-sample costs bit for bit, as for the registered models (tests/test_gpu_parity.py); the softmin reduction
     order follows each kernel's cluster size, so U and the action agree to fp32 rounding of that order."""
     m = um.step_dependent_user_model()
