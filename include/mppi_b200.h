@@ -366,6 +366,21 @@ uint64_t mppi_plan_env_scratch_bytes(void* plan);
  * PENDULUM_MLP models (no per-environment kernel).  All checked before any CUDA call. */
 int mppi_plan_set_env_params(void* plan, const MppiEnvParams* ep, void* stream);
 
+/* Per-environment horizons of a batched plan: environment e rolls out h_e <= T steps (T: the plan's horizon), so it is the
+ * single-environment MPPI command with horizon h_e on the first h_e * nu rows of the shared standard normals — rollout,
+ * running and action costs over t < h_e, its update added to its first h_e rows, and the shift moving rows 1..h_e-1 up
+ * with u_init into row h_e-1.  Rows h_e.. of its nominal sequence are left at the post-shift nominal, u_init when they
+ * held it.  `horizon_host`: (n_env) HOST int32 values with u_per_command <= h_e <= T, read during the call; NULL: back to T
+ * for every environment.  The values go to `scratch` (caller-owned DEVICE memory, mppi_plan_env_horizon_bytes(plan)
+ * bytes, 16-byte aligned, kept for as long as the plan runs with these horizons; may be NULL with horizon_host NULL) with
+ * one stream-ordered copy: commands enqueued before the call keep the horizons they were launched with.  No new plan:
+ * kernel, geometry, tiles and strides stay the plan's. */
+uint64_t mppi_plan_env_horizon_bytes(void* plan);   /* 0 for a null plan */
+/* MPPI_ERR_BAD_ARG: null plan, a horizon < 1, < u_per_command or > T, scratch NULL / misaligned.  MPPI_ERR_UNSUPPORTED:
+ * single-environment plans, sharded plans, the PENDULUM_MLP models (their batched kernels fix their own tiles).  All
+ * checked before any CUDA call. */
+int mppi_plan_set_env_horizon(void* plan, const int32_t* horizon_host, void* scratch, void* stream);
+
 /* ---- Resident mode: command() without a kernel launch ---------------------------------------------
  * For a host control loop (mppi.py:240-252 called once per control step).  One cooperative launch leaves the
  * command's grid on the SMs; each following command is a record (flags, Philox counter, start state) written into

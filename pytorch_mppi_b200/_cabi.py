@@ -207,6 +207,8 @@ SYMBOLS = [
     ("mppi_plan_closed_loop", C.c_int, [C.c_void_p, C.POINTER(MppiClosedLoop), C.c_void_p]),
     ("mppi_plan_env_scratch_bytes", C.c_uint64, [C.c_void_p]),
     ("mppi_plan_set_env_params", C.c_int, [C.c_void_p, C.POINTER(MppiEnvParams), C.c_void_p]),
+    ("mppi_plan_env_horizon_bytes", C.c_uint64, [C.c_void_p]),
+    ("mppi_plan_set_env_horizon", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     ("mppi_resident_start", C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
     ("mppi_resident_command", C.c_int, [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_void_p]),
     ("mppi_resident_sync", C.c_int, [C.c_void_p]),

@@ -322,6 +322,39 @@ int set_env_params_t(Plan* pl, const MppiEnvParams* ep, cudaStream_t stream) {
     return MPPI_OK;
 }
 
+// ---- per-environment horizons (mppi_plan_set_env_horizon) ------------------------------------------------
+inline uint64_t env_horizon_bytes(const Plan* pl) { return ((uint64_t)pl->p.n_env * sizeof(int32_t) + 15) / 16 * 16; }
+
+// the reasons the horizons are refused, before any CUDA call (MPPI_OK: none)
+int check_env_horizon(const Plan* pl, const int32_t* h, const void* scratch) {
+    if (pl == nullptr) return MPPI_ERR_BAD_ARG;
+    if (pl->p.n_env <= 1) return UNSUPPORTED("per-environment horizons: the plan has one environment (MPPI_Batched only)");
+    if (pl->p.world > 1 || (pl->p.flags & MPPI_FLAG_EXPORT_PARTIAL))
+        return UNSUPPORTED("per-environment horizons: not available on sharded controllers");
+    if (pl->mk->is_mlp) return UNSUPPORTED("per-environment horizons: not available for the PendulumMLP models (their batched kernels fix their own tiles)");
+    if (h == nullptr) return MPPI_OK;
+    const int lo = pl->p.u_per_command > 1 ? pl->p.u_per_command : 1;
+    for (int e = 0; e < pl->p.n_env; ++e)
+        if (h[e] < lo || h[e] > pl->p.T) return MPPI_ERR_BAD_ARG;
+    if (scratch == nullptr || (uintptr_t)scratch % 16 != 0) return MPPI_ERR_BAD_ARG;
+    return MPPI_OK;
+}
+
+template <typename real>
+int set_env_horizon_t(Plan* pl, const int32_t* h, void* scratch, cudaStream_t stream) {
+    KArgs<real>* a = reinterpret_cast<KArgs<real>*>(pl->kargs);
+    if (h == nullptr) {      // back to the plan's T
+        a->env_horizon = nullptr;
+        return MPPI_OK;
+    }
+    // pageable source: the copy has taken the data when the call returns; commands enqueued before it have read the old
+    // horizons by the time it lands (stream order)
+    const cudaError_t ce = cudaMemcpyAsync(scratch, h, (size_t)pl->p.n_env * sizeof(int32_t), cudaMemcpyHostToDevice, stream);
+    if (ce != cudaSuccess) return cuda_fail(ce, "per-environment horizons: copy");
+    a->env_horizon = (const int*)scratch;
+    return MPPI_OK;
+}
+
 // ---- resident mode: the device backend of csrc/mppi_resident_host.h ---------------------------------
 template <typename real>
 int resident_launch_t(Plan* pl, uint64_t seed, uint64_t offset_pred, int shift_pred, uint64_t seq_start, uint32_t gen) {
@@ -725,6 +758,19 @@ int mppi_plan_set_env_params(void* plan, const MppiEnvParams* ep, void* stream) 
     const int rc = check_env_params(pl, ep);
     if (rc) return rc;
     return pl->is_double ? set_env_params_t<double>(pl, ep, (cudaStream_t)stream) : set_env_params_t<float>(pl, ep, (cudaStream_t)stream);
+}
+
+uint64_t mppi_plan_env_horizon_bytes(void* plan) {
+    const Plan* pl = reinterpret_cast<const Plan*>(plan);
+    return pl == nullptr ? 0 : env_horizon_bytes(pl);
+}
+
+int mppi_plan_set_env_horizon(void* plan, const int32_t* horizon_host, void* scratch, void* stream) {
+    Plan* pl = reinterpret_cast<Plan*>(plan);
+    const int rc = check_env_horizon(pl, horizon_host, scratch);
+    if (rc) return rc;
+    return pl->is_double ? set_env_horizon_t<double>(pl, horizon_host, scratch, (cudaStream_t)stream)
+                         : set_env_horizon_t<float>(pl, horizon_host, scratch, (cudaStream_t)stream);
 }
 
 int mppi_plan_command_host(void* plan, const double* state, uint32_t flags, uint64_t seed, uint64_t offset, const void* z,

@@ -88,7 +88,12 @@ template <typename real> struct KArgs {
     unsigned long long* host_mailbox;   // optional pinned host memory: [0]=epoch flag, [2..]=action values
     unsigned long long host_epoch;
     // generic-path extras (sample_kernel / softmin_update_kernel)
-    real* out_pa;
+    // The batched fused kernels read no generic-path extras: their per-environment horizons (n_env of them, or nullptr:
+    // every environment rolls out T) share the space of sample_kernel's perturbed-action output, so KArgs keeps its size.
+    union {
+        real* out_pa;                     // sample_kernel
+        const int* env_horizon;           // batched fused kernels (mppi_plan_set_env_horizon)
+    };
     real* out_noise;
     // The batched fused kernels read no generic-path extras: their per-environment noise models (n_env of them, or
     // nullptr: every environment takes `nm`) share the space of sample_kernel's KMPPI output, so KArgs keeps its size.
@@ -584,12 +589,15 @@ __device__ __forceinline__ void host_store<double>(unsigned long long* box, int 
 }
 
 // ---- final update from (beta, eta, numerators) with the post-shift nominal in shared memory -----
-template <typename real, int VARIANT>
+// ENV (the batched fused kernels, MPPI): a.T is the environment's horizon h_e, and only its first h_e * nu rows take the
+// update; the rows past it keep the post-shift nominal, u_init (the fold ran over all R rows, their numerators unused).
+template <typename real, int VARIANT, bool ENV = false>
 __device__ void finish_update(const KArgs<real>& a, const double* numd, const real* Us, const real* As, real* ths,
                               const real* Ws, int nu) {
     typedef Ops<real> O;
     const int tid = threadIdx.x, BD = blockDim.x;
     const int TN = a.TN, R = a.R;
+    const int HN = ENV ? a.T * nu : TN;
     const double eta = numd[1];
     const double inv_eta = 1.0 / eta;
     // nominal_used: U | A | theta slots, as sampled from (post-shift, pre-update)
@@ -609,7 +617,7 @@ __device__ void finish_update(const KArgs<real>& a, const double* numd, const re
     unsigned long long* hact = a.host_mailbox;
     if (VARIANT == V_MPPI) {
         for (int j = tid; j < TN; j += BD) {
-            const real un = O::add(Us[j], (real)(numd[2 + j] * inv_eta));                // mppi.py:270
+            const real un = ENV && j >= HN ? Us[j] : O::add(Us[j], (real)(numd[2 + j] * inv_eta));   // mppi.py:270
             a.U[j] = un;
             if (j < a.upc * nu) {                                                          // mppi.py:271-275
                 a.action_out[j] = un;
@@ -1039,7 +1047,8 @@ __device__ __noinline__ void xchg_timed_out_rare(const KArgs<real>& a, Smem<real
 // finish_update — and its combines, publish and collect are inlined into it: the finisher runs on a cold instruction
 // cache (the L2 flushed between commands), where every jump into out-of-line code that no SM has fetched yet waits on
 // memory while the rest of the GPU idles.  Only the timeout report stays out of line.
-template <typename real, int VARIANT, int NU, bool PERSISTENT = false, bool LL1 = false>
+// ENV: the batched fused kernels (finish_update<..., ENV>).
+template <typename real, int VARIANT, int NU, bool PERSISTENT = false, bool LL1 = false, bool ENV = false>
 __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
     const int tid = threadIdx.x, BD = blockDim.x, lane = tid & 31, warp = tid >> 5;
     const int R = a.R, RW = R + 2;
@@ -1137,7 +1146,7 @@ __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
         combine<real>(sm, sm.xstage, xw, R, nfl);
     }
     stamp(a.dbg, 11);
-    finish_update<real, VARIANT>(a, sm.numd, sm.Us, sm.As, sm.ths, sm.Ws, NU);
+    finish_update<real, VARIANT, ENV>(a, sm.numd, sm.Us, sm.As, sm.ths, sm.Ws, NU);
     if (tid == 0) a.stats[3] = 0.0;
     return true;
 }
@@ -1145,15 +1154,17 @@ __device__ bool warp_tail(const KArgs<real>& a, Smem<real>& sm) {
 // ---- per-environment view of the kernel arguments (batched launches) -------------------------------
 // The argument block lives in constant (parameter) space; a batched CTA needs its environment's
 // pointers, so it builds an adjusted copy in shared memory once and every stage reads that copy.
-// ENV_NM (the batched fused kernels): the environment's own noise model replaces `nm` where env_nm is set.
-template <typename real, int NXv, int NUv, bool ENV_NM = false>
+// ENV (the batched fused kernels): the environment's own noise model replaces `nm` where env_nm is set, and its own
+// horizon h_e replaces `T` where env_horizon is set.  Only `T` changes: TN, R and every stride and layout derived from them
+// stay the plan's, so the environment's rows are the first h_e * nu of the plan's.
+template <typename real, int NXv, int NUv, bool ENV = false>
 __device__ void make_env_args(const KArgs<real>& in, KArgs<real>* out) {
     const int tid = threadIdx.x, BD = blockDim.x;
     const uint32_t* src = reinterpret_cast<const uint32_t*>(&in);
     uint32_t* dst = reinterpret_cast<uint32_t*>(out);
     for (int i = tid; i < (int)(sizeof(KArgs<real>) / 4); i += BD) dst[i] = src[i];
     __syncthreads();
-    if (ENV_NM && in.env_nm != nullptr) {
+    if (ENV && in.env_nm != nullptr) {
         static_assert(sizeof(NoiseModel<real>) % 4 == 0, "word copy of the noise model");
         const uint32_t* nsrc = reinterpret_cast<const uint32_t*>(in.env_nm + blockIdx.y);
         uint32_t* ndst = reinterpret_cast<uint32_t*>(&out->nm);
@@ -1175,7 +1186,11 @@ __device__ void make_env_args(const KArgs<real>& in, KArgs<real>* out) {
             if (in.world == 1 || in.export_partial)      // this GPU's own record mailbox lives in the environment's workspace
                 out->peers[0] = reinterpret_cast<unsigned long long*>(reinterpret_cast<unsigned char*>(in.peers[0]) + off);
         }
-        if (in.out_pa) out->out_pa = in.out_pa + e * K * TN;
+        if (ENV) {
+            if (in.env_horizon != nullptr) out->T = in.env_horizon[e];
+        } else if (in.out_pa) {
+            out->out_pa = in.out_pa + e * K * TN;
+        }
         if (in.out_noise) out->out_noise = in.out_noise + e * K * TN;
         if (in.out_cost_init) out->out_cost_init = in.out_cost_init + e * K;
         if (in.in_cost) out->in_cost = in.in_cost + e * K;
@@ -1538,7 +1553,8 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
     const int BS = BD / a.tps;
     const int xst = fused_xstage_doubles(a.world > 1 && !a.export_partial, a.world, a.xchg_npub, a.R);
     const int cs_ = (int)cluster_nctarank(), NC_ = (int)gridDim.x / cs_;
-    const SmemLayout L = make_layout<real>(VARIANT, a.T, NU, a.S, a.R, BD, BS, fused_layout_nb(NC_, a.xchg_npub),
+    // the layout is the plan's (a_in.T): with per-environment horizons a.T is this environment's h_e
+    const SmemLayout L = make_layout<real>(VARIANT, a_in.T, NU, a.S, a.R, BD, BS, fused_layout_nb(NC_, a.xchg_npub),
                                            layout_extra(VARIANT != V_MPPI, SPLIT ? NX : 0, cs_, xst), GTILE);
     Smem<real> sm(smem, L);
     if (GTILE) gtile_bind<real>(a, sm, VARIANT != V_MPPI);
@@ -1607,7 +1623,7 @@ __device__ __forceinline__ void fused_command_body(const KArgs<real>& a_in, cons
         if (tile + (int)gridDim.x < a.n_tiles) __syncthreads();      // the tile is refilled by the next pass
     }
     if (!staged) stage_finish<real, VARIANT, NU>(a, sm);
-    warp_tail<real, VARIANT, NU, false, LL1>(a, sm);
+    warp_tail<real, VARIANT, NU, false, LL1, BATCHED>(a, sm);
     stamp(a.dbg, 7);
 }
 

@@ -1713,6 +1713,8 @@ class MPPI_Batched(MPPI):
         self._env_model_params = self._env_lambda = self._env_sigma = self._env_mu = None
         self._env_factors = None          # (diagonal, L, inverse, sqrt-diagonal) per environment of _env_sigma
         self._env_scratch = None          # device blocks the plan reads (mppi_plan_set_env_params)
+        self._env_horizon = None          # (N,) int32 per-environment horizons (set_env_horizon), or None: T for all
+        self._env_horizon_scratch = None  # device copy the plan reads (mppi_plan_set_env_horizon)
         super().__init__(dynamics, running_cost, nx, noise_sigma, num_samples=num_samples, horizon=horizon, device=device,
                          lambda_=lambda_, noise_mu=noise_mu, u_min=u_min, u_max=u_max, u_init=u_init, u_scale=u_scale,
                          u_per_command=u_per_command, step_dependent_dynamics=step_dependent_dynamics,
@@ -1748,8 +1750,9 @@ class MPPI_Batched(MPPI):
         p.env_u_stride = self._u_stride
 
     def reset(self):
-        """mppi.py:819-820"""
+        """mppi.py:819-820; with per-environment horizons, the rows past each environment's horizon hold u_init."""
         self.U = self._sample_noise((self.N, self.T))
+        self._fill_past_horizon()
 
     def _sample_noise(self, shape):
         """As MPPI's; with per-environment noise (set_env_params), environment e's rows are coloured with its own
@@ -1879,10 +1882,71 @@ class MPPI_Batched(MPPI):
         stream = torch._C._cuda_getCurrentRawStream(self.d.index)
         _cabi.check(lib.mppi_plan_set_env_params(self._plan, C.byref(ep), stream), "mppi_plan_set_env_params")
 
+    def set_env_horizon(self, horizon=None):
+        """Give each environment its own horizon h_e (the reference's one horizon per controller, `change_horizon`, per
+        environment of one launch).  `horizon`: (N,) integers with u_per_command <= h_e <= T, where T (the constructor's
+        horizon) is the maximum; None returns every environment to T.  Environment e is then the single-environment MPPI
+        command with horizon h_e on the first h_e rows of the shared standard normals: rollout, running and action costs
+        over t < h_e, its update added to U[e, :h_e], and the shift moving U[e, 1:h_e] up with u_init into row h_e - 1.
+
+        Rows t >= h_e of ``U[e]`` hold u_init: here, after reset() and after every command.  Growing a horizon therefore
+        extends the sequence with u_init and shrinking it truncates, as `MPPI.change_horizon` does (mppi.py:277-284).
+        The horizons take effect at the next command, without a new plan; commands already enqueued keep theirs.
+        Available on the fused route (registered models and CudaModels, not the PendulumMLP models)."""
+        N = self.N
+        if horizon is not None:
+            if self._model is None:
+                raise ValueError("set_env_horizon: per-environment horizons run on the fused route only (registered models "
+                                 "and CudaModels); arbitrary dynamics / cost callables take the stepped route")
+            if self._model.model_id in (_cabi.MODEL_PENDULUM_MLP, _cabi.MODEL_PENDULUM_MLP_ENSEMBLE):
+                raise ValueError("set_env_horizon: not available for the PendulumMLP models (their batched kernels fix "
+                                 "their own tiles)")
+            t = horizon if torch.is_tensor(horizon) else torch.as_tensor(horizon)
+            if t.is_floating_point() or t.is_complex() or t.dtype == torch.bool:
+                raise ValueError(f"set_env_horizon: horizon must hold integers, got {t.dtype}")
+            if tuple(t.shape) != (N,):
+                raise ValueError(f"set_env_horizon: horizon must have shape {(N,)}, got {tuple(t.shape)}")
+            h = t.detach().to("cpu", torch.int64)
+            lo = max(1, self.u_per_command)
+            if not bool(((h >= lo) & (h <= self.T)).all()):
+                raise ValueError(f"set_env_horizon: every horizon must be in [{lo}, T={self.T}] (u_per_command <= h <= T), "
+                                 f"got {h.tolist()}")
+            horizon = h.to(torch.int32).contiguous()
+        self._env_horizon = horizon
+        self._fill_past_horizon()
+        if self._plan is not None:
+            self._apply_env_horizon()
+
+    env_horizon = property(lambda self: self._env_horizon,
+                           doc="(N,) int32 per-environment horizons, or None (every environment rolls out T)")
+
+    def _fill_past_horizon(self):
+        """U[e, h_e:] = u_init for every environment (nothing without per-environment horizons)."""
+        if self._env_horizon is None:
+            return
+        past = torch.arange(self.T).view(1, self.T) >= self._env_horizon.view(self.N, 1).to(torch.int64)
+        self.U[past.to(self.d)] = self._u_init.to(self.d, self.dtype)
+
+    def _apply_env_horizon(self):
+        """Hand the per-environment horizons to the plan (mppi_plan_set_env_horizon): no new plan."""
+        lib = self._lib
+        h = self._env_horizon
+        scratch = None
+        if h is not None:
+            need = int(lib.mppi_plan_env_horizon_bytes(self._plan))
+            if self._env_horizon_scratch is None or self._env_horizon_scratch.numel() < need:
+                self._env_horizon_scratch = torch.empty(need, device=self.d, dtype=torch.uint8)
+            scratch = self._env_horizon_scratch.data_ptr()
+        stream = torch._C._cuda_getCurrentRawStream(self.d.index)
+        _cabi.check(lib.mppi_plan_set_env_horizon(self._plan, None if h is None else h.data_ptr(), scratch, stream),
+                    "mppi_plan_set_env_horizon")
+
     def _make_plan(self, p):
         super()._make_plan(p)
         if any(v is not None for v in (self._env_model_params, self._env_lambda, self._env_sigma, self._env_mu)):
             self._apply_env_params()
+        if self._env_horizon is not None:
+            self._apply_env_horizon()
 
     def _take_model_params(self):
         super()._take_model_params()
