@@ -174,7 +174,7 @@ typedef struct MppiFusedParams {
      * (n_env, nx) on the device.  n_env <= 1 means a single problem.  MPPI variant only. */
     int32_t n_env;
     int32_t env_u_stride;        /* ELEMENTS between consecutive environments' U (>= T*nu, 16-byte multiple for TMA) */
-    uint64_t env_ws_stride;      /* BYTES between consecutive environments' workspace slices                       */
+    uint64_t env_ws_stride;      /* BYTES between consecutive environments' workspace slices (a multiple of 256)   */
     void* host_mailbox;          /* optional PINNED HOST memory (device-visible under UVA), u_per_command*nu 8-byte
                                     words (x2 for f64): the kernel stores every action value as a self-validating
                                     word, payload32 | (host_epoch & 0xffffffff) << 32, so the host spins on the

@@ -437,7 +437,9 @@ inline bool gtile_of(const MppiFusedParams* p) { return (p->flags & MPPI_FLAG_GL
 inline int check_gtile_workspace(const MppiFusedParams* p, const Geometry& g, int rows2) {
     const uint64_t need = ws_bytes(g.nb, rows_of(p)) + ws_gtile_plan_bytes(p, g.nb, g.BS, rows2);
     if (p->workspace == nullptr || p->workspace_bytes < need) return MPPI_ERR_WORKSPACE;
-    if (p->n_env > 1 && (p->env_ws_stride < need || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env)) return MPPI_ERR_WORKSPACE;
+    if (p->n_env > 1 && (p->env_ws_stride < need || p->env_ws_stride % MPPI_WS_ALIGN != 0 ||
+                         p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env))
+        return MPPI_ERR_WORKSPACE;
     return MPPI_OK;
 }
 
@@ -521,7 +523,9 @@ int plan_softmin(const MppiFusedParams* p, Geometry& g, bool check_ws = true) {
     if (rc || !check_ws) return rc;
     const uint64_t need_ws = ws_bytes(g.nb, rows_of(p));
     if (p->workspace == nullptr || p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
-    if (p->n_env > 1 && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env)) return MPPI_ERR_WORKSPACE;
+    if (p->n_env > 1 && (p->env_ws_stride < need_ws || p->env_ws_stride % MPPI_WS_ALIGN != 0 ||
+                         p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env))
+        return MPPI_ERR_WORKSPACE;
     return MPPI_OK;
 }
 

@@ -229,8 +229,8 @@ template <typename real> int build_plan(const ModelKernels* mk, const MppiFusedP
         return MPPI_ERR_BAD_ARG;
     const uint64_t need_ws = ws_bytes(pl->g.nb, rows_of(p)) + (c.gtile ? ws_gtile_plan_bytes(p, pl->g.nb, pl->g.BS, V != V_MPPI) : 0);
     if (p->workspace_bytes < need_ws) return MPPI_ERR_WORKSPACE;
-    if (batched && (p->env_ws_stride < need_ws || p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env ||
-                    p->env_u_stride < p->T * p->nu))
+    if (batched && (p->env_ws_stride < need_ws || p->env_ws_stride % MPPI_WS_ALIGN != 0 ||
+                    p->workspace_bytes < p->env_ws_stride * (uint64_t)p->n_env || p->env_u_stride < p->T * p->nu))
         return MPPI_ERR_WORKSPACE;
     if (mk->param_bytes > (int)sizeof(pl->mparams)) return UNSUPPORTED("model parameter block too large");
     KArgs<real>* a = reinterpret_cast<KArgs<real>*>(pl->kargs);

@@ -202,6 +202,9 @@ template <typename real> void fill_noise_model(const MppiFusedParams* p, NoiseMo
 // ... followed by this GPU's own record mailbox (single-GPU LL mode): two epoch parities of MPPI_LL_LOCAL_WORDS flagged words
 // (MPPI_LL_STAGE_BYTES / MPPI_LL_LOCAL_WORDS: mppi_fused.cuh)
 // ... followed, for the global-tile kernels, by one tile slice per CTA (gtile_slice_bytes; ws_gtile_bytes below)
+// Every environment's workspace of a batched plan (env_ws_stride apart) starts MPPI_WS_ALIGN-aligned, so its ticket, records
+// (doubles), mailbox words and tile slices are aligned as environment 0's are.
+#define MPPI_WS_ALIGN 256
 inline uint64_t ws_partials_bytes(int nb, int R) { return (16 + (uint64_t)nb * (uint64_t)(R + 2) * 8 + 255) / 256 * 256; }
 inline uint64_t ws_bytes(int nb, int R) { return ws_partials_bytes(nb, R) + 2ull * MPPI_LL_LOCAL_WORDS * 8; }
 
@@ -225,14 +228,16 @@ inline int gtile_grid_cap(int sm_count, int BS) {
 }
 // The tile slices of any global-tile plan of these dimensions (per environment): at most min(K + 511, cap) samples in
 // flight, one slice per CTA of at least 32 samples.  rows2 (T*nu per sample) only where a kernel of the variant has it:
-// SMPPI (fused) and KMPPI (fused and sampling); MPPI's slices hold `rows` alone.
+// SMPPI (fused) and KMPPI (fused and sampling); MPPI's slices hold `rows` alone.  A multiple of MPPI_WS_ALIGN, as ws_bytes
+// is: the workspace of a batched plan's environment e starts e x (ws_bytes + ws_gtile_bytes) bytes in (env_ws_stride).
 inline uint64_t ws_gtile_bytes(const MppiFusedParams* p, int sm_count) {
     const long long K = p->K_geom > p->K ? p->K_geom : p->K;
     long long n = (long long)sm_count * MPPI_GTILE_SAMPLES_PER_SM;
     if (K + 511 < n) n = K + 511;
     const int es = p->dtype == MPPI_F64 ? 8 : 4;
     const long long per_sample = rows_of(p) + (p->variant != MPPI_VARIANT_MPPI ? (long long)p->T * p->nu : 0);
-    return (uint64_t)n * (uint64_t)per_sample * es + (uint64_t)(n / 32 + 1) * 256;
+    const uint64_t bytes = (uint64_t)n * (uint64_t)per_sample * es + (uint64_t)(n / 32 + 1) * 256;
+    return (bytes + MPPI_WS_ALIGN - 1) / MPPI_WS_ALIGN * MPPI_WS_ALIGN;
 }
 // ... and the slices of a planned grid
 inline uint64_t ws_gtile_plan_bytes(const MppiFusedParams* p, int nb, int BS, int rows2) {

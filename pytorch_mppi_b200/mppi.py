@@ -1784,9 +1784,17 @@ class MPPI_Batched(MPPI):
         An argument left None stays shared (the controller's own value applies to every environment);
         ``set_env_params()`` returns to fully shared settings.  The values take effect at the next command, without a new
         plan; commands already enqueued keep the values they were launched with.  With model parameters and
-        plant_params=None, run_closed_loop's plant of environment e is the model with e's parameters."""
+        plant_params=None, run_closed_loop's plant of environment e is the model with e's parameters.  A LinearPoint block
+        with terminal_scale != 0 adds environment e's terminal cost on its state after h_e steps (set_env_horizon), as a
+        single controller with that model and horizon does.  If the library refuses the settings, the controller keeps
+        the ones it had."""
         N, nu = self.N, self.nu
         given = [v is not None for v in (model_params, lambda_, noise_sigma, noise_mu)]
+        if N == 1:      # one environment: its settings are the controller's own (the library refuses a per-environment set)
+            if any(given):
+                raise ValueError("set_env_params: a controller of one environment has no per-environment settings; give "
+                                 "them to the constructor")
+            return
         m = self._model
         if any(given) and m is None:
             raise ValueError("set_env_params: per-environment settings run on the fused route only (registered models and "
@@ -1831,10 +1839,15 @@ class MPPI_Batched(MPPI):
                 factors.append(f)
         if noise_mu is not None:
             mu = host(noise_mu, "noise_mu", (N, nu)).to(self.d, self.dtype)
+        old = (self._env_model_params, self._env_lambda, self._env_sigma, self._env_mu, self._env_factors)
         self._env_model_params, self._env_lambda, self._env_sigma, self._env_mu = mp, lam, sig, mu
         self._env_factors = factors
         if self._plan is not None:
-            self._apply_env_params()
+            try:
+                self._apply_env_params()
+            except Exception:      # refused: omega and _sample_noise keep reading the settings the plan still has
+                self._env_model_params, self._env_lambda, self._env_sigma, self._env_mu, self._env_factors = old
+                raise
 
     env_model_params = property(lambda self: self._env_model_params,
                                 doc="(N, n_params) float64 per-environment model parameters, or None (shared)")
@@ -1892,8 +1905,14 @@ class MPPI_Batched(MPPI):
         Rows t >= h_e of ``U[e]`` hold u_init: here, after reset() and after every command.  Growing a horizon therefore
         extends the sequence with u_init and shrinking it truncates, as `MPPI.change_horizon` does (mppi.py:277-284).
         The horizons take effect at the next command, without a new plan; commands already enqueued keep theirs.
-        Available on the fused route (registered models and CudaModels, not the PendulumMLP models)."""
+        Available on the fused route (registered models and CudaModels, not the PendulumMLP models), with at least two
+        environments.  If the library refuses the horizons, the controller (horizons and U) stays as it was."""
         N = self.N
+        if N == 1:      # one environment: its horizon is the controller's T (the library refuses a per-environment set)
+            if horizon is not None:
+                raise ValueError("set_env_horizon: a controller of one environment has no per-environment horizons; give "
+                                 "its horizon to the constructor")
+            return
         if horizon is not None:
             if self._model is None:
                 raise ValueError("set_env_horizon: per-environment horizons run on the fused route only (registered models "
@@ -1912,10 +1931,10 @@ class MPPI_Batched(MPPI):
                 raise ValueError(f"set_env_horizon: every horizon must be in [{lo}, T={self.T}] (u_per_command <= h <= T), "
                                  f"got {h.tolist()}")
             horizon = h.to(torch.int32).contiguous()
+        if self._plan is not None:
+            self._apply_env_horizon(horizon)      # first: a refusal raises before anything here changes
         self._env_horizon = horizon
         self._fill_past_horizon()
-        if self._plan is not None:
-            self._apply_env_horizon()
 
     env_horizon = property(lambda self: self._env_horizon,
                            doc="(N,) int32 per-environment horizons, or None (every environment rolls out T)")
@@ -1927,10 +1946,10 @@ class MPPI_Batched(MPPI):
         past = torch.arange(self.T).view(1, self.T) >= self._env_horizon.view(self.N, 1).to(torch.int64)
         self.U[past.to(self.d)] = self._u_init.to(self.d, self.dtype)
 
-    def _apply_env_horizon(self):
-        """Hand the per-environment horizons to the plan (mppi_plan_set_env_horizon): no new plan."""
+    def _apply_env_horizon(self, h):
+        """Hand the per-environment horizons h ((N,) int32, or None) to the plan (mppi_plan_set_env_horizon): no new
+        plan."""
         lib = self._lib
-        h = self._env_horizon
         scratch = None
         if h is not None:
             need = int(lib.mppi_plan_env_horizon_bytes(self._plan))
@@ -1946,7 +1965,7 @@ class MPPI_Batched(MPPI):
         if any(v is not None for v in (self._env_model_params, self._env_lambda, self._env_sigma, self._env_mu)):
             self._apply_env_params()
         if self._env_horizon is not None:
-            self._apply_env_horizon()
+            self._apply_env_horizon(self._env_horizon)
 
     def _take_model_params(self):
         super()._take_model_params()

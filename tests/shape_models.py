@@ -148,7 +148,7 @@ def shape_model(nx, nu, terminal=True):
 
 def prebuilt():
     """(model, dtype, variant) of every shape-model kernel the GPU tests load: all variants in both dtypes, and the
-    terminal-free (3,3) form the MPPI_Batched tests take."""
+    terminal-free (3,3) form the MPPI_Batched tests take, in both dtypes."""
     out = [(shape_model(nx, nu), dt, v) for nx, nu in SHAPES for dt in (torch.float32, torch.float64) for v in (0, 1, 2)]
-    out.append((shape_model(3, 3, terminal=False), torch.float64, 0))
+    out += [(shape_model(3, 3, terminal=False), dt, 0) for dt in (torch.float32, torch.float64)]
     return out

@@ -22,7 +22,7 @@ def test_abi_checks_come_before_any_cuda_call():
 
 class _Lib:
     def __init__(self):
-        self.calls, self.creates = [], 0
+        self.calls, self.creates, self.refuse = [], 0, False
 
     def mppi_plan_create(self, p, out):
         self.creates += 1
@@ -34,7 +34,7 @@ class _Lib:
     def mppi_plan_set_env_horizon(self, plan, h, scratch, stream):
         n = 3
         self.calls.append(dict(h=None if not h else list((C.c_int32 * n).from_address(h)), scratch=bool(scratch)))
-        return 0
+        return -2 if self.refuse else 0          # MPPI_ERR_UNSUPPORTED
 
 
 def _controller(monkeypatch, model=None, N=3, nu=2, T=6, upc=1, dtype=torch.float64):
@@ -101,6 +101,31 @@ def test_refusals_before_anything_is_handed_over(monkeypatch, h, why):
     with pytest.raises(ValueError, match=why):
         c.set_env_horizon(h)
     assert c._lib.calls == [] and c.env_horizon is None and torch.equal(c.U, U_before)
+
+
+def test_a_library_refusal_keeps_the_horizons_and_U(monkeypatch):
+    """The library refuses the new horizons (or the return to T): the controller keeps the horizons the plan has, and
+    U is not filled with u_init past horizons that never took effect."""
+    build.build()
+    c = _controller(monkeypatch)
+    c.set_env_horizon([6, 2, 4])
+    h_before, U_before = c.env_horizon, c.U.clone()
+    c._lib.refuse = True
+    for h in ([3, 3, 3], None):
+        with pytest.raises(_cabi.MppiLibraryError, match="mppi_plan_set_env_horizon"):
+            c.set_env_horizon(h)
+        assert c.env_horizon is h_before and c.env_horizon.tolist() == [6, 2, 4], h
+        assert torch.equal(c.U, U_before), h
+
+
+def test_one_environment_refuses_per_environment_horizons(monkeypatch):
+    """MPPI_Batched(num_envs=1): ValueError before anything changes; None is a no-op."""
+    c = _controller(monkeypatch, N=1)
+    U_before = c.U.clone()
+    with pytest.raises(ValueError, match="one environment"):
+        c.set_env_horizon([3])
+    c.set_env_horizon(None)
+    assert c.env_horizon is None and torch.equal(c.U, U_before) and c._lib.calls == []
 
 
 def test_refusal_below_u_per_command(monkeypatch):

@@ -30,7 +30,7 @@ class _Lib:
     SCRATCH = 512
 
     def __init__(self):
-        self.calls, self.creates = [], 0
+        self.calls, self.creates, self.refuse = [], 0, False
 
     def mppi_plan_create(self, p, out):
         self.creates += 1
@@ -47,7 +47,7 @@ class _Lib:
                                sinv=rd(ep.sigma_inv, n * MU * MU), mu=rd(ep.noise_mu, n * MU),
                                mp=rd(ep.model_params, n * ep.n_model_params), n_mp=ep.n_model_params,
                                scratch=bool(ep.scratch), size=ep.struct_size))
-        return 0
+        return -2 if self.refuse else 0          # MPPI_ERR_UNSUPPORTED
 
 
 def _controller(monkeypatch, model=None, N=3, nu=2, dtype=torch.float64):
@@ -126,6 +126,36 @@ def test_refusals_before_anything_launches(monkeypatch, kw, why):
     with pytest.raises(ValueError, match=why):
         c.set_env_params(**kw)
     assert c._lib.calls == [] and c.env_lambda is None and c.env_noise_sigma is None
+
+
+def test_a_library_refusal_keeps_the_settings_the_plan_has(monkeypatch):
+    """The library refuses the new settings: every per-environment attribute (omega's lambda, _sample_noise's factors
+    and mu, the model blocks) is still the one the plan was given before."""
+    build.build()
+    c = _controller(monkeypatch)
+    lin = eng.LinearPoint.unit_test_env()
+    sig = torch.tensor([[[0.5, 0.0], [0.0, 2.0]]] * 3, dtype=torch.float64)
+    c.set_env_params(model_params=[lin.param_blob()] * 3, lambda_=[0.5, 1.0, 2.0], noise_sigma=sig)
+    before = (c._env_model_params, c._env_lambda, c._env_sigma, c._env_mu, c._env_factors)
+    c._lib.refuse = True
+    for kw in (dict(lambda_=[3.0, 3.0, 3.0], noise_mu=[[0.1, 0.0]] * 3), dict()):
+        with pytest.raises(_cabi.MppiLibraryError, match="mppi_plan_set_env_params"):
+            c.set_env_params(**kw)
+        after = (c._env_model_params, c._env_lambda, c._env_sigma, c._env_mu, c._env_factors)
+        assert all(a is b for a, b in zip(after, before)), kw
+    assert c.env_lambda.tolist() == [0.5, 1.0, 2.0] and c.env_noise_mu is None
+
+
+def test_one_environment_refuses_per_environment_settings(monkeypatch):
+    """MPPI_Batched(num_envs=1): the library has no per-environment settings for one environment, so a setting raises
+    ValueError before any attribute changes; clearing is a no-op."""
+    c = _controller(monkeypatch, N=1)
+    for kw in (dict(lambda_=[2.0]), dict(noise_mu=[[0.1, 0.0]]), dict(model_params=[eng.LinearPoint.unit_test_env().param_blob()])):
+        with pytest.raises(ValueError, match="one environment"):
+            c.set_env_params(**kw)
+        assert c.env_lambda is None and c.env_noise_mu is None and c.env_model_params is None and c._env_factors is None
+    c.set_env_params()
+    assert c._lib.calls == [] and c.env_lambda is None
 
 
 def test_refusal_on_a_device_other_than_the_controllers(monkeypatch):
