@@ -119,7 +119,12 @@ class MPPI:
     Constructor and methods mirror the reference (mppi.py:45-61, 208-290, 425-448)."""
 
     _VARIANT = _cabi.VARIANT_MPPI
+    # immutable defaults every controller starts from, until an instance sets its own
     _model_version = 0                  # the model's `_param_version` the plan was last given
+    _env_axis = ()                      # leading axis of the per-environment buffers: (N,) on MPPI_Batched
+    _resident = False                   # a resident grid is armed for command_host (start_resident)
+    _offset_dev = None                  # compile(): the Philox counter on the device, advanced by every graph replay
+    _xchg_status = _xchg_status_word = None      # sharded p2p: the pinned word a timed-out peer exchange sets
 
     def __init__(self, dynamics, running_cost, nx, noise_sigma, num_samples=100, horizon=15, device="cuda",
                  terminal_state_cost=None,
@@ -268,8 +273,12 @@ class MPPI:
         self._host_epoch = 0            # launch-route command_host() calls so far: the mailbox tag, carried across re-plans
         self._plan = None
         self._last = None
-        self._resident = False          # a resident grid is armed for command_host (start_resident)
         self._resident_wanted = 0       # idle_us to re-enter resident mode with, after something made the grid leave
+        self._resident_idle_us = 0      # idle_us of the armed grid
+        self._res_box = self._res_board = self._res_stream = None     # start_resident's pinned box, device board, stream
+        self._graph_mode, self._graphs = False, {}
+        self._debug_clocks = None       # optional device buffer the fused kernel stamps its phase clocks into
+        self._pa_buf = self._noise_buf = self._cost_init = self._noise_theta_buf = None     # stepped route buffers
 
         # device state
         self._alloc_nominal(U_init)
@@ -312,7 +321,7 @@ class MPPI:
 
     def _mk(name):   # noqa: N805  (tiny property factory)
         def get(self):
-            return getattr(self, "_" + name)
+            return getattr(self, "_" + name)          # the attribute this property is made for
 
         def set_(self, v):
             setattr(self, "_" + name, v)
@@ -332,15 +341,11 @@ class MPPI:
     # ------------------------------------------------------------------------------------------
     # buffers
     # ------------------------------------------------------------------------------------------
-    def _rows(self):
-        return self.T * self.nu
-
     def _alloc_nominal(self, U_init):
-        es = _ES[self.dtype]
-        tn = self.T * self.nu
-        self._Ubuf = torch.zeros(_pad16(tn, es), device=self.d, dtype=self.dtype)
-        if U_init is None:
-            self.U = self._one_draw_for_all_ranks(self._sample_noise((self.T,)))            # mppi.py:144-145
+        row = _pad16(self.T * self.nu, _ES[self.dtype])         # MPPI_Batched: one row per environment (env_u_stride)
+        self._Ubuf = torch.zeros(self._env_axis + (row,), device=self.d, dtype=self.dtype)
+        if U_init is None:                                                      # mppi.py:144-145, 807
+            self.U = self._one_draw_for_all_ranks(self._sample_noise(self._env_axis + (self.T,)))
         else:
             self.U = U_init
 
@@ -355,10 +360,10 @@ class MPPI:
         return t
 
     def _alloc_results(self):
-        K, tn = self._K_local, self.T * self.nu
-        self._cost_buf = torch.empty(K, device=self.d, dtype=self.dtype)
-        self._nominal_used = torch.zeros(3 * tn + 4, device=self.d, dtype=self.dtype)
-        self._stats = torch.zeros(4, device=self.d, dtype=torch.float64)
+        lead, tn = self._env_axis, self.T * self.nu
+        self._cost_buf = torch.empty(lead + (self._K_local,), device=self.d, dtype=self.dtype)
+        self._nominal_used = torch.zeros(lead + (3 * tn + 4,), device=self.d, dtype=self.dtype)
+        self._stats = torch.zeros(lead + (4,), device=self.d, dtype=torch.float64)
         self._workspace = None
         self._partial = None
 
@@ -476,8 +481,7 @@ class MPPI:
         for g in range(_cabi.MPPI_MAX_RANKS):
             p.peer_slots[g] = None
         p.partial_out = None
-        dbg = getattr(self, "_debug_clocks", None)
-        p.debug_clocks = None if dbg is None else dbg.data_ptr()
+        p.debug_clocks = None if self._debug_clocks is None else self._debug_clocks.data_ptr()
         p.n_env, p.env_u_stride, p.env_ws_stride = 0, 0, 0
         p.torch_rng_total = 0
         if self._rng_mode == "torch":
@@ -488,15 +492,14 @@ class MPPI:
             unroll = 4 if self.dtype == torch.float32 else 2
             self._torch_counter_offset = ((numel - 1) // (256 * grid * unroll) + 1) * 4
             p.torch_rng_total = 256 * grid
-        od = getattr(self, "_offset_dev", None)
-        p.offset_dev = None if od is None else od.data_ptr()
+        p.offset_dev = None if self._offset_dev is None else self._offset_dev.data_ptr()
         per = 4 if self.dtype == torch.float32 else 2
         p.offset_inc = (self._noise_rows() + per - 1) // per
         p.host_mailbox = None
         p.host_epoch = 0
         p.xchg_status_host = None
         if self._world > 1 and self._exchange == "p2p":
-            if getattr(self, "_xchg_status", None) is None:
+            if self._xchg_status is None:
                 self._xchg_status = torch.zeros(1, dtype=torch.int64).pin_memory()     # written by the kernel on a peer timeout
                 # read on every command: through ctypes (0.07 us), not int(tensor[0]) (2.2 us)
                 self._xchg_status_word = C.c_longlong.from_address(self._xchg_status.data_ptr())
@@ -599,9 +602,9 @@ class MPPI:
         self._host_template = torch.empty(self._host_out_shape, dtype=self.dtype)
 
     def _drop_plan(self):
-        plan = getattr(self, "_plan", None)
+        plan = getattr(self, "_plan", None)     # __del__ of a controller whose __init__ raised before _plan was set
         if plan is not None:
-            if getattr(self, "_resident", False):        # mppi_plan_destroy sends the resident grid away
+            if self._resident:        # mppi_plan_destroy sends the resident grid away
                 self._resident, self._resident_wanted = False, self._resident_idle_us
             # the next plan continues this one's command epochs (the tags of the reduction / exchange records)
             self._epoch = max(self._epoch, int(self._lib.mppi_plan_epoch(plan)))
@@ -658,14 +661,8 @@ class MPPI:
             return self._rng_seed, base, chunks
         gen = torch.cuda.default_generators[self.d.index]
         seed = gen.initial_seed() & 0xFFFFFFFFFFFFFFFF
-        try:
-            off = gen.get_offset()
-            gen.set_offset(off + 4 * chunks * n)
-        except (AttributeError, RuntimeError):   # very old torch: private counter keyed by the seed
-            if getattr(self, "_rng_last_seed", None) != seed:
-                self._rng_last_seed, self._rng_counter = seed, 0
-            off = 4 * self._rng_counter
-            self._rng_counter += n * chunks
+        off = gen.get_offset()
+        gen.set_offset(off + 4 * chunks * n)
         return seed, off // 4, chunks
 
     def refresh(self):
@@ -710,19 +707,16 @@ class MPPI:
         setters, not through views obtained earlier.
         Requires a registered analytic model on the split-cost rollout (a problem of at most one tile per SM, e.g.
         BASELINE config 2), host states and a single-GPU controller."""
-        if self._dirty:
-            self._pack()
+        self._prepare(leave_resident=False)        # an armed grid is re-armed below
         if self._model is None or self._plan is None:
             raise _cabi.MppiLibraryError("resident mode needs a registered model (the fused route)")
-        if getattr(self._model, "_param_version", 0) != self._model_version:
-            self._take_model_params()
         if self._z_out is not None:
             raise _cabi.MppiLibraryError("resident mode does not record noise; call record_noise(False) first")
         if self.launch_info.global_tile:
             raise _cabi.MppiLibraryError("resident mode keeps its tiles in shared memory: not available on a global-tile plan "
                                          "(tile_memory)")
         words = 64 + self.u_per_command * self.nu * (2 if self.dtype == torch.float64 else 1)
-        if getattr(self, "_res_box", None) is None or self._res_box.numel() != words:
+        if self._res_box is None or self._res_box.numel() != words:
             self._res_box = torch.zeros(words, dtype=torch.int64).pin_memory()
             self._res_board = torch.zeros(128, dtype=torch.int64, device=self.d)
             self._res_stream = torch.cuda.Stream(device=self.d)       # non-blocking, used for nothing else
@@ -758,29 +752,23 @@ class MPPI:
 
     def _resident_sync(self):
         """Reads of device-side results: wait until the resident grid finished writing the last command's."""
-        if getattr(self, "_resident", False):
+        if self._resident:
             _cabi.check(self._lib.mppi_resident_sync(self._plan), "mppi_resident_sync")
 
     def _leave_resident(self):
         """Writes to controller state / launch-route commands: the grid leaves now, the next command_host() re-enters."""
-        if getattr(self, "_resident", False):
+        if self._resident:
             _cabi.check(self._lib.mppi_resident_stop(self._plan), "mppi_resident_stop")
             self._resident, self._resident_wanted = False, self._resident_idle_us
 
     def _command_resident(self, shift):
         flags = self._base_flags | (_cabi.FLAG_SHIFT if shift else 0)
         _, seed, off = self._noise_source()
-        self._last = (flags, seed, off, None, None)
-        self._cmd_count += 1
         out = torch.empty_like(self._host_template)
         rc = self._lib.mppi_resident_command(self._plan, self._state_arr, flags, seed, off, out.data_ptr())
         if rc != 0:
             _cabi.check(rc, "mppi_resident_command")
-        if self._world > 1:
-            self._epoch += 1           # mirrors the plan's exchange epoch, as on the launch route
-        self._cost_total = self._cost_buf
-        self._states = None
-        self._actions = None
+        self._commanded((flags, seed, off, None, None))
         return out
 
     # ------------------------------------------------------------------------------------------
@@ -798,7 +786,7 @@ class MPPI:
 
     # ---- CUDA-graph replay of the stepped route ---------------------------------------------------
     def _graph_eligible(self, state):
-        return (getattr(self, "_graph_mode", False) and self._z_inject is None and self._z_out is None and self._world == 1
+        return (self._graph_mode and self._z_inject is None and self._z_out is None and self._world == 1
                 and self.specific_action_sampler is None)
 
     def _command_graphed(self, state, shift):
@@ -819,35 +807,23 @@ class MPPI:
                 except Exception:      # noqa: BLE001 — best effort; older torch has no graph-safe generator states
                     pass
                 return self._command_stepped(state, shift)
-        g, st_static, action_static, cost_buf = self._graphs[key]
+        g, st_static, action_static, cost_buf, states, actions = self._graphs[key]
         st_static.copy_(st)
         g.replay()
-        self._cmd_count += 1
-        self._materialized_at["noise"] = self._cmd_count
-        self._last = None
         self._cost_buf = cost_buf                      # the buffer THIS graph writes (several keys = several graphs)
         self._p.cost_total = cost_buf.data_ptr()
-        self.cost_total = self._cost_buf
+        self._commanded(None)
+        self._materialized_at["noise"] = self._cmd_count
+        self._states, self._actions = states, actions  # the graph's own, rewritten by every replay
         out = action_static.clone()
         return out[0] if self.u_per_command == 1 else out
 
-    def _nominal_snapshot(self):
-        snap = {"U": self._Ubuf.clone()}
-        if getattr(self, "_Abuf", None) is not None:
-            snap["A"] = self._Abuf.clone()
-        if getattr(self, "_theta", None) is not None:
-            snap["theta"] = self._theta.clone()
-        return snap
-
-    def _nominal_restore(self, snap):
-        self._Ubuf.copy_(snap["U"])
-        if "A" in snap:
-            self._Abuf.copy_(snap["A"])
-        if "theta" in snap:
-            self._theta.copy_(snap["theta"])
+    def _nominal_buffers(self):
+        """The device buffers a command updates in place."""
+        return [self._Ubuf]
 
     def _capture_graph(self, key, st, shift):
-        if getattr(self, "_offset_dev", None) is None:
+        if self._offset_dev is None:
             # continue the host-side stream on the device: same seed, counter where the host counter stands
             if self._rng_seed is not None:
                 self._graph_seed, start = self._rng_seed, self._rng_counter
@@ -858,7 +834,7 @@ class MPPI:
         if self._dirty:
             self._pack()
         st_static = st.clone()
-        snap = self._nominal_snapshot()
+        snap = [b.clone() for b in self._nominal_buffers()]
         off0 = self._offset_dev.clone()
         count0 = self._cmd_count
         try:
@@ -872,17 +848,18 @@ class MPPI:
             torch.cuda.synchronize(self.d)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                p, action = self._begin_command(st_static, shift)
+                p, action = self._begin_command(shift)
                 action = self._stepped_body(p, action, st_static)
-            cost_buf = self._cost_buf                           # this graph's own result buffer
         finally:
             # the warm-up (and a failed capture) ran real commands: undo them whatever happened, so that the caller's
             # command() — replayed from the graph, or re-run eagerly after a capture failure — is the only one applied
             torch.cuda.synchronize(self.d)
-            self._nominal_restore(snap)
+            for b, s in zip(self._nominal_buffers(), snap):
+                b.copy_(s)
             self._offset_dev.copy_(off0)
             self._cmd_count = count0
-        self._graphs[key] = (g, st_static, action, cost_buf)
+        # this graph's own result buffers
+        self._graphs[key] = (g, st_static, action, self._cost_buf, self._states, self._actions)
 
     def get_params(self):
         return f"K={self.K} T={self.T} M={self.M} lambda={self.lambda_} noise_mu={self.noise_mu.cpu().numpy()} noise_sigma={self.noise_sigma.cpu().numpy()}".replace(
@@ -918,14 +895,37 @@ class MPPI:
         self._alloc_results()
         self._dirty = True
 
+    def _prepare(self, leave_resident=True):
+        """Before every command: the resident grid leaves (unless the command goes to it), the packed constants are
+        current, the plan holds the model's latest parameters, and no earlier peer exchange timed out."""
+        if leave_resident:
+            self._leave_resident()
+        if self._dirty:
+            self._pack()
+        if getattr(self._model, "_param_version", 0) != self._model_version:      # the stepped route has no model
+            self._take_model_params()
+        if self._world > 1:
+            self._check_exchange_status()
+
+    def _commanded(self, last, n=1):
+        """After every `n` commands: the count that keys the lazily materialised intermediates, the last command's launch
+        values `last` ((flags, seed, offset, z, state pointer) to materialise from, or None), its costs, and on a
+        sharded controller the exchange epoch, which mirrors the plan's."""
+        self._cmd_count += n
+        self._last = last
+        self._cost_total = self._cost_buf
+        self._states = None
+        self._actions = None
+        if self._world > 1:
+            self._epoch += n
+
     def command(self, state, shift_nominal_trajectory=True, info=None):
         """mppi.py:240-252: returns the first `u_per_command` actions of the updated sequence."""
         self.info = info
-        self._leave_resident()
-        if self._dirty:
-            self._pack()
+        self._prepare()
         if self._model is not None:
-            return self._command_fused(state, shift_nominal_trajectory)
+            action = self._command_fused(*self._host_state(state), shift_nominal_trajectory)
+            return action[0] if self.u_per_command == 1 else action                        # mppi.py:273-274
         if self._graph_eligible(state):
             return self._command_graphed(state, shift_nominal_trajectory)
         return self._command_stepped(state, shift_nominal_trajectory)
@@ -963,7 +963,7 @@ class MPPI:
         """A peer exchange that timed out inside an earlier command left this rank's nominal one update behind its
         peers (the kernel returned the un-updated nominal as the action and flagged a pinned status word): refuse to
         continue silently."""
-        st = getattr(self, "_xchg_status_word", None)
+        st = self._xchg_status_word
         if st is not None and st.value != 0:
             code = int(st.value)
             st.value = 0
@@ -979,35 +979,26 @@ class MPPI:
             self._z_inject = None
             return self._z_keep.data_ptr(), 0, 0
         self._z_keep = None
-        if getattr(self, "_offset_dev", None) is not None:     # counter lives on the device (CUDA-graph mode)
+        if self._offset_dev is not None:     # counter lives on the device (CUDA-graph mode)
             return None, self._graph_seed, 0
         seed, off = self._next_rng()
         return None, seed, off
 
-    def _command_fused(self, state, shift):
-        if getattr(self._model, "_param_version", 0) != self._model_version:
-            self._take_model_params()
-        if self._world > 1:
-            self._check_exchange_status()
-        sflags, sdev = self._host_state(state)
+    def _command_fused(self, sflags, sdev, shift):
+        """One launch of the plan from the state `_host_state` (or MPPI_Batched) gave; returns the ([N,] u_per_command, nu)
+        action."""
         flags = self._base_flags | sflags | (_cabi.FLAG_SHIFT if shift else 0)
         zptr, seed, off = self._noise_source()
-        action = torch.empty((self.u_per_command, self.nu), device=self.d, dtype=self.dtype)
+        action = torch.empty(self._env_axis + (self.u_per_command, self.nu), device=self.d, dtype=self.dtype)
         stream = torch._C._cuda_getCurrentRawStream(self.d.index)
-        self._last = (flags, seed, off, zptr, sdev)
-        self._cmd_count += 1
         rc = self._lib.mppi_plan_command(self._plan, None if sdev is not None else self._state_arr, sdev, flags, seed, off,
                                          zptr, action.data_ptr(), stream)
         if rc != 0:
             _cabi.check(rc, "mppi_plan_command")
-        if self._world > 1:
-            self._epoch += 1
-            if self._exchange != "p2p":
-                self._finish_exported(action, stream)
-        self.cost_total = self._cost_buf
-        self._states = None
-        self._actions = None
-        return action[0] if self.u_per_command == 1 else action                            # mppi.py:273-274
+        if self._world > 1 and self._exchange != "p2p":
+            self._finish_exported(action, stream)
+        self._commanded((flags, seed, off, zptr, sdev))
+        return action
 
     def _finish_exported(self, action, stream):
         """NCCL route: all-gather the per-rank records, then `mppi_apply_partials` finishes the update."""
@@ -1030,7 +1021,7 @@ class MPPI:
             p.state[i] = self._state_arr[i]
 
     # -- struct-based command setup used by the stepped route ------------------------------------
-    def _begin_command(self, state, shift):
+    def _begin_command(self, shift):
         p = self._p
         flags = self._base_flags | (_cabi.FLAG_SHIFT if shift else 0)
         zptr, seed, off = self._noise_source()
@@ -1039,26 +1030,13 @@ class MPPI:
         p.state_dev = None
         p.z_out = None if self._z_out is None else self._z_out.data_ptr()
         if self._world > 1:
-            self._epoch += 1
-            p.epoch = self._epoch
+            p.epoch = self._epoch + 1          # this command's; _commanded advances _epoch to it
             if self._exchange != "p2p":
                 flags |= _cabi.FLAG_EXPORT_PARTIAL
         p.flags = flags
-        action = torch.empty((self.u_per_command, self.nu), device=self.d, dtype=self.dtype)
+        action = torch.empty(self._env_axis + (self.u_per_command, self.nu), device=self.d, dtype=self.dtype)
         p.action_out = action.data_ptr()
-        self._cmd_count += 1
-        self._last = None
         return p, action
-
-    def _finish_command(self, p, action, stream):
-        if self._world > 1 and self._exchange != "p2p":
-            self._finish_exported(action, stream)
-        self.cost_total = self._cost_buf
-        self._states = None
-        self._actions = None
-        if self.u_per_command == 1:                                                        # mppi.py:273-274
-            return action[0]
-        return action
 
     def command_host(self, state, shift_nominal_trajectory=True, info=None):
         """`command()` for a control loop that lives on the host: the start state travels in the
@@ -1078,64 +1056,61 @@ class MPPI:
         sflags, sdev = self._host_state(state)
         if sdev is not None:
             return self.command(state, shift_nominal_trajectory, info).cpu()
-        if getattr(self._model, "_param_version", 0) != self._model_version:
-            self._take_model_params()       # a resident grid leaves; the branch below brings it back
-        if self._resident or self._resident_wanted:
-            if self._z_inject is None and getattr(self, "_offset_dev", None) is None:
-                if not self._resident:
-                    self.start_resident(self._resident_wanted)
-                return self._command_resident(shift_nominal_trajectory)
-            self._leave_resident()         # injected noise / device-resident counter: a launch-route command
-        if self._world > 1:
-            self._check_exchange_status()
+        # injected noise and a device-resident counter take the launch route
+        resident = (self._resident or self._resident_wanted) and self._z_inject is None and self._offset_dev is None
+        self._prepare(leave_resident=not resident)     # new model parameters make the grid leave all the same
+        if resident:
+            if not self._resident:
+                self.start_resident(self._resident_wanted)
+            return self._command_resident(shift_nominal_trajectory)
         flags = self._base_flags | (_cabi.FLAG_SHIFT if shift_nominal_trajectory else 0)
         zptr, seed, off = self._noise_source()
         stream = torch._C._cuda_getCurrentRawStream(self.d.index)
-        self._last = (flags, seed, off, zptr, None)
-        self._cmd_count += 1
         out = torch.empty_like(self._host_template)
         self._host_epoch += 1
         rc = self._lib.mppi_plan_command_host(self._plan, self._state_arr, flags, seed, off, zptr,
                                               self._scratch_action.data_ptr(), self._host_box.data_ptr(), out.data_ptr(), stream)
         if rc != 0:
             _cabi.check(rc, "mppi_plan_command_host")
-        if self._world > 1:
-            self._epoch += 1
-        self._cost_total = self._cost_buf
-        self._states = None
-        self._actions = None
+        self._commanded((flags, seed, off, zptr, None))
         return out
 
     # ------------------------------------------------------------------------------------------
     # stepped route (arbitrary callables): mppi.py:297-373 with kernels around the T-loop
     # ------------------------------------------------------------------------------------------
     def _ensure_step_buffers(self):
-        K, T, nu = self._K_local, self.T, self.nu
-        if getattr(self, "_pa_buf", None) is None or self._pa_buf.shape != (K, T, nu):
-            self._pa_buf = torch.empty(K, T, nu, device=self.d, dtype=self.dtype)
-            self._noise_buf = torch.empty(K, T, nu, device=self.d, dtype=self.dtype)
-            self._cost_init = torch.empty(K, device=self.d, dtype=self.dtype)
+        shape = self._env_axis + (self._K_local, self.T, self.nu)
+        if self._pa_buf is None or self._pa_buf.shape != shape:
+            self._pa_buf = torch.empty(shape, device=self.d, dtype=self.dtype)
+            self._noise_buf = torch.empty(shape, device=self.d, dtype=self.dtype)
+            self._cost_init = torch.empty(shape[:-2], device=self.d, dtype=self.dtype)
             self._noise_theta_buf = None
 
     def _eps_for_update(self):
         return self._noise_buf
 
+    def _start_rows(self, st):
+        """The (K_local, nx) start state of every sample: the state, or this shard's rows of a (K, nx) batch of them."""
+        K = self._K_local
+        if st.shape == (self.K, self.nx) and self.K != 1:
+            return st[self._k_offset:self._k_offset + K].clone()
+        return st.view(1, -1).expand(K, -1)
+
     def _command_stepped(self, state, shift):
-        lib = self._lib
         self._ensure_step_buffers()
         if not torch.is_tensor(state):
             state = torch.tensor(state)
         st = state.to(dtype=self.dtype, device=self.d)                                     # mppi.py:262-264
-        p, action = self._begin_command(st, shift)
+        p, action = self._begin_command(shift)
         out = self._stepped_body(p, action, st)
         return out[0] if self.u_per_command == 1 else out
 
     def _stepped_body(self, p, action, st):
-        """Everything of one stepped command that runs on the device; returns the (u_per_command, nu) action."""
+        """Everything of one stepped command that runs on the device; returns the ([N,] u_per_command, nu) action."""
         lib = self._lib
         self.state = st
         stream = torch.cuda.current_stream(self.d).cuda_stream
-        K, T, nu = self._K_local, self.T, self.nu
+        T, nu = self.T, self.nu
 
         ovr_ptr, n_ovr, ovr_start = None, 0, 0
         if self.specific_action_sampler is not None:                                       # mppi.py:393-399
@@ -1150,33 +1125,30 @@ class MPPI:
         _cabi.check(lib.mppi_sample_perturb(C.byref(p), self._pa_buf.data_ptr(), self._noise_buf.data_ptr(), nth,
                                             self._cost_init.data_ptr(), ovr_ptr, n_ovr, ovr_start, stream),
                     "mppi_sample_perturb")
-        self._materialized_at["noise"] = self._cmd_count
 
-        if self.M == 1:
-            rollout, states, actions = self._rollout_single(self._pa_buf, stream)
-        else:
-            rollout, states, actions = self._rollout_multi(self._pa_buf, stream)
+        rollout_fn = self._rollout_single if self.M == 1 else self._rollout_multi
+        # the batched controller's N*K samples are rows of one rollout
+        rollout, states, actions = rollout_fn(self._pa_buf.view(-1, T, nu), self._start_rows(st), stream)
         # cost_total = rollout + perturbation (+ smoothness), mppi.py:416 / :569
-        _cabi.check(lib.mppi_cost_accumulate(rollout.data_ptr(), self._cost_init.data_ptr(), None, 1, K, 1.0,
+        _cabi.check(lib.mppi_cost_accumulate(rollout.data_ptr(), self._cost_init.data_ptr(), None, 1, rollout.numel(), 1.0,
                                              _DT[self.dtype], stream), "mppi_cost_accumulate")
-        self._cost_buf = rollout
+        self._cost_buf = rollout.view_as(self._cost_init)
         p.cost_total = rollout.data_ptr()
         _cabi.check(lib.mppi_softmin_update(C.byref(p), rollout.data_ptr(), self._eps_for_update().data_ptr(), stream),
                     "mppi_softmin_update")
-        self._finish_command(p, action, stream)
+        if self._world > 1 and self._exchange != "p2p":
+            self._finish_exported(action, stream)
+        self._commanded(None)
+        self._materialized_at["noise"] = self._cmd_count
         self._states = states
         self._actions = actions / self._u_scale if actions is not None else None         # mppi.py:412
         return action
 
-    def _rollout_single(self, perturbed_actions, stream):
-        """mppi.py:297-332"""
+    def _rollout_single(self, perturbed_actions, state, stream):
+        """mppi.py:297-332, from the (K, nx) start rows `state`"""
         lib = self._lib
         K, T, nu = perturbed_actions.shape
         cost_total = torch.zeros(K, device=self.d, dtype=self.dtype)
-        if self.state.shape == (self.K, self.nx) and self.K != 1:
-            state = self.state[self._k_offset:self._k_offset + K].clone()
-        else:
-            state = self.state.view(1, -1).expand(K, -1)
         need_storage = self.terminal_state_cost is not None
         states = actions = None
         if need_storage:
@@ -1210,18 +1182,14 @@ class MPPI:
                 cost_total += c
         return cost_total, states, actions
 
-    def _rollout_multi(self, perturbed_actions, stream):
-        """mppi.py:334-373 (M>1: stochastic dynamics with a discounted variance cost)"""
+    def _rollout_multi(self, perturbed_actions, state, stream):
+        """mppi.py:334-373 (M>1: stochastic dynamics with a discounted variance cost), from the (K, nx) start rows"""
         lib = self._lib
         K, T, nu = perturbed_actions.shape
         M = self.M
         dt = _DT[self.dtype]
         cost_samples = torch.zeros(M, K, device=self.d, dtype=self.dtype)
         cost_var = torch.zeros(K, device=self.d, dtype=self.dtype)
-        if self.state.shape == (self.K, self.nx) and self.K != 1:
-            state = self.state[self._k_offset:self._k_offset + K]
-        else:
-            state = self.state.view(1, -1).expand(K, -1)
         state = state.repeat(M, 1, 1)
         states = torch.empty(M, K, T, self.nx, device=self.d, dtype=self.dtype)
         actions = torch.empty(M, K, T, nu, device=self.d, dtype=self.dtype)
@@ -1258,7 +1226,7 @@ class MPPI:
             return True
         self._ensure_step_buffers()
         p = self._p
-        if getattr(self, "_last", None) is not None:
+        if self._last is not None:
             self._sync_params_for_materialize()
         stream = torch.cuda.current_stream(self.d).cuda_stream
         nth = None if self._noise_theta_buf is None else self._noise_theta_buf.data_ptr()
@@ -1406,7 +1374,7 @@ class MPPI:
             raise ValueError("run_closed_loop draws its noise from the RNG stream: a noise tensor is injected (inject_noise)")
         if self._z_out is not None:
             raise ValueError("run_closed_loop does not record the noise it draws: call record_noise(False) first")
-        if getattr(self, "_offset_dev", None) is not None:
+        if self._offset_dev is not None:
             raise ValueError("run_closed_loop: this controller's Philox counter lives on the device (compile() captured a "
                              "CUDA graph); build a controller without compile() for closed loops")
         if not torch.is_tensor(state) or state.dtype != self.dtype or state.device != self.d or \
@@ -1429,12 +1397,7 @@ class MPPI:
                 raise ValueError(f"plant_params must have shape {' or '.join(map(str, shapes))} (the model's "
                                  f"param_blob() + param_blob_ext()), got {tuple(pt.shape)}")
             plant = pt.detach().to("cpu", torch.float64).reshape(-1, n_params).contiguous()
-        # ---- the controller as command() leaves it for a launch --------------------------------------------------------
-        self._leave_resident()
-        if self._dirty:
-            self._pack()
-        if getattr(m, "_param_version", 0) != self._model_version:
-            self._take_model_params()
+        self._prepare()
         lib = self._lib
         seed, base, stride = self._rng_block(steps)
         states = torch.empty((steps + 1,) + lead + (self.nx,), device=self.d, dtype=self.dtype)
@@ -1450,16 +1413,12 @@ class MPPI:
                                   n_plant_params=n_params if plant is not None else 0, plant_blocks=blocks.data_ptr())
         stream = torch._C._cuda_getCurrentRawStream(self.d.index)
         _cabi.check(lib.mppi_plan_closed_loop(self._plan, C.byref(cl), stream), "mppi_plan_closed_loop")
-        # ---- bookkeeping of the last command (lazy noise / perturbed_action, materialised from its state row) ----------
-        self._cmd_count += steps
+        # ---- the last command (lazy noise / perturbed_action are materialised from its state row) ---------------------
         self._z_keep = None
         last = states[steps - 1]
         self.state = last                  # keeps the rows the last command read alive for materialisation
-        self._last = (self._base_flags | _cabi.FLAG_STATE_DEVICE | _cabi.FLAG_SHIFT, seed, base + (steps - 1) * stride, None,
-                      last.data_ptr())
-        self.cost_total = self._cost_buf
-        self._states = None
-        self._actions = None
+        self._commanded((self._base_flags | _cabi.FLAG_STATE_DEVICE | _cabi.FLAG_SHIFT, seed, base + (steps - 1) * stride,
+                         None, last.data_ptr()), steps)
         return ClosedLoopResult(states, actions, costs)
 
 
@@ -1473,6 +1432,7 @@ class SMPPI(MPPI):
         self.w_action_seq_cost = w_action_seq_cost
         self.delta_t = delta_t
         self._Abuf = None
+        self._A_view = None             # the (T, nu) view `action_sequence` hands out
         super().__init__(*args, U_init=U_init, **kwargs)
         if action_min is not None and action_max is None:                                  # mppi.py:464-477
             action_min = torch.as_tensor(action_min)
@@ -1502,12 +1462,15 @@ class SMPPI(MPPI):
             n = min(old.numel(), self._Abuf.numel())
             self._Abuf[:n].copy_(old[:n])
 
+    def _nominal_buffers(self):
+        return super()._nominal_buffers() + [self._Abuf]
+
     @property
     def action_sequence(self):
         self._resident_sync()
         # one view object per buffer: `ctrl.get_action_sequence() is ctrl.action_sequence` holds as in the reference
         # (test_mppi.py:452-456), and the kernels update it in place
-        v = getattr(self, "_A_view", None)
+        v = self._A_view
         if v is None or v.data_ptr() != self._Abuf.data_ptr() or v.shape != (self.T, self.nu):
             v = self._A_view = self._Abuf[: self.T * self.nu].view(self.T, self.nu)
         return v
@@ -1665,6 +1628,9 @@ class KMPPI(MPPI):
         self.U = self._W @ self._theta
         self._dirty = True
 
+    def _nominal_buffers(self):
+        return super()._nominal_buffers() + [self._theta]
+
     def _variant_pack(self, p):
         p.S = self.num_support_pts
         p.theta = self._theta.data_ptr()
@@ -1709,6 +1675,7 @@ class MPPI_Batched(MPPI):
                  step_dependent_dynamics=False, noise_abs_cost=False, *, rng_seed=None, block_threads=0,
                  tile_memory="shared"):
         self.N = int(num_envs)
+        self._env_axis = (self.N,)
         # per-environment settings (set_env_params): None = the controller's shared value
         self._env_model_params = self._env_lambda = self._env_sigma = self._env_mu = None
         self._env_factors = None          # (diagonal, L, inverse, sqrt-diagonal) per environment of _env_sigma
@@ -1722,20 +1689,6 @@ class MPPI_Batched(MPPI):
                          tile_memory=tile_memory)
 
     # ---- (N, ...) buffers ------------------------------------------------------------------------
-    def _alloc_nominal(self, U_init):
-        es = _ES[self.dtype]
-        self._u_stride = _pad16(self.T * self.nu, es)
-        self._Ubuf = torch.zeros(self.N, self._u_stride, device=self.d, dtype=self.dtype)
-        self.U = self._sample_noise((self.N, self.T)) if U_init is None else U_init          # mppi.py:807
-
-    def _alloc_results(self):
-        tn = self.T * self.nu
-        self._cost_buf = torch.empty(self.N, self.K, device=self.d, dtype=self.dtype)
-        self._nominal_used = torch.zeros(self.N, 3 * tn + 4, device=self.d, dtype=self.dtype)
-        self._stats = torch.zeros(self.N, 4, device=self.d, dtype=torch.float64)
-        self._workspace = None
-        self._partial = None
-
     @property
     def U(self):
         return self._Ubuf[:, : self.T * self.nu].view(self.N, self.T, self.nu)
@@ -1747,7 +1700,7 @@ class MPPI_Batched(MPPI):
 
     def _variant_pack(self, p):
         p.n_env = self.N
-        p.env_u_stride = self._u_stride
+        p.env_u_stride = self._Ubuf.shape[1]
 
     def reset(self):
         """mppi.py:819-820; with per-environment horizons, the rows past each environment's horizon hold u_init."""
@@ -1989,50 +1942,17 @@ class MPPI_Batched(MPPI):
             states = torch.tensor(states)
         states = states.to(dtype=self.dtype, device=self.d).reshape(self.N, self.nx).contiguous()
         self.state = states
-        if self._dirty:
-            self._pack()
-        N, K, T, nu = self.N, self.K, self.T, self.nu
-        action = torch.empty((N, self.u_per_command, nu), device=self.d, dtype=self.dtype)
-        stream = torch._C._cuda_getCurrentRawStream(self.d.index)
-        flags = self._base_flags | _cabi.FLAG_STATE_DEVICE | (_cabi.FLAG_SHIFT if shift_nominal_trajectory else 0)
-        zptr, seed, off = self._noise_source()
-        self._cmd_count += 1
+        self._prepare()
         if self._model is not None:
-            if getattr(self._model, "_param_version", 0) != self._model_version:
-                self._take_model_params()
-            self._last = (flags, seed, off, zptr, states.data_ptr())
-            _cabi.check(self._lib.mppi_plan_command(self._plan, None, states.data_ptr(), flags, seed, off, zptr,
-                                                    action.data_ptr(), stream), "mppi_plan_command")
+            action = self._command_fused(_cabi.FLAG_STATE_DEVICE, states.data_ptr(), shift_nominal_trajectory)
         else:
-            self._last = None
-            p = self._p
-            p.flags = flags & ~_cabi.FLAG_STATE_DEVICE
-            p.z, p.seed, p.offset = zptr, seed, off
-            p.action_out = action.data_ptr()
-            if getattr(self, "_pa_buf", None) is None or self._pa_buf.shape != (N, K, T, nu):
-                self._pa_buf = torch.empty(N, K, T, nu, device=self.d, dtype=self.dtype)
-                self._noise_buf = torch.empty(N, K, T, nu, device=self.d, dtype=self.dtype)
-                self._cost_init = torch.empty(N, K, device=self.d, dtype=self.dtype)
-            lib = self._lib
-            _cabi.check(lib.mppi_sample_perturb(C.byref(p), self._pa_buf.data_ptr(), self._noise_buf.data_ptr(), None,
-                                                self._cost_init.data_ptr(), None, 0, 0, stream), "mppi_sample_perturb")
-            NK = N * K
-            state = states.unsqueeze(1).expand(N, K, self.nx).reshape(NK, self.nx)                # mppi.py:846
-            total = torch.zeros(N, K, device=self.d, dtype=self.dtype)
-            dt = _DT[self.dtype]
-            for t in range(T):                                                                    # mppi.py:849-853
-                u = self._u_scale * self._pa_buf[:, :, t].reshape(NK, nu)
-                state = self._dynamics_fn(state, u, t)
-                c = self._running_cost_fn(state, u, t).reshape(NK).to(self.dtype).contiguous()
-                _cabi.check(lib.mppi_cost_accumulate(total.data_ptr(), c.data_ptr(), None, 1, NK, 1.0, dt, stream),
-                            "mppi_cost_accumulate")
-            _cabi.check(lib.mppi_cost_accumulate(total.data_ptr(), self._cost_init.data_ptr(), None, 1, NK, 1.0, dt, stream),
-                        "mppi_cost_accumulate")
-            self._cost_buf = total
-            _cabi.check(lib.mppi_softmin_update(C.byref(p), total.data_ptr(), self._noise_buf.data_ptr(), stream),
-                        "mppi_softmin_update")
-        self.cost_total = self._cost_buf
+            self._ensure_step_buffers()
+            action = self._stepped_body(*self._begin_command(shift_nominal_trajectory), states)
         return action[:, 0] if self.u_per_command == 1 else action                               # mppi.py:870-873
+
+    def _start_rows(self, st):
+        """Every environment's state for each of its K samples: (N*K, nx)."""
+        return st.unsqueeze(1).expand(self.N, self.K, self.nx).reshape(self.N * self.K, self.nx)    # mppi.py:846
 
     def run_closed_loop(self, states, steps, *, plant_params=None, disturbance=None):
         """`MPPI.run_closed_loop` for the N environments: states (N, nx); plant_params (n_params,) for one plant or
