@@ -1,7 +1,11 @@
 """CPU: the per-sample math header the kernels are built from (csrc/mppi_math.cuh), compiled for the host
 with g++ (tests/emu/emu_math.cpp — test infrastructure, never part of the product path), against the oracle:
 Philox known answers, the normal-stream definition, model rollouts (states and accumulated cost), noise
-colouring and the action-cost term, torch.remainder semantics."""
+colouring and the action-cost term, torch.remainder semantics.
+
+g++ takes the header's host branch.  For the float primitives with a separate device body (fmod_, fmod_small_ and
+remainder, tanh_ and tanh4_, Normals<float>::pair) that branch is plain libm, so this file checks the host bodies only;
+tests/test_gpu_device_math.py checks the device bodies on the GPU."""
 import ctypes as C
 import math
 import os
