@@ -1,9 +1,15 @@
-"""Golden-case table shared by make_golden.py (which runs the live reference) and the tests
-(which replay the committed .npz files against the oracle and the CUDA engine).
+"""Golden fixture families, and the base family's case tables.
 
-Each case is plain JSON-able data.  `draw_z` defines the injected standard-normal stream.
+A family is a table of cases plus the .npz fixtures tests/golden/make_golden.py makes from them by running the live
+reference; the tests replay those fixtures against the oracle (tests/golden/replay.py) and the CUDA engine
+(tests/golden/engine.py).  `Family` holds what differs between families; everything else is shared.
+
+Each case is plain JSON-able data; a case with "N" is an MPPI_Batched case.  `draw_z` defines the injected
+standard-normal stream.
 """
 import math
+from dataclasses import dataclass
+from typing import Callable
 
 import numpy as np
 import torch
@@ -116,6 +122,23 @@ BATCHED_CASES = {
 }
 
 
+@dataclass(frozen=True)
+class Family:
+    """What one fixture family supplies; cases with "N" run MPPI_Batched, the others MPPI / SMPPI / KMPPI."""
+    name: str
+    cases: dict
+    # (case, fixture) -> (the oracle's Problem, plant): plant(x, u) steps the closed loop's simulated system on rows of
+    # states and scaled actions.  `fixture` maps the names of the extra arrays (below) to their values.
+    model: Callable
+    # (case, oracle Problem, fixture) -> (dynamics, running_cost, controller keywords) the live reference is given; the
+    # keyword `specific_actions` (state -> (n,T,nu)) becomes a SpecificActionSampler
+    reference: Callable
+    # case -> the extra arrays the fixture stores and `model` reads (networks, maps)
+    fixture: Callable = lambda case: {}
+    smooth_key: str = "A"           # the fixture key of SMPPI's action sequence
+    scalars: bool = True            # whether the fixture stores cost_sum, beta and eta per step
+
+
 def make_mlp_net(seed, dtype):
     """pendulum_approximate.py:35, 47-53: seed, then build the network (no draws in between)."""
     torch.manual_seed(seed)
@@ -130,10 +153,10 @@ def mlp_state_arrays(net):
     return {f"mlp_{k.replace('.', '_')}": v.detach().cpu().numpy() for k, v in net.state_dict().items()}
 
 
-def load_mlp_net(gold, dtype):
+def load_mlp_net(fixture, dtype):
     """The network a fixture was generated with (weights stored in the .npz)."""
     net = make_mlp_net(0, dtype)
-    sd = {k: torch.from_numpy(np.asarray(gold[f"mlp_{k.replace('.', '_')}"])).to(dtype) for k in net.state_dict()}
+    sd = {k: torch.from_numpy(np.asarray(fixture[f"mlp_{k.replace('.', '_')}"])).to(dtype) for k in net.state_dict()}
     net.load_state_dict(sd)
     return net
 
@@ -169,7 +192,7 @@ def draw_z(gen: np.random.Generator, shape, dtype: torch.dtype, z_dtype=None):
     return torch.from_numpy(gen.standard_normal(shape, dtype=np_dt)).to(dtype)
 
 
-def build_problem(case, gold=None):
+def build_problem(case, fixture):
     dt = _DT[case["dtype"]]
     m = case["model"]
     if m["kind"] == "pendulum":
@@ -177,7 +200,7 @@ def build_problem(case, gold=None):
         model.has_terminal = False
         model.terminal_cost = None
     elif m["kind"] == "pendulum_mlp":
-        model = MlpPendulumModel(load_mlp_net(gold, dt) if gold is not None else make_mlp_net(m["seed"], dt))
+        model = MlpPendulumModel(load_mlp_net(fixture, dt))
     elif m["kind"] == "shape":
         from tests.golden.shape_cases import ShapeTwin
         model = ShapeTwin(m)
@@ -205,3 +228,57 @@ def build_problem(case, gold=None):
         rollout_var_discount=case.get("rollout_var_discount", 0.95),
         specific_actions=(lambda state: sampler_actions(case, state)) if case.get("sampler") is not None else None)
     return prob, model
+
+
+def _base_fixture(case):
+    m = case["model"]
+    return mlp_state_arrays(make_mlp_net(m["seed"], _DT[case["dtype"]])) if m["kind"] == "pendulum_mlp" else {}
+
+
+def _base_model(case, fixture):
+    prob, _ = build_problem(case, fixture)
+    return prob, prob.dynamics
+
+
+def _pendulum_plugins():
+    """The pendulum written with the same np.sin / np.clip-on-tensor calls as reference tests/pendulum.py:30-60, so the
+    fixtures also pin that those equal the oracle's torch.sin / torch.clamp."""
+    def dynamics(state, perturbed_action):
+        th = state[:, 0].view(-1, 1)
+        thdot = state[:, 1].view(-1, 1)
+        g, m, l, dt = 10, 1, 1, 0.05
+        u = torch.clamp(perturbed_action, -2, 2)
+        newthdot = thdot + (3 * g / (2 * l) * np.sin(th) + 3.0 / (m * l ** 2) * u) * dt
+        newthdot = np.clip(newthdot, -8, 8)
+        newth = th + newthdot * dt
+        return torch.cat((newth, newthdot), dim=1)
+
+    def angle_normalize(x):
+        return ((x + math.pi) % (2 * math.pi)) - math.pi
+
+    def running_cost(state, action):
+        return angle_normalize(state[:, 0]) ** 2 + 0.1 * state[:, 1] ** 2
+
+    return dynamics, running_cost
+
+
+def _base_reference(case, prob, fixture):
+    """Every model but the pendulum hands the reference the callables of the oracle's problem (the MLP network and the
+    per-copy offset dynamics are torch callables)."""
+    dt = prob.dtype
+    bd = torch.float32 if case.get("bounds_fp32") else dt
+    kw = {k: case[k] for k in ("u_scale", "sample_null_action", "noise_abs_cost", "rollout_samples", "rollout_var_cost",
+                               "rollout_var_discount", "u_per_command") if k in case}
+    kw.update({k: torch.tensor(case[k], dtype=bd if k in ("u_min", "u_max") else dt)
+               for k in ("noise_mu", "u_init", "u_min", "u_max") if case.get(k) is not None})
+    kw["noise_sigma"] = torch.tensor(case["noise_sigma"], dtype=dt)
+    if prob.terminal_state_cost is not None:
+        kw["terminal_state_cost"] = prob.terminal_state_cost
+    if case.get("sampler") is not None:
+        kw["specific_actions"] = lambda state: sampler_actions(case, state)
+    if case["model"]["kind"] == "pendulum":
+        return (*_pendulum_plugins(), kw)
+    return prob.dynamics, prob.running_cost, kw
+
+
+BASE = Family("base", dict(CASES, **BATCHED_CASES), _base_model, _base_reference, _base_fixture)

@@ -1,22 +1,15 @@
 """Golden cases of rollout_samples M > 1 with copies that differ (reference mppi.py:334-373): the models of
 tests/ensemble_models.py under MPPI, SMPPI and KMPPI.  Fixtures tests/golden/ens_*.npz, produced by the live reference
-(tests/golden/make_golden_ensemble.py); kept apart from cases.CASES so that the tests parametrised over those do not see
-them.  The step-dependent case hands the oracle its callables through step_cases.HorizonClock: an M-copy rollout also
-calls dynamics, then the running cost, once per horizon step.
-
-The oracle's `mppi_command` rolls out through `rollout`, which dispatches on M (mppi.py:292-295), but its `smppi_command`
-and `kmppi_command` call the one-copy `rollout_costs` by name, while the reference's SMPPI and KMPPI dispatch on M too
-(mppi.py:564, inherited `_compute_rollout_costs`).  `EnsembleOracleRunner` therefore binds that name to
-`rollout_costs_multi` for the duration of each command (`multi_copy_rollouts`); the oracle itself is unchanged."""
-import contextlib
+(tests/golden/make_golden.py); kept apart from cases.CASES so that the tests parametrised over those do not see them.
+The step-dependent case hands the oracle its callables through step_cases.HorizonClock: an M-copy rollout also calls
+dynamics, then the running cost, once per horizon step."""
 import functools
 
 import torch
 
 from oracle import mppi_oracle as orc
 from tests import ensemble_models as em
-from tests.golden.cases import _DT
-from tests.golden.replay import Stream
+from tests.golden.cases import _DT, Family
 from tests.golden.step_cases import HorizonClock
 
 ENSEMBLE_CASES = {
@@ -78,58 +71,23 @@ def ensemble_problem(case, dyn_params=None):
                        rollout_var_discount=case["var_discount"])
 
 
-@contextlib.contextmanager
-def multi_copy_rollouts():
-    """Inside: the oracle's `rollout_costs` is `rollout_costs_multi`, the rollout of an M > 1 command (see the module
-    docstring).  Only for problems with rollout_samples > 1."""
-    one_copy = orc.rollout_costs
-    orc.rollout_costs = orc.rollout_costs_multi
-    try:
-        yield
-    finally:
-        orc.rollout_costs = one_copy
-
-
 def plant_step(case, x, u):
     """The closed loop's simulated system: copy 0 (at t = 0)."""
     f, _, _ = callables(case)
     return f(x, u) if case["model"] == "pendulum" else f(x, u, 0)
 
 
-class EnsembleOracleRunner:
-    """Steps the oracle through an ensemble case on the fixture's injected draws."""
+def _model(case, fixture):
+    return ensemble_problem(case), functools.partial(plant_step, case)
 
-    def __init__(self, case, dyn_params=None):
-        self.case = case
-        self.prob = ensemble_problem(case, dyn_params)
-        dt = self.prob.dtype
-        self.stream = Stream(case, self.prob)
-        T = case["T"]
-        self.U = self.stream.U0.clone()
-        if case["variant"] == "smppi":
-            sm = case["smooth"]
-            self.U, self.A = torch.zeros(T, 1, dtype=dt), torch.zeros(T, 1, dtype=dt)
-            self.sp = orc.SmoothParams(w_action_seq_cost=sm["w"], delta_t=sm["delta_t"],
-                                       action_max=torch.tensor(sm["action_max"], dtype=dt))
-        if case["variant"] == "kmppi":
-            S, sig = case["kernel"]["S"], case["kernel"]["sigma"]
-            self.theta = torch.zeros(S, 1, dtype=dt)
-            self.W, self.Wshift = orc.kernel_matrices(T, S, lambda a, b: orc.rbf_kernel(a, b, sig), dt)
 
-    def step(self, x, z):
-        v = self.case["variant"]
-        if v == "mppi":
-            r = orc.mppi_command(self.prob, self.U, x, z)
-        elif v == "smppi":
-            with multi_copy_rollouts():
-                r = orc.smppi_command(self.prob, self.sp, self.U, self.A, x, z)
-            self.A = r["action_sequence"]
-        else:
-            with multi_copy_rollouts():
-                r = orc.kmppi_command(self.prob, self.U, self.theta, x, z, self.W, self.Wshift)
-            self.theta = r["theta"]
-        self.U = r["U"]
-        return r
+def _reference(case, prob, fixture):
+    dt = _DT[case["dtype"]]
+    f, c, term = callables(case)
+    return f, c, dict(noise_sigma=torch.tensor(case["noise_sigma"], dtype=dt), u_max=torch.tensor(case["u_max"], dtype=dt),
+                      terminal_state_cost=term, rollout_samples=case["M"], rollout_var_cost=case["var_cost"],
+                      rollout_var_discount=case["var_discount"],
+                      step_dependent_dynamics=case["model"] == "scenario_integrator")
 
-    def advance(self, x, action):
-        return plant_step(self.case, x.view(1, -1), (self.prob.u_scale * action).view(1, -1)).view(-1)
+
+ENSEMBLE = Family("ensemble", ENSEMBLE_CASES, _model, _reference, smooth_key="action_sequence", scalars=False)

@@ -1,18 +1,13 @@
 """Golden cases of an ensemble of learned pendulum networks (PendulumMLPEnsemble, rollout_samples = M networks, one per
 copy; reference mppi.py:334-373) under MPPI, SMPPI and KMPPI.  Fixtures tests/golden/mlpens_*.npz, produced by the live
-reference with the ensemble's torch twin (tests/golden/make_golden_mlp_ensemble.py); they store the networks' weights,
-so replaying them needs neither the reference nor the seeds' torch initialisation.
-
-The oracle is driven by ensemble_cases.EnsembleOracleRunner: the stream of injected draws and the SMPPI / KMPPI state it
-sets up depend only on the case's seed, sizes and controller settings, and its SMPPI / KMPPI commands already roll out
-through `rollout_costs_multi`.  `MLPEnsembleOracleRunner` only swaps in the twin's problem and plant."""
+reference with the ensemble's torch twin (tests/golden/make_golden.py); they store the networks' weights, so replaying
+them needs neither the reference nor the seeds' torch initialisation."""
 import numpy as np
 import torch
 
 from oracle import mppi_oracle as orc
 from pytorch_mppi_b200.models import PendulumMLP, PendulumMLPEnsemble
-from tests.golden.cases import _DT, make_mlp_net
-from tests.golden.ensemble_cases import EnsembleOracleRunner
+from tests.golden.cases import _DT, Family, make_mlp_net
 
 _BASE = dict(lambda_=1.0, noise_sigma=1.0, u_max=2.0, steps=3)
 MLP_ENSEMBLE_CASES = {
@@ -55,21 +50,24 @@ def twin(case, nets):
     return PendulumMLPEnsemble(nets, max_torque=case["u_max"])
 
 
-class MLPEnsembleOracleRunner(EnsembleOracleRunner):
-    """Steps the oracle through an ensemble-of-networks case: the problem's dynamics and running cost are the twin's
-    (M*K rows, block m through nets[m]), and the closed loop's simulated system is nets[0]."""
+def _model(case, fixture):
+    """The oracle's problem runs the twin (M*K rows, block m through network m); the closed loop's simulated system is
+    network 0."""
+    nets = load_nets(case, fixture)
+    ens, dt = twin(case, nets), _DT[case["dtype"]]
+    prob = orc.Problem(ens.dynamics, ens.running_cost, 2, torch.tensor(case["noise_sigma"], dtype=dt), K=case["K"],
+                       T=case["T"], lambda_=case["lambda_"], u_max=torch.tensor(case["u_max"], dtype=dt),
+                       rollout_samples=case["M"], rollout_var_cost=case["var_cost"],
+                       rollout_var_discount=case["var_discount"])
+    return prob, lambda x, u: PendulumMLP.net_step(nets[0], x, u, case["u_max"])
 
-    def __init__(self, case, nets):
-        super().__init__(dict(case, model="pendulum"))       # the stream and the SMPPI / KMPPI state
-        self.case, self.nets = case, nets
-        ens = twin(case, nets)
-        dt = _DT[case["dtype"]]
-        self.prob = orc.Problem(ens.dynamics, ens.running_cost, 2, torch.tensor(case["noise_sigma"], dtype=dt),
-                                K=case["K"], T=case["T"], lambda_=case["lambda_"],
-                                u_max=torch.tensor(case["u_max"], dtype=dt), rollout_samples=case["M"],
-                                rollout_var_cost=case["var_cost"], rollout_var_discount=case["var_discount"])
-        self.stream.prob = self.prob
 
-    def advance(self, x, action):
-        u = (self.prob.u_scale * action).view(1, -1)
-        return PendulumMLP.net_step(self.nets[0], x.view(1, -1), u, self.case["u_max"]).view(-1)
+def _reference(case, prob, fixture):
+    dt = _DT[case["dtype"]]
+    return prob.dynamics, prob.running_cost, dict(
+        noise_sigma=torch.tensor(case["noise_sigma"], dtype=dt), u_max=torch.tensor(case["u_max"], dtype=dt),
+        rollout_samples=case["M"], rollout_var_cost=case["var_cost"], rollout_var_discount=case["var_discount"])
+
+
+MLP_ENSEMBLE = Family("mlp_ensemble", MLP_ENSEMBLE_CASES, _model, _reference, lambda case: net_arrays(make_nets(case)),
+                      smooth_key="action_sequence", scalars=False)

@@ -1,8 +1,8 @@
 """Golden cases at the edges of the model envelope: the (nx, nu) = (1,1), (3,3) and (8,4) models of
 tests/shape_models.py under MPPI, SMPPI, KMPPI and MPPI_Batched.  Fixtures tests/golden/shape_*.npz, produced by the live
-reference (tests/golden/make_golden_shapes.py); kept apart from cases.CASES so that the tests parametrised over those do
-not see them.  `cases.build_problem` and `engine.make_model` know the model kind "shape", so the replay and engine
-helpers of the other golden cases serve these too.
+reference (tests/golden/make_golden.py); kept apart from cases.CASES so that the tests parametrised over those do not see
+them.  `cases.build_problem` and `engine.make_model` know the model kind "shape", so the family runs on the base family's
+hooks.
 
 What the cases reach that no other fixture does: a 4x4 covariance whose off-diagonal entries are all non-zero (the
 colouring and the Sigma^-1 action cost with a full Cholesky factor), R = T*nu not a multiple of the normals per Philox
@@ -11,6 +11,7 @@ edges."""
 import torch
 
 from tests import shape_models as shm
+from tests.golden import cases
 
 SIG3 = [[1.0, 0.3, -0.2], [0.3, 0.8, 0.25], [-0.2, 0.25, 0.9]]
 SIG4 = [[1.0, 0.3, -0.2, 0.1], [0.3, 0.8, 0.25, -0.15], [-0.2, 0.25, 0.9, 0.2], [0.1, -0.15, 0.2, 0.7]]
@@ -64,3 +65,6 @@ def engine_model(m):
 def sigma_is_full(case):
     s = torch.tensor(case["noise_sigma"])
     return s.dim() == 2 and bool((s - torch.diag(torch.diag(s)) != 0).sum() == s.numel() - s.shape[0])
+
+
+SHAPES = cases.Family("shapes", dict(SHAPE_CASES, **SHAPE_BATCHED_CASES), cases.BASE.model, cases.BASE.reference)

@@ -1,7 +1,7 @@
 """Golden cases of step-dependent dynamics and cost (step_dependent_dynamics=True, reference mppi.py:147-157): the model
 of tests/step_models.py under MPPI, KMPPI and MPPI_Batched.  Fixtures tests/golden/stepint_*.npz, produced by the live
-reference (tests/golden/make_golden_step.py); kept apart from cases.CASES so that the tests parametrised over those do
-not see them.
+reference (tests/golden/make_golden.py); kept apart from cases.CASES so that the tests parametrised over those do not see
+them.
 
 The oracle (oracle/mppi_oracle.py) calls its plugins as `dynamics(state, u)` / `running_cost(state, u)`.  Its rollouts,
 like the reference's (mppi.py:312-319, 849-853), call dynamics and then running_cost exactly once per horizon step,
@@ -9,13 +9,11 @@ t = 0, ..., T-1, in order, once per command; `HorizonClock` relies on that order
 their t, and refuses any other call sequence."""
 import functools
 
-import numpy as np
 import torch
 
 from oracle import mppi_oracle as orc
 from tests import step_models as sm
-from tests.golden.cases import _DT, draw_z
-from tests.golden.replay import Stream
+from tests.golden.cases import _DT, Family
 
 STEPINT = {"kind": "step_integrator", "params": list(sm.SD_PARAMS), "terminal": True}
 STEP_CASES = {
@@ -69,55 +67,20 @@ def step_problem(case, dynamics=None, running_cost=None):
                        terminal_state_cost=term)
 
 
-def plant_step(case, x, u):
-    """The closed loop's simulated system: the model at t = 0, the horizon index of the step being applied."""
-    return sm.sd_dyn(x, u, 0, case["model"]["params"])
+def _model(case, fixture):
+    """The oracle's problem, and the closed loop's simulated system: the model at t = 0, the horizon index of the step
+    being applied."""
+    return step_problem(case), lambda x, u: sm.sd_dyn(x, u, 0, case["model"]["params"])
 
 
-class StepOracleRunner:
-    """Steps the oracle through an MPPI / KMPPI step case on the fixture's injected draws."""
-
-    def __init__(self, case, dynamics=None, running_cost=None):
-        self.case = case
-        self.prob = step_problem(case, dynamics, running_cost)
-        self.stream = Stream(case, self.prob)
-        self.U = self.stream.U0.clone()
-        if case["variant"] == "kmppi":
-            S, sig = case["kernel"]["S"], case["kernel"]["sigma"]
-            self.theta = torch.zeros(S, self.prob.nu, dtype=self.prob.dtype)
-            self.W, self.Wshift = orc.kernel_matrices(case["T"], S, lambda a, b: orc.rbf_kernel(a, b, sig), self.prob.dtype)
-
-    def step(self, x, z):
-        if self.case["variant"] == "kmppi":
-            r = orc.kmppi_command(self.prob, self.U, self.theta, x, z, self.W, self.Wshift)
-            self.theta = r["theta"]
-        else:
-            r = orc.mppi_command(self.prob, self.U, x, z)
-        self.U = r["U"]
-        return r
-
-    def advance(self, x, action):
-        return plant_step(self.case, x.view(1, -1), (self.prob.u_scale * action).view(1, -1)).view(-1)
+def _reference(case, prob, fixture):
+    f, c, term = callables(case)
+    dt = _DT[case["dtype"]]
+    kw = dict(noise_sigma=torch.tensor(case["noise_sigma"], dtype=dt), u_max=torch.tensor(case["u_max"], dtype=dt),
+              step_dependent_dynamics=True)
+    if term is not None:
+        kw["terminal_state_cost"] = term
+    return f, c, kw
 
 
-class StepBatchedOracleRunner:
-    """MPPI_Batched step case: shared (K,T,nu) draws, (N,T,nu) nominal, (N,nx) states."""
-
-    def __init__(self, case):
-        self.case = case
-        self.prob = step_problem(case)
-        self.gen = np.random.Generator(np.random.Philox(key=case["seed"]))
-        self.U0 = torch.from_numpy(self.gen.standard_normal((case["N"], case["T"], 1), dtype=np.float32)).to(self.prob.dtype)
-        self.U = self.U0.clone()
-
-    def next_z(self):
-        c = self.case
-        return draw_z(self.gen, (c["K"], c["T"], 1), self.prob.dtype, c.get("z_dtype"))
-
-    def step(self, x, z):
-        r = orc.mppi_batched_command(self.prob, self.U, x, z)
-        self.U = r["U"]
-        return r
-
-    def advance(self, x, action):
-        return plant_step(self.case, x, self.prob.u_scale * action)
+STEP = Family("step", dict(STEP_CASES, **STEP_BATCHED_CASES), _model, _reference)

@@ -1,6 +1,6 @@
 """Golden cases of a model that reads device tensors (tests/tensor_models.py: bilinear costmap lookup + a reference path
 indexed by the horizon step) under MPPI and KMPPI.  Fixtures tests/golden/tens_*.npz, produced by the live reference with
-the torch twins (tests/golden/make_golden_tensors.py); each holds the costmap and the path it was made with."""
+the torch twins (tests/golden/make_golden.py); each holds the costmap and the path it was made with."""
 import functools
 
 import numpy as np
@@ -8,8 +8,7 @@ import torch
 
 from oracle import mppi_oracle as orc
 from tests import tensor_models as tm
-from tests.golden.cases import _DT
-from tests.golden.replay import Stream
+from tests.golden.cases import _DT, Family
 from tests.golden.step_cases import HorizonClock
 
 TENSOR_CASES = {
@@ -32,39 +31,33 @@ def callables(costmap, path, params=tm.NAV_PARAMS):
             lambda s, a, t: tm.nav_cost(s, a, t, params, costmap, path))
 
 
-class TensorOracleRunner:
-    """Steps the oracle through a tensor case on the fixture's injected draws."""
+def _fixture(case):
+    costmap, path = case_tensors(case)
+    return {"costmap": costmap.numpy(), "path": path.numpy()}
 
-    def __init__(self, case, costmap, path):
-        self.case = case
-        dt = _DT[case["dtype"]]
-        f, c = callables(costmap, path)
-        self.f = f
-        clock = HorizonClock(f, c, case["T"])
-        self.prob = orc.Problem(clock.dynamics, clock.running_cost, 2, case["noise_sigma"] * torch.eye(2, dtype=dt),
-                                K=case["K"], T=case["T"], lambda_=case["lambda_"],
-                                u_max=torch.full((2,), case["u_max"], dtype=dt))
-        self.stream = Stream(case, self.prob)
-        self.U = self.stream.U0.clone()
-        if case["variant"] == "kmppi":
-            S, sig = case["kernel"]["S"], case["kernel"]["sigma"]
-            self.theta = torch.zeros(S, 2, dtype=dt)
-            self.W, self.Wshift = orc.kernel_matrices(case["T"], S, lambda a, b: orc.rbf_kernel(a, b, sig), dt)
 
-    def step(self, x, z):
-        if self.case["variant"] == "kmppi":
-            r = orc.kmppi_command(self.prob, self.U, self.theta, x, z, self.W, self.Wshift)
-            self.theta = r["theta"]
-        else:
-            r = orc.mppi_command(self.prob, self.U, x, z)
-        self.U = r["U"]
-        return r
+def _model(case, fixture):
+    """The oracle's problem on the fixture's costmap and path; the closed loop's simulated system is the dynamics at
+    t = 0."""
+    dt = _DT[case["dtype"]]
+    f, c = callables(*fixture_tensors(fixture, "cpu"))
+    clock = HorizonClock(f, c, case["T"])
+    prob = orc.Problem(clock.dynamics, clock.running_cost, 2, case["noise_sigma"] * torch.eye(2, dtype=dt),
+                       K=case["K"], T=case["T"], lambda_=case["lambda_"], u_max=torch.full((2,), case["u_max"], dtype=dt))
+    return prob, lambda x, u: f(x, u, 0)
 
-    def advance(self, x, action):
-        return self.f(x.view(1, -1), action.view(1, -1), 0).view(-1)
+
+def _reference(case, prob, fixture):
+    dt = _DT[case["dtype"]]
+    return (*callables(*fixture_tensors(fixture, "cpu")),
+            dict(noise_sigma=case["noise_sigma"] * torch.eye(2, dtype=dt), u_max=torch.full((2,), case["u_max"], dtype=dt),
+                 step_dependent_dynamics=True))
 
 
 def fixture_tensors(gold, device):
     """The costmap and path a fixture was made with, on `device`."""
     return (torch.from_numpy(np.asarray(gold["costmap"])).to(device).contiguous(),
             torch.from_numpy(np.asarray(gold["path"])).to(device).contiguous())
+
+
+TENSORS = Family("tensors", TENSOR_CASES, _model, _reference, _fixture, scalars=False)

@@ -1,6 +1,6 @@
 """CPU: user models whose rollout copies differ (CudaModel(copies=M), rollout_samples=M) — generated header, NVRTC
-compilation, the route rule, the controller setters, the oracle against the live-reference fixtures, and the C entry
-points' argument checks.  No GPU."""
+compilation, the route rule, the controller setters, what the live-reference fixtures detect, and the C entry points'
+argument checks.  No GPU."""
 import ctypes as C
 
 import numpy as np
@@ -12,10 +12,8 @@ from pytorch_mppi_b200 import _cabi, build
 from pytorch_mppi_b200.mppi import SpecificActionSampler, fused_route_model
 from tests import ensemble_models as em
 from tests import user_models
-from tests.golden.ensemble_cases import ENSEMBLE_CASES, EnsembleOracleRunner, shifted_params
-from tests.golden.replay import load
-
-TOL = {"f64": 1e-11, "f32": 2e-5}        # tests/test_oracle_golden.py
+from tests.golden.ensemble_cases import ENSEMBLE, ENSEMBLE_CASES, ensemble_problem, shifted_params
+from tests.golden.replay import OracleRunner, load
 
 
 def test_copies_header():
@@ -90,32 +88,12 @@ def test_rollout_var_setters_mark_the_constants_dirty():
 
 
 @pytest.mark.parametrize("name", sorted(ENSEMBLE_CASES))
-def test_oracle_matches_reference_golden_ensemble(name):
-    torch.set_num_threads(1)
-    case, gold = load(name)
-    assert case == ENSEMBLE_CASES[name], "fixture is stale: re-run tests/golden/make_golden_ensemble.py"
-    run = EnsembleOracleRunner(case)
-    tol = TOL[case["dtype"]]
-    np.testing.assert_array_equal(run.stream.U0.numpy(), gold["U0"])
-    x = torch.tensor(case["x0"], dtype=run.prob.dtype)
-    for step in range(case["steps"]):
-        z = run.stream.next_z()
-        assert abs(float(z.double().sum()) - float(gold["z_sums"][step])) < 1e-6
-        np.testing.assert_allclose(x.numpy(), gold[f"x_{step}"], atol=tol, rtol=0)
-        r = run.step(x, z)
-        np.testing.assert_allclose(r["U"].numpy(), gold[f"U_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["action"].numpy(), gold[f"action_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["cost_total"].numpy(), gold[f"cost_total_{step}"], rtol=50 * tol, atol=0)
-        x = run.advance(x, r["action"])
-
-
-@pytest.mark.parametrize("name", sorted(ENSEMBLE_CASES))
 def test_fixture_detects_a_copy_index_off_by_one(name):
     """Every fixture's copies differ enough that dynamics reading copy m+1's parameters for copy m miss it by orders of
     magnitude more than any tolerance the engine or the oracle is held to (<= 2e-5)."""
     torch.set_num_threads(1)
     case, gold = load(name)
-    run = EnsembleOracleRunner(case, shifted_params(case, 1))
+    run = OracleRunner(case, family=ENSEMBLE, prob=ensemble_problem(case, shifted_params(case, 1)))
     r = run.step(torch.tensor(case["x0"], dtype=run.prob.dtype), run.stream.next_z())
     assert float(np.abs(r["cost_total"].numpy() - gold["cost_total_0"]).max()) > 1e-3
     assert float(np.abs(r["U"].numpy() - gold["U_0"]).max()) > 2e-4

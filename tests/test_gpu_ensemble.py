@@ -12,7 +12,8 @@ import torch
 import pytorch_mppi_b200 as eng
 from pytorch_mppi_b200 import _cabi
 from tests import ensemble_models as em
-from tests.golden.ensemble_cases import ENSEMBLE_CASES, EnsembleOracleRunner, case_params
+from tests.golden.engine import replay
+from tests.golden.ensemble_cases import ENSEMBLE, ENSEMBLE_CASES, case_params
 from tests.golden.replay import OracleRunner, load
 
 pytestmark = pytest.mark.gpu
@@ -57,22 +58,13 @@ def _ctrl(case, m, stepped=False, **kw):
 @pytest.mark.parametrize("name", sorted(ENSEMBLE_CASES))
 def test_fused_matches_reference_golden(name):
     case, gold = load(name)
-    run = EnsembleOracleRunner(case)
+    run = OracleRunner(case, family=ENSEMBLE)
     m = _model(case)
     kw = {} if case["variant"] == "smppi" else dict(U_init=run.stream.U0.clone())
     c = _ctrl(case, m, **kw)
     tol = TOL[run.prob.dtype]
-    for step in range(case["steps"]):
-        c.inject_noise(run.stream.next_z())
-        a = c.command(torch.from_numpy(gold[f"x_{step}"]))
-        assert float(np.abs(c.U.cpu().numpy() - gold[f"U_{step}"]).max()) <= tol, step
-        assert float(np.abs(a.cpu().numpy() - gold[f"action_{step}"]).max()) <= tol, step
-        ct = gold[f"cost_total_{step}"]
-        assert float(np.abs(c.cost_total.cpu().numpy() - ct).max()) <= tol * max(1.0, float(np.abs(ct).max())), step
-        if case["variant"] == "kmppi":
-            assert float(np.abs(c.theta.cpu().numpy() - gold[f"theta_{step}"]).max()) <= tol
-        if case["variant"] == "smppi":
-            assert float(np.abs(c.action_sequence.cpu().numpy() - gold[f"action_sequence_{step}"]).max()) <= tol
+    replay(c, run, gold, tol, lambda got, want: np.testing.assert_allclose(got, want, rtol=0,
+                                                                          atol=tol * max(1.0, float(np.abs(want).max()))))
     assert c.launch_info.split_cost == 0
 
 
@@ -130,12 +122,7 @@ def test_copy_offset_fixtures_replay_on_the_fused_route(name):
                  rollout_samples=case["rollout_samples"], rollout_var_cost=case["rollout_var_cost"],
                  rollout_var_discount=case["rollout_var_discount"])
     assert c._model is m
-    tol = TOL[dt]
-    for step in range(case["steps"]):
-        c.inject_noise(run.stream.next_z())
-        a = c.command(torch.from_numpy(gold[f"x_{step}"]))
-        assert float(np.abs(c.U.cpu().numpy() - gold[f"U_{step}"]).max()) <= tol, step
-        assert float(np.abs(a.cpu().numpy() - gold[f"action_{step}"]).max()) <= tol, step
+    replay(c, run, gold, TOL[dt])
 
 
 def test_set_params_between_commands_matches_a_controller_built_with_them():

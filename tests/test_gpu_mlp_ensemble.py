@@ -11,8 +11,9 @@ import torch
 import pytorch_mppi_b200 as eng
 from pytorch_mppi_b200 import _cabi
 from tests.golden.cases import make_mlp_net
-from tests.golden.mlp_ensemble_cases import MLP_ENSEMBLE_CASES, MLPEnsembleOracleRunner, load_nets
-from tests.golden.replay import load
+from tests.golden.engine import replay
+from tests.golden.mlp_ensemble_cases import MLP_ENSEMBLE, MLP_ENSEMBLE_CASES, load_nets
+from tests.golden.replay import OracleRunner, load
 
 pytestmark = pytest.mark.gpu
 
@@ -73,25 +74,13 @@ def _routes():
 @pytest.mark.parametrize("name,tc", _routes())
 def test_fused_matches_reference_golden(name, tc):
     case, gold = load(name)
+    run = OracleRunner(case, gold, MLP_ENSEMBLE)
     nets = [n.cuda() for n in load_nets(case, gold)]
-    run = MLPEnsembleOracleRunner(case, nets)
     ens = eng.PendulumMLPEnsemble(nets, max_torque=case["u_max"], tensor_cores=tc)
     c = _ctrl(case, ens, **({} if case["variant"] == "smppi" else dict(U_init=run.stream.U0.clone())))
     tol = FIXTURE_TOL.get((name, tc), TOL[(case["dtype"], tc)])
-    for step in range(case["steps"]):
-        c.inject_noise(run.stream.next_z())
-        a = c.command(torch.from_numpy(gold[f"x_{step}"]))
-        assert float(np.abs(c.U.cpu().numpy() - gold[f"U_{step}"]).max()) <= tol, step
-        assert float(np.abs(a.cpu().numpy() - gold[f"action_{step}"]).max()) <= tol, step
-        _assert_costs_close(c.cost_total.cpu().numpy(), gold[f"cost_total_{step}"], tol, run.prob.dtype)
-        if case["variant"] == "kmppi":
-            assert float(np.abs(c.theta.cpu().numpy() - gold[f"theta_{step}"]).max()) <= tol
-            c.theta = torch.from_numpy(gold[f"theta_{step}"])
-        if case["variant"] == "smppi":
-            assert float(np.abs(c.action_sequence.cpu().numpy() - gold[f"action_sequence_{step}"]).max()) <= tol
-            c.action_sequence = torch.from_numpy(gold[f"action_sequence_{step}"])
-        # the nominal in lock-step with the reference's, as tests/test_gpu_parity.py: per-step errors do not compound
-        c.U = torch.from_numpy(gold[f"U_{step}"])
+    # the nominal in lock-step with the reference's, as tests/test_gpu_parity.py: per-step errors do not compound
+    replay(c, run, gold, tol, lambda got, want: _assert_costs_close(got, want, tol, run.prob.dtype), reset_nominal=True)
     assert c.launch_info.split_cost == 0
 
 

@@ -11,9 +11,10 @@ import torch
 import pytorch_mppi_b200 as eng
 from oracle import mppi_oracle as orc
 from tests import tensor_models as tm
-from tests.golden.replay import load
+from tests.golden.engine import replay
+from tests.golden.replay import OracleRunner, load
 from tests.golden.step_cases import HorizonClock
-from tests.golden.tensor_cases import TENSOR_CASES, TensorOracleRunner, fixture_tensors
+from tests.golden.tensor_cases import TENSOR_CASES, TENSORS, fixture_tensors
 
 pytestmark = pytest.mark.gpu
 
@@ -125,21 +126,16 @@ def test_fused_matches_reference_golden(name):
     assert case == TENSOR_CASES[name]
     costmap, path = fixture_tensors(gold, "cuda")
     m = tm.nav_model(costmap, path)
-    run = TensorOracleRunner(case, costmap.cpu(), path.cpu())
+    run = OracleRunner(case, gold, TENSORS)
     dt = run.prob.dtype
-    tol = 1e-9 if case["dtype"] == "f64" else 1e-5
     kw = dict(lambda_=case["lambda_"])
     if case["variant"] == "kmppi":
         kw.update(num_support_pts=case["kernel"]["S"], kernel=eng.RBFKernel(sigma=case["kernel"]["sigma"]))
     cls = eng.KMPPI if case["variant"] == "kmppi" else eng.MPPI
     c = _ctrl(cls, m, case["K"], case["T"], dt, run.stream.U0.clone(), **kw)
-    for step in range(case["steps"]):
-        c.inject_noise(run.stream.next_z())
-        a = c.command(torch.from_numpy(gold[f"x_{step}"]))
-        assert float(np.abs(c.U.cpu().numpy() - gold[f"U_{step}"]).max()) <= tol, step
-        assert float(np.abs(a.cpu().numpy() - gold[f"action_{step}"]).max()) <= tol
-        ctol = 1e-10 if case["dtype"] == "f64" else 5e-6        # tests/test_gpu_parity.py
-        np.testing.assert_allclose(c.cost_total.cpu().numpy(), gold[f"cost_total_{step}"], rtol=ctol, atol=ctol)
+    ctol = 1e-10 if case["dtype"] == "f64" else 5e-6        # tests/test_gpu_parity.py
+    replay(c, run, gold, 1e-9 if case["dtype"] == "f64" else 1e-5,
+           lambda got, want: np.testing.assert_allclose(got, want, rtol=ctol, atol=ctol))
 
 
 def _single(m, T):

@@ -14,7 +14,7 @@ import pytest
 import torch
 
 from tests.golden.cases import BATCHED_CASES, CASES
-from tests.golden.replay import OracleRunner, load
+from tests.golden.replay import BatchedOracleRunner, OracleRunner, load
 
 pytestmark = pytest.mark.gpu
 
@@ -37,67 +37,20 @@ def _record(key, err):
 
 
 def _run(name, route, check_oracle=True, model_kw=None, tol=None, cost_atol=None):
-    from tests.golden.engine import make_engine
+    from tests.golden.engine import make_engine, replay
     torch.set_num_threads(1)
     case, gold = load(name)
     run = OracleRunner(case, gold)
     tol = tol if tol is not None else U_TOL_OVERRIDE.get(name, U_TOL[case["dtype"]])
     ctrl = make_engine(case, run.stream.U0, route=route, gold=gold, model_kw=model_kw)
     assert (ctrl._model is not None) == (route == "fused")
-    x = torch.tensor(case["x0"], dtype=run.prob.dtype)
-    worst = 0.0
-    for step in range(case["steps"]):
-        z = run.stream.next_z()
-        ctrl.inject_noise(z)
-        # the engine sees the golden state sequence, so per-step errors do not compound through x
-        xg = torch.from_numpy(gold[f"x_{step}"]).to(run.prob.dtype)
-        a = ctrl.command(xg.numpy())
-        U = ctrl.U.detach().cpu()
-        err = float(np.abs(U.numpy() - gold[f"U_{step}"]).max())
-        worst = max(worst, err)
-        _record(f"{name}/{route}" + (f"/{model_kw}" if model_kw else ""), err)
-        assert err <= tol, f"{name}/{route} step {step}: |U - U_ref| = {err:.3e} > {tol}"
-        aerr = float(np.abs(a.detach().cpu().numpy() - gold[f"action_{step}"]).max())
-        assert aerr <= tol, f"{name}/{route} step {step}: action error {aerr:.3e}"
-        if case["variant"] == "smppi":
-            A = ctrl.action_sequence.detach().cpu().numpy()
-            assert np.abs(A - gold[f"A_{step}"]).max() <= tol
-        if case["variant"] == "kmppi":
-            th = ctrl.theta.detach().cpu().numpy()
-            assert np.abs(th - gold[f"theta_{step}"]).max() <= tol
-        if f"cost_total_{step}" in gold:
-            c = ctrl.cost_total.detach().cpu().numpy()
-            rtol = 1e-10 if case["dtype"] == "f64" else (5e-6 if model_kw is None and case["model"]["kind"] != "pendulum_mlp" else 2e-3)
-            _record(f"{name}/{route}/cost_abs", np.abs(c - gold[f"cost_total_{step}"]).max())
-            np.testing.assert_allclose(c, gold[f"cost_total_{step}"], rtol=rtol, atol=rtol if cost_atol is None else cost_atol)
-        if check_oracle and case["K"] <= 2048:
-            r = run.step(xg, z)
-            om = ctrl.omega.detach().cpu().numpy()
-            otol = 1e-9 if case["dtype"] == "f64" else 2e-5
-            np.testing.assert_allclose(om, r["omega"].numpy(), atol=otol, rtol=0)
-            assert abs(om.sum() - 1.0) < 1e-5                                    # test_mppi.py:269-274
-            np.testing.assert_allclose(ctrl.noise.cpu().numpy(), r["noise"].numpy(), atol=otol, rtol=0)
-            np.testing.assert_allclose(ctrl.perturbed_action.cpu().numpy(), r["perturbed_action"].numpy(), atol=otol, rtol=0)
-            if f"pa_head_{step}" in gold:                     # null action + SpecificActionSampler rows (mppi.py:387-400)
-                n = gold[f"pa_head_{step}"].shape[0]
-                np.testing.assert_allclose(ctrl.perturbed_action[:n].cpu().numpy(), gold[f"pa_head_{step}"], atol=otol, rtol=0)
-                i0 = 1 if case.get("sample_null_action") else 0
-                smp = ctrl.specific_action_sampler
-                assert (smp.start_idx, smp.end_idx) == (i0, i0 + case["sampler"]["n"])
-            if r["states"] is not None and ctrl.states is not None:
-                assert ctrl.states.shape == r["states"].shape
-                np.testing.assert_allclose(ctrl.states.cpu().numpy(), r["states"].numpy(), atol=max(otol, 1e-5 if case["dtype"] == "f32" else 0), rtol=0)
-        # keep the engine's nominal in lock-step with the reference trajectory
-        ctrl.U = torch.from_numpy(gold[f"U_{step}"])
-        if case["variant"] == "smppi":
-            ctrl.action_sequence = torch.from_numpy(gold[f"A_{step}"])
-        if case["variant"] == "kmppi":
-            ctrl.theta = torch.from_numpy(gold[f"theta_{step}"])
-            run.theta = torch.from_numpy(gold[f"theta_{step}"]).clone()
-        run.U = torch.from_numpy(gold[f"U_{step}"]).clone()
-        if case["variant"] == "smppi":
-            run.A = torch.from_numpy(gold[f"A_{step}"]).clone()
-    return worst
+    rtol = 1e-10 if case["dtype"] == "f64" else (5e-6 if model_kw is None and case["model"]["kind"] != "pendulum_mlp" else 2e-3)
+
+    def cost(c, want):
+        _record(f"{name}/{route}/cost_abs", np.abs(c - want).max())
+        np.testing.assert_allclose(c, want, rtol=rtol, atol=rtol if cost_atol is None else cost_atol)
+    return replay(ctrl, run, gold, tol, cost, reset_nominal=True, lock_step=check_oracle and case["K"] <= 2048,
+                  record=lambda err: _record(f"{name}/{route}" + (f"/{model_kw}" if model_kw else ""), err))
 
 
 def _routes(name):
@@ -130,28 +83,15 @@ def test_tensor_core_mlp_matches_reference_golden(mode, fast, tol):
 @pytest.mark.parametrize("route", ["fused", "stepped"])
 def test_mppi_batched_matches_reference_golden(name, route):
     """MPPI_Batched against fixtures produced by the live `ref.MPPI_Batched` (mppi.py:822-873)."""
-    from tests.golden.engine import make_batched_engine
-    from tests.golden.replay import BatchedOracleRunner
+    from tests.golden.engine import make_batched_engine, replay
     torch.set_num_threads(1)
     case, gold = load(name)
     run = BatchedOracleRunner(case)
-    tol = U_TOL[case["dtype"]]
-    ctrl = make_batched_engine(case, run.U0, route=route)
+    ctrl = make_batched_engine(case, run.stream.U0, route=route)
     assert (ctrl._model is not None) == (route == "fused")
-    for step in range(case["steps"]):
-        z = run.next_z()
-        ctrl.inject_noise(z)
-        xg = torch.from_numpy(gold[f"x_{step}"]).to(run.prob.dtype)
-        a = ctrl.command(xg.cuda())
-        err = float(np.abs(ctrl.U.cpu().numpy() - gold[f"U_{step}"]).max())
-        _record(f"{name}/{route}", err)
-        assert err <= tol, f"{name}/{route} step {step}: |U - U_ref| = {err:.3e} > {tol}"
-        assert a.shape == gold[f"action_{step}"].shape
-        assert float(np.abs(a.cpu().numpy() - gold[f"action_{step}"]).max()) <= tol
-        rtol = 1e-10 if case["dtype"] == "f64" else 5e-6
-        np.testing.assert_allclose(ctrl.cost_total.cpu().numpy(), gold[f"cost_total_{step}"], rtol=rtol, atol=rtol)
-        np.testing.assert_allclose(ctrl.omega.cpu().numpy(), gold[f"omega_{step}"], atol=1e-9 if case["dtype"] == "f64" else 2e-5, rtol=0)
-        ctrl.U = torch.from_numpy(gold[f"U_{step}"])
+    rtol = 1e-10 if case["dtype"] == "f64" else 5e-6
+    replay(ctrl, run, gold, U_TOL[case["dtype"]], lambda c, want: np.testing.assert_allclose(c, want, rtol=rtol, atol=rtol),
+           reset_nominal=True, record=lambda err: _record(f"{name}/{route}", err))
 
 
 @pytest.mark.parametrize("name", sorted(n for n in CASES if "fused" in _routes(n) and CASES[n]["model"]["kind"] != "pendulum_mlp"))

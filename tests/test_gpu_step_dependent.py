@@ -161,33 +161,30 @@ def test_get_rollouts_equals_torch_loop():
 
 
 def test_mppi_batched_matches_reference_golden():
-    from tests.golden.replay import load
-    from tests.golden.step_cases import StepBatchedOracleRunner
+    from tests.golden.engine import replay
+    from tests.golden.replay import BatchedOracleRunner, load
+    from tests.golden.step_cases import STEP
     case, gold = load("stepint_batched_f64")
-    run = StepBatchedOracleRunner(case)
+    run = BatchedOracleRunner(case, family=STEP)
     m = um.step_dependent_user_model(case["model"]["params"], terminal=False)
     dt = torch.float64
     c = eng.MPPI_Batched(m.dynamics, m.running_cost, 2, torch.tensor(case["noise_sigma"], dtype=dt), case["N"],
                          num_samples=case["K"], horizon=case["T"], lambda_=case["lambda_"], u_max=torch.tensor(case["u_max"], dtype=dt),
                          step_dependent_dynamics=True, device="cuda")
     assert c._model is m
-    c.U = run.U0.clone()
-    for step in range(case["steps"]):
-        c.inject_noise(run.next_z())
-        a = c.command(torch.from_numpy(gold[f"x_{step}"]))
-        assert float(np.abs(c.U.cpu().numpy() - gold[f"U_{step}"]).max()) <= 1e-9
-        assert float(np.abs(a.cpu().numpy() - gold[f"action_{step}"]).max()) <= 1e-9
-        np.testing.assert_allclose(c.cost_total.cpu().numpy(), gold[f"cost_total_{step}"], rtol=1e-10, atol=1e-10)
+    c.U = run.stream.U0.clone()
+    replay(c, run, gold, 1e-9, lambda got, want: np.testing.assert_allclose(got, want, rtol=1e-10, atol=1e-10))
 
 
 # stepint_kmppi_f32: the force sin(0.7 t) is CUDA's sinf in the kernel and numpy's float32 sin in the reference (1-ulp
 # differences, as the pendulum's sin: tests/test_gpu_parity.py U_TOL_OVERRIDE); measured 1.2e-5 on H100, bound 2e-5
 @pytest.mark.parametrize("name,tol", [("stepint_mppi_f64", 1e-9), ("stepint_kmppi_f32", 2e-5)])
 def test_fused_matches_reference_golden(name, tol):
-    from tests.golden.replay import load
-    from tests.golden.step_cases import StepOracleRunner
+    from tests.golden.engine import replay
+    from tests.golden.replay import OracleRunner, load
+    from tests.golden.step_cases import STEP
     case, gold = load(name)
-    run = StepOracleRunner(case)
+    run = OracleRunner(case, family=STEP)
     dt = run.prob.dtype
     m = um.step_dependent_user_model(case["model"]["params"])
     kw = dict(lambda_=case["lambda_"])
@@ -198,13 +195,7 @@ def test_fused_matches_reference_golden(name, tol):
             horizon=case["T"], U_init=run.stream.U0.clone(), u_max=torch.tensor(case["u_max"], dtype=dt),
             terminal_state_cost=m.terminal_cost, step_dependent_dynamics=True, device="cuda", **kw)
     assert c._model is m
-    for step in range(case["steps"]):
-        c.inject_noise(run.stream.next_z())
-        a = c.command(torch.from_numpy(gold[f"x_{step}"]))
-        assert float(np.abs(c.U.cpu().numpy() - gold[f"U_{step}"]).max()) <= tol, step
-        assert float(np.abs(a.cpu().numpy() - gold[f"action_{step}"]).max()) <= tol
-        if case["variant"] == "kmppi":
-            assert float(np.abs(c.theta.cpu().numpy() - gold[f"theta_{step}"]).max()) <= tol
+    replay(c, run, gold, tol)
 
 
 def test_set_params_takes_effect_at_the_next_command_without_a_new_plan():

@@ -1,6 +1,6 @@
 """CPU: ensembles of learned pendulum networks (PendulumMLPEnsemble, rollout_samples = M networks, one per copy) —
-constructor checks, the torch twin's block split, the route rule, the C ABI field and the plans' argument checks, and the
-oracle against the live-reference fixtures.  No GPU."""
+constructor checks, the torch twin's block split, the route rule, the C ABI field and the plans' argument checks, and what
+the live-reference fixtures detect.  No GPU."""
 import ctypes as C
 
 import numpy as np
@@ -11,10 +11,8 @@ import pytorch_mppi_b200 as eng
 from pytorch_mppi_b200 import _cabi, build
 from pytorch_mppi_b200.mppi import SpecificActionSampler, fused_route_model
 from tests.golden.cases import make_mlp_net
-from tests.golden.mlp_ensemble_cases import MLP_ENSEMBLE_CASES, MLPEnsembleOracleRunner, load_nets
-from tests.golden.replay import load
-
-TOL = {"f64": 1e-11, "f32": 2e-5}        # tests/test_oracle_golden.py
+from tests.golden.mlp_ensemble_cases import MLP_ENSEMBLE, MLP_ENSEMBLE_CASES, load_nets, net_arrays
+from tests.golden.replay import OracleRunner, load
 
 
 def _nets(M, dtype=torch.float64, seed=10):
@@ -119,29 +117,13 @@ def test_plans_check_the_ensemble_arguments_before_any_cuda_call():
         assert lib.mppi_plan_create(C.byref(p), C.byref(C.c_void_p())) == (-2 if model == _cabi.MODEL_PENDULUM else -1)
 
 
-@pytest.mark.parametrize("name", sorted(MLP_ENSEMBLE_CASES))
-def test_oracle_matches_reference_golden_mlp_ensemble(name):
-    torch.set_num_threads(1)
-    case, gold = load(name)
-    assert case == MLP_ENSEMBLE_CASES[name], "fixture is stale: re-run tests/golden/make_golden_mlp_ensemble.py"
-    run = MLPEnsembleOracleRunner(case, load_nets(case, gold))
-    tol = TOL[case["dtype"]]
-    np.testing.assert_array_equal(run.stream.U0.numpy(), gold["U0"])
-    x = torch.tensor(case["x0"], dtype=run.prob.dtype)
-    for step in range(case["steps"]):
-        z = run.stream.next_z()
-        assert abs(float(z.double().sum()) - float(gold["z_sums"][step])) < 1e-6
-        np.testing.assert_allclose(x.numpy(), gold[f"x_{step}"], atol=tol, rtol=0)
-        r = run.step(x, z)
-        np.testing.assert_allclose(r["U"].numpy(), gold[f"U_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["action"].numpy(), gold[f"action_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["cost_total"].numpy(), gold[f"cost_total_{step}"], rtol=50 * tol, atol=0)
-        x = run.advance(x, r["action"])
+def _replay(case, nets):
+    return OracleRunner(case, net_arrays(nets), MLP_ENSEMBLE)
 
 
 def _replay_error(case, gold, nets):
     """Largest deviation of U and cost_total from a fixture over its closed loop, replayed with these networks."""
-    run = MLPEnsembleOracleRunner(case, nets)
+    run = _replay(case, nets)
     x, du, dc = torch.tensor(case["x0"], dtype=run.prob.dtype), 0.0, 0.0
     for step in range(case["steps"]):
         r = run.step(x, run.stream.next_z())
@@ -162,7 +144,7 @@ def test_fixture_detects_permuted_networks(name):
     nets = load_nets(case, gold)
     du, dc = _replay_error(case, gold, nets[1:] + nets[:1])
     assert du > 5e-3 and dc > 1e-2, (du, dc)
-    run = MLPEnsembleOracleRunner(case, [nets[0]] * case["M"])
+    run = _replay(case, [nets[0]] * case["M"])
     r = run.step(torch.tensor(case["x0"], dtype=run.prob.dtype), run.stream.next_z())
     assert float(np.abs(r["cost_total"].numpy() - gold["cost_total_0"]).max()) > 1e-2
     assert float(np.abs(r["U"].numpy() - gold["U_0"]).max()) > 5e-3

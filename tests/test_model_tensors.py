@@ -1,7 +1,6 @@
 """CPU: user models that read device tensors (CudaModel(tensors=...)) — the generated header and its NVRTC compilation,
 the agreement between the views the library packs and the struct the header declares, every ValueError of the Python
-API, the ABI of the new fields and the C entry points' argument checks, and the oracle against the live-reference
-fixtures.  No GPU."""
+API, the ABI of the new fields and the C entry points' argument checks.  No GPU."""
 import ctypes as C
 import hashlib
 import os
@@ -15,8 +14,6 @@ import pytorch_mppi_b200 as eng
 from pytorch_mppi_b200 import _cabi, build
 from tests import tensor_models as tm
 from tests import user_models
-from tests.golden.replay import load
-from tests.golden.tensor_cases import TENSOR_CASES, TensorOracleRunner, case_tensors, fixture_tensors
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "pytorch_mppi_b200", "csrc")
@@ -190,28 +187,6 @@ def test_entry_points_refuse_bad_arguments_before_any_cuda_call(lib):
     p.n_model_tensors = 1
     assert lib.mppi_plan_create(C.byref(p), C.byref(C.c_void_p())) == -1
     assert lib.mppi_rollout_states(C.byref(p), 16, 16, 0, 1, 1, 16, None) == -1
-
-
-@pytest.mark.parametrize("name", sorted(TENSOR_CASES))
-def test_oracle_matches_reference_golden_tensors(name):
-    torch.set_num_threads(1)
-    case, gold = load(name)
-    assert case == TENSOR_CASES[name], "fixture is stale: re-run tests/golden/make_golden_tensors.py"
-    costmap, path = fixture_tensors(gold, "cpu")
-    want_map, want_path = case_tensors(case)
-    assert torch.equal(costmap, want_map) and torch.equal(path, want_path)
-    run = TensorOracleRunner(case, costmap, path)
-    tol = {"f64": 1e-11, "f32": 2e-5}[case["dtype"]]
-    x = torch.tensor(case["x0"], dtype=run.prob.dtype)
-    for step in range(case["steps"]):
-        z = run.stream.next_z()
-        assert abs(float(z.double().sum()) - float(gold["z_sums"][step])) < 1e-6
-        np.testing.assert_allclose(x.numpy(), gold[f"x_{step}"], atol=tol, rtol=0)
-        r = run.step(x, z)
-        np.testing.assert_allclose(r["U"].numpy(), gold[f"U_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["action"].numpy(), gold[f"action_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["cost_total"].numpy(), gold[f"cost_total_{step}"], rtol=50 * tol, atol=0)
-        x = run.advance(x, r["action"])
 
 
 def test_twin_clamps_lookups_to_the_border():

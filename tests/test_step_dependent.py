@@ -1,6 +1,6 @@
 """CPU: step-dependent user models (CudaModel(step_dependent=True), step_dependent_dynamics=True) — generated header,
-NVRTC compilation, the route rule, set_params, the oracle against the live-reference fixtures, and the C entry point's
-argument checks.  No GPU."""
+NVRTC compilation, the route rule, set_params, what the live-reference fixtures detect, and the C entry point's argument
+checks.  No GPU."""
 import ctypes as C
 import hashlib
 
@@ -13,11 +13,8 @@ from pytorch_mppi_b200 import _cabi, build
 from pytorch_mppi_b200.mppi import SpecificActionSampler, fused_route_model
 from tests import step_models as um
 from tests import user_models
-from tests.golden.replay import load
-from tests.golden.step_cases import (STEP_BATCHED_CASES, STEP_CASES, HorizonClock, StepBatchedOracleRunner,
-                                     StepOracleRunner)
-
-TOL = {"f64": 1e-11, "f32": 2e-5}        # tests/test_oracle_golden.py
+from tests.golden.replay import OracleRunner, load
+from tests.golden.step_cases import STEP, HorizonClock, step_problem
 
 
 def test_header_without_t_is_unchanged():
@@ -95,46 +92,6 @@ def test_set_params():
     assert torch.equal(m.running_cost(s, a, 0), um.sd_cost(s, a, 0, p2))    # the torch twins follow
 
 
-@pytest.mark.parametrize("name", sorted(STEP_CASES))
-def test_oracle_matches_reference_golden_step_dependent(name):
-    torch.set_num_threads(1)
-    case, gold = load(name)
-    assert case == STEP_CASES[name], "fixture is stale: re-run tests/golden/make_golden_step.py"
-    run = StepOracleRunner(case)
-    tol = TOL[case["dtype"]]
-    np.testing.assert_array_equal(run.stream.U0.numpy(), gold["U0"])
-    x = torch.tensor(case["x0"], dtype=run.prob.dtype)
-    for step in range(case["steps"]):
-        z = run.stream.next_z()
-        assert abs(float(z.double().sum()) - float(gold["z_sums"][step])) < 1e-6
-        np.testing.assert_allclose(x.numpy(), gold[f"x_{step}"], atol=tol, rtol=0)
-        r = run.step(x, z)
-        np.testing.assert_allclose(r["U"].numpy(), gold[f"U_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["action"].numpy(), gold[f"action_{step}"], atol=tol, rtol=0)
-        if f"cost_total_{step}" in gold:
-            np.testing.assert_allclose(r["cost_total"].numpy(), gold[f"cost_total_{step}"], rtol=50 * tol, atol=0)
-        if case["variant"] == "kmppi":
-            np.testing.assert_allclose(r["theta"].numpy(), gold[f"theta_{step}"], atol=tol, rtol=0)
-        x = run.advance(x, r["action"])
-
-
-@pytest.mark.parametrize("name", sorted(STEP_BATCHED_CASES))
-def test_oracle_matches_reference_golden_step_dependent_batched(name):
-    torch.set_num_threads(1)
-    case, gold = load(name)
-    assert case == STEP_BATCHED_CASES[name], "fixture is stale: re-run tests/golden/make_golden_step.py"
-    run = StepBatchedOracleRunner(case)
-    tol = TOL[case["dtype"]]
-    x = torch.tensor(case["x0"], dtype=run.prob.dtype)
-    for step in range(case["steps"]):
-        z = run.next_z()
-        np.testing.assert_allclose(x.numpy(), gold[f"x_{step}"], atol=tol, rtol=0)
-        r = run.step(x, z)
-        np.testing.assert_allclose(r["U"].numpy(), gold[f"U_{step}"], atol=tol, rtol=0)
-        np.testing.assert_allclose(r["cost_total"].numpy(), gold[f"cost_total_{step}"], rtol=50 * tol, atol=0)
-        x = run.advance(x, r["action"])
-
-
 @pytest.mark.parametrize("shift", [-1, 1])
 def test_fixture_detects_an_off_by_one_in_t(shift):
     """The golden model's t weight is large enough that evaluating it at t -+ 1 misses the fixture by orders of magnitude
@@ -144,7 +101,7 @@ def test_fixture_detects_an_off_by_one_in_t(shift):
     x0 = torch.tensor(case["x0"], dtype=torch.float64)
     for kw in (dict(running_cost=lambda s, a, t: um.sd_cost(s, a, t + shift, p)),
                dict(dynamics=lambda s, a, t: um.sd_dyn(s, a, t + shift, p))):
-        run = StepOracleRunner(case, **kw)
+        run = OracleRunner(case, family=STEP, prob=step_problem(case, **kw))
         r = run.step(x0, run.stream.next_z())
         assert float(np.abs(r["U"].numpy() - gold["U_0"]).max()) > 2e-4
 
