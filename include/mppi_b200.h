@@ -244,7 +244,7 @@ int mppi_b200_abi_version(void);
  * 2 offsetof(state), 3 offsetof(U), 4 offsetof(rank), 5 offsetof(partial_out), 6 sizeof(MppiLaunchInfo),
  * 7 offsetof(model_weights), 8 offsetof(model_tensors); and of MppiClosedLoop: 9 sizeof, 10 offsetof(states),
  * 11 offsetof(plant_params), 12 offsetof(plant_blocks); and of MppiEnvParams: 13 sizeof, 14 offsetof(chol),
- * 15 offsetof(model_params), 16 offsetof(scratch). */
+ * 15 offsetof(model_params), 16 offsetof(scratch); and of MppiPlantModel: 17 sizeof, 18 offsetof(model_tensors). */
 uint64_t mppi_abi_layout(int which);
 const char* mppi_status_string(int status);
 const char* mppi_last_cuda_error(void);
@@ -327,6 +327,32 @@ uint64_t mppi_plan_model_block_bytes(void* plan);
  * u_per_command != 1, sharded plans (world > 1 or EXPORT_PARTIAL), plans that record their noise (z_out) or draw it from a
  * device counter (offset_dev), a resident grid armed.  All checked before any CUDA call. */
 int mppi_plan_closed_loop(void* plan, const MppiClosedLoop* cl, void* stream);
+
+/* The plant of a closed loop named apart from the plan's model: the controller plans with its own model (a learned
+ * PENDULUM_MLP network, an ensemble, a simpler analytic model) while the episode follows this one.  Its nx and nu are the
+ * plan's; its kernels are the plan's dtype. */
+typedef struct MppiPlantModel {
+    uint32_t struct_size;                 /* sizeof(MppiPlantModel), ABI check                                    */
+    int32_t model;                        /* MPPI_MODEL_PENDULUM, _LINEAR_POINT or _USER                          */
+    const void* user_model;               /* MPPI_MODEL_USER: handle compiled for the plan's dtype, else NULL     */
+    const MppiTensorRef* model_tensors;   /* HOST array of the plant's own tensors (user models), or NULL         */
+    int32_t n_model_tensors, reserved;    /* reserved: 0                                                          */
+} MppiPlantModel;
+/* Bytes one packed parameter block of this plant takes in MppiClosedLoop.plant_blocks (a multiple of 16); plant NULL: the
+ * plan's model, as mppi_plan_model_block_bytes.  0 for arguments mppi_plan_closed_loop_plant refuses. */
+uint64_t mppi_plant_block_bytes(void* plan, const MppiPlantModel* plant);
+/* mppi_plan_closed_loop against `plant` (NULL: the plan's model, exactly mppi_plan_closed_loop): states row s + 1 = the
+ * plant's step of row s under u_scale * action, plus disturbance row s; costs row s = the plant's running cost.  With a
+ * plant, plant_params is required: n_plant rows of n_plant_params doubles in the plant's own layout, packed into
+ * plant_blocks (n_plant * mppi_plant_block_bytes bytes); a user plant reads its own tensors, and replays copy 0 of a model
+ * with copies.  The plan's model need not have a plant step, and per-environment model parameters of the plan
+ * (mppi_plan_set_env_params) stay the controller's.
+ * MPPI_ERR_ABI: struct_size of cl or plant.  MPPI_ERR_BAD_ARG: those of mppi_plan_closed_loop, an unknown model, a user
+ * model whose handle is NULL, not a handle or compiled for the other dtype, reserved != 0, plant nx / nu not the plan's,
+ * tensors the plant's signature refuses, plant_params NULL.  MPPI_ERR_UNSUPPORTED: a PENDULUM_MLP / _ENSEMBLE plant or a
+ * plant without a plant step (step-dependent user models), and those of mppi_plan_closed_loop but the plan's model's own
+ * plant step.  All checked before any CUDA call. */
+int mppi_plan_closed_loop_plant(void* plan, const MppiClosedLoop* cl, const MppiPlantModel* plant, void* stream);
 
 /* ---- Per-environment settings of a batched plan (n_env > 1) ---------------------------------------
  * Environment e of a batched plan may have its own temperature, noise covariance, noise mean and model parameters; the

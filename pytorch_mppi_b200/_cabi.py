@@ -169,6 +169,19 @@ class MppiClosedLoop(C.Structure):
     ]
 
 
+class MppiPlantModel(C.Structure):
+    """Mirror of `struct MppiPlantModel`: the plant of a closed loop, named apart from the plan's model
+    (mppi_plan_closed_loop_plant)."""
+    _fields_ = [
+        ("struct_size", C.c_uint32),
+        ("model", C.c_int32),
+        ("user_model", C.c_void_p),
+        ("model_tensors", C.c_void_p),
+        ("n_model_tensors", C.c_int32),
+        ("reserved", C.c_int32),
+    ]
+
+
 class MppiEnvParams(C.Structure):
     """Mirror of `struct MppiEnvParams`: per-environment settings of a batched plan (mppi_plan_set_env_params)."""
     _fields_ = [
@@ -205,6 +218,8 @@ SYMBOLS = [
     ("mppi_plan_set_model_tensors", C.c_int, [C.c_void_p, C.c_void_p, C.c_int32]),
     ("mppi_plan_model_block_bytes", C.c_uint64, [C.c_void_p]),
     ("mppi_plan_closed_loop", C.c_int, [C.c_void_p, C.POINTER(MppiClosedLoop), C.c_void_p]),
+    ("mppi_plant_block_bytes", C.c_uint64, [C.c_void_p, C.POINTER(MppiPlantModel)]),
+    ("mppi_plan_closed_loop_plant", C.c_int, [C.c_void_p, C.POINTER(MppiClosedLoop), C.POINTER(MppiPlantModel), C.c_void_p]),
     ("mppi_plan_env_scratch_bytes", C.c_uint64, [C.c_void_p]),
     ("mppi_plan_set_env_params", C.c_int, [C.c_void_p, C.POINTER(MppiEnvParams), C.c_void_p]),
     ("mppi_plan_env_horizon_bytes", C.c_uint64, [C.c_void_p]),

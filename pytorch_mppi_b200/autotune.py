@@ -434,7 +434,10 @@ class ClosedLoopEvaluation:
                   step-dependent), rollout_samples = 1, no terminal cost, u_per_command = 1, one GPU
     start_states  (S, nx) start states; every candidate runs one episode from each
     steps         control steps per episode
-    plant_params  None (the plant is the controller's model), (n_params,) or (S, n_params): the plant of each start
+    plant         None (the plant is the controller's model), or the system the episodes run on, as
+                  `run_closed_loop`'s plant (e.g. a nonlinear plant for a controller that plans with a linear model)
+    plant_params  None (the plant's current parameters), (n_params,) or (S, n_params) in the plant's layout: the plant
+                  of each start
     max_horizon   the longest horizon a candidate may have (default ctrl.T, at least ctrl.T)
 
     The batched controller takes K, dtype, bounds, u_init, u_scale, noise_abs_cost and tile_memory from `ctrl` and has
@@ -442,10 +445,16 @@ class ClosedLoopEvaluation:
     Every episode of a call starts from ctrl's nominal sequence as it was when this object was made (cut or extended
     with u_init to each candidate's horizon), and all candidates share the K draws of every command."""
 
-    def __init__(self, ctrl, start_states, steps, plant_params=None, max_horizon=None):
+    def __init__(self, ctrl, start_states, steps, plant=None, plant_params=None, max_horizon=None):
         why = self._refusal(ctrl)
         if why is not None:
             raise ValueError(f"ClosedLoopEvaluation: {why}")
+        if plant is not None:
+            try:
+                ctrl._check_plant(plant)
+            except ValueError as e:
+                raise ValueError(f"ClosedLoopEvaluation: {e}") from None
+        self.plant = plant
         if isinstance(steps, bool) or not isinstance(steps, int) or steps < 1:
             raise ValueError(f"ClosedLoopEvaluation: steps must be an integer >= 1, got {steps!r}")
         x0 = torch.as_tensor(start_states).to(ctrl.d, ctrl.dtype)
@@ -456,7 +465,7 @@ class ClosedLoopEvaluation:
             raise ValueError(f"ClosedLoopEvaluation: max_horizon={self.max_horizon} is below the controller's T={ctrl.T}")
         self.ctrl, self.steps, self.start_states = ctrl, steps, x0.contiguous()
         self.S = x0.shape[0]
-        m = ctrl._model
+        m = ctrl._model if plant is None else plant
         n_params = len(m.param_blob()) + len(m.param_blob_ext())
         self.plant_params = None
         if plant_params is not None:
@@ -524,7 +533,8 @@ class ClosedLoopEvaluation:
         plant = None
         if self.plant_params is not None:
             plant = self.plant_params if self.plant_params.dim() == 1 else self.plant_params.repeat(P, 1)
-        res = b.run_closed_loop(x0, self.steps, plant_params=plant)
+        kw = {} if self.plant is None else {"plant": self.plant}
+        res = b.run_closed_loop(x0, self.steps, plant_params=plant, **kw)
         costs = res.costs.sum(0).view(P, S)
         return costs, res.states.view(self.steps + 1, P, S, -1)
 

@@ -137,35 +137,78 @@ int plan_command(Plan* pl, const double* state, const void* state_dev, uint32_t 
     return plan_launch(pl, stream);
 }
 
-// ---- closed-loop episodes (mppi_plan_closed_loop) -------------------------------------------------------
+// ---- closed-loop episodes (mppi_plan_closed_loop, mppi_plan_closed_loop_plant) ------------------------------
 // one packed parameter block in the plant scratch: the model's block rounded up to 16 bytes (alignment of every block)
-inline uint64_t plant_block_bytes(const Plan* pl) { return ((uint64_t)pl->mk->param_bytes + 15) / 16 * 16; }
+inline uint64_t plant_block_bytes(const ModelKernels* mk) { return ((uint64_t)mk->param_bytes + 15) / 16 * 16; }
 
 // n rows of n_params doubles in the model's own layout (the first MPPI_MODEL_PARAM_DOUBLES are its model_params,
-// zero-padded, the rest its model_params_ext), packed with the model's loader into n blocks plant_block_bytes apart
-void pack_param_rows(const Plan* pl, const double* rows, int n, int n_params, unsigned char* dst) {
-    MppiFusedParams pp = pl->p;
-    const uint64_t bb = plant_block_bytes(pl);
+// zero-padded, the rest its model_params_ext), packed with the model's loader into n blocks plant_block_bytes apart;
+// everything else a block holds (a user model's tensor views, the ensemble's weight table) comes from `p`
+void pack_param_rows(const ModelKernels* mk, const MppiFusedParams* p, const double* rows, int n, int n_params, unsigned char* dst) {
+    MppiFusedParams pp = *p;
+    const uint64_t bb = plant_block_bytes(mk);
     for (int i = 0; i < n; ++i) {
         const double* row = rows + (size_t)i * n_params;
         for (int j = 0; j < MPPI_MODEL_PARAM_DOUBLES; ++j) pp.model_params[j] = j < n_params ? row[j] : 0.0;
         pp.model_params_ext = n_params > MPPI_MODEL_PARAM_DOUBLES ? row + MPPI_MODEL_PARAM_DOUBLES : nullptr;
         pp.n_model_params_ext = n_params > MPPI_MODEL_PARAM_DOUBLES ? n_params - MPPI_MODEL_PARAM_DOUBLES : 0;
-        load_model_params(pl->mk, &pp, dst + (size_t)i * bb);
+        load_model_params(mk, &pp, dst + (size_t)i * bb);
     }
 }
 
-// the reasons a closed loop is refused, before any CUDA call (MPPI_OK: none)
-int check_closed_loop(const Plan* pl, const MppiClosedLoop* cl) {
+// The plant of a closed loop: its kernels and the parameters its blocks are packed from.  Without a plant descriptor,
+// the plan's model and parameters; with one, the plan's parameters with the plant's model, handle and tensors in place
+// of the plan's (find_kernels then picks the plant's kernels of the plan's dtype).  No CUDA call.
+struct PlantOf {
+    const ModelKernels* mk;
+    MppiFusedParams p;
+};
+int resolve_plant(const Plan* pl, const MppiPlantModel* pm, PlantOf* out) {
+    if (pm != nullptr) {      // what can be checked without the plan
+        if (pm->struct_size != sizeof(MppiPlantModel)) return MPPI_ERR_ABI;
+        if (pm->reserved != 0 || pm->n_model_tensors < 0) return MPPI_ERR_BAD_ARG;
+        if (pm->model == MPPI_MODEL_PENDULUM_MLP || pm->model == MPPI_MODEL_PENDULUM_MLP_ENSEMBLE)
+            return UNSUPPORTED("closed loop: a PendulumMLP model is learned, not a plant (it has no plant step)");
+        if (pm->model != MPPI_MODEL_PENDULUM && pm->model != MPPI_MODEL_LINEAR_POINT && pm->model != MPPI_MODEL_USER)
+            return MPPI_ERR_BAD_ARG;
+        if (pm->model == MPPI_MODEL_USER &&
+            (pm->user_model == nullptr || reinterpret_cast<const UserModelHandle*>(pm->user_model)->magic != kUserMagic))
+            return MPPI_ERR_BAD_ARG;
+    }
+    if (pl == nullptr) return MPPI_ERR_BAD_ARG;
+    out->mk = pl->mk;
+    out->p = pl->p;
+    if (pm == nullptr) return MPPI_OK;
+    MppiFusedParams& pp = out->p;
+    pp.model = pm->model;
+    pp.user_model = pm->model == MPPI_MODEL_USER ? const_cast<void*>(pm->user_model) : nullptr;
+    pp.model_tensors = pm->model_tensors;
+    pp.n_model_tensors = pm->n_model_tensors;
+    pp.model_params_ext = nullptr;
+    pp.n_model_params_ext = 0;
+    pp.model_weights = nullptr;
+    pp.rollout_samples = 0;
+    int rc = MPPI_OK;
+    out->mk = find_kernels(&pp, &rc);
+    if (out->mk == nullptr) return rc;
+    if (out->mk->nx != pl->nx || out->mk->nu != pl->p.nu) return MPPI_ERR_BAD_ARG;
+    if (out->mk->plant == nullptr)
+        return UNSUPPORTED("closed loop: the plant has no plant step (a step-dependent user model: a closed loop has no horizon index)");
+    return check_model_tensors(out->mk, pm->model_tensors, pm->n_model_tensors);
+}
+
+// the reasons a closed loop is refused, before any CUDA call (MPPI_OK: none); `plant` resolved by resolve_plant
+int check_closed_loop(const Plan* pl, const MppiClosedLoop* cl, const PlantOf& plant, bool own_plant) {
     if (pl == nullptr || cl == nullptr) return MPPI_ERR_BAD_ARG;
     if (cl->struct_size != sizeof(MppiClosedLoop)) return MPPI_ERR_ABI;
     const int n_env = pl->p.n_env > 1 ? pl->p.n_env : 1;
     if (cl->steps < 1 || cl->states == nullptr || cl->actions == nullptr || cl->plant_blocks == nullptr) return MPPI_ERR_BAD_ARG;
     if ((uintptr_t)cl->plant_blocks % 16 != 0 || cl->n_plant_params < 0) return MPPI_ERR_BAD_ARG;
     if (cl->n_plant != 1 && cl->n_plant != n_env) return MPPI_ERR_BAD_ARG;
-    if (cl->plant_params == nullptr && cl->n_plant != 1) return MPPI_ERR_BAD_ARG;
-    if (pl->mk->plant == nullptr)
-        return UNSUPPORTED("closed loop: this model has no plant step (the PendulumMLP models, step-dependent user models)");
+    if (cl->plant_params == nullptr && (cl->n_plant != 1 || own_plant)) return MPPI_ERR_BAD_ARG;
+    if (plant.mk->plant == nullptr)
+        return UNSUPPORTED("closed loop: this model has no plant step (the PendulumMLP models, step-dependent user models): "
+                           "name the plant apart (mppi_plan_closed_loop_plant)");
     if (pl->p.u_per_command != 1) return UNSUPPORTED("closed loop: u_per_command must be 1 (the plant applies one action per command)");
     if (pl->p.world > 1 || (pl->p.flags & MPPI_FLAG_EXPORT_PARTIAL)) return UNSUPPORTED("closed loop: not available on sharded controllers");
     if (pl->p.z_out != nullptr) return UNSUPPORTED("closed loop: the plan records the noise it draws (z_out)");
@@ -174,12 +217,14 @@ int check_closed_loop(const Plan* pl, const MppiClosedLoop* cl) {
     return MPPI_OK;
 }
 
+// A plant named apart from the plan's model always comes with plant_params (check_closed_loop): the plan's own block and
+// its per-environment blocks serve only the plan's model.
 template <typename real>
-int closed_loop_t(Plan* pl, const MppiClosedLoop* cl, cudaStream_t stream) {
-    const ModelKernels* mk = pl->mk;
+int closed_loop_t(Plan* pl, const MppiClosedLoop* cl, const PlantOf& plant, cudaStream_t stream) {
+    const ModelKernels* mk = plant.mk;
     const int n_env = pl->p.n_env > 1 ? pl->p.n_env : 1;
     const int nx = mk->nx, nu = mk->nu;
-    const uint64_t bb = plant_block_bytes(pl);
+    const uint64_t bb = plant_block_bytes(mk);
     PlantStepArgs<real> ps;
     ps.plants = (const unsigned char*)cl->plant_blocks;
     ps.plant_stride = (long long)bb;
@@ -190,12 +235,13 @@ int closed_loop_t(Plan* pl, const MppiClosedLoop* cl, cudaStream_t stream) {
         ps.plants = pl->env_mp;
         ps.n_plant = n_env;
     } else {
-        // the plant blocks, packed once per call with the model's loader (a user model's views: the plan's tensors)
+        // the plant blocks, packed once per call with the plant's loader (a user model's views: the plant's tensors —
+        // the plan's when the plant is the plan's model)
         unsigned char* host = new (std::nothrow) unsigned char[bb * cl->n_plant];
         if (host == nullptr) return MPPI_ERR_BAD_ARG;
         memset(host, 0, bb * cl->n_plant);
         if (cl->plant_params == nullptr) memcpy(host, pl->mparams, mk->param_bytes);
-        else pack_param_rows(pl, cl->plant_params, cl->n_plant, cl->n_plant_params, host);
+        else pack_param_rows(mk, &plant.p, cl->plant_params, cl->n_plant, cl->n_plant_params, host);
         // pageable source: the copy has taken the data when the call returns
         const cudaError_t ce = cudaMemcpyAsync(cl->plant_blocks, host, bb * cl->n_plant, cudaMemcpyHostToDevice, stream);
         delete[] host;
@@ -219,6 +265,7 @@ int closed_loop_t(Plan* pl, const MppiClosedLoop* cl, cudaStream_t stream) {
         ps.u = us;
         ps.w = w != nullptr ? w + (size_t)s * xrow : nullptr;
         ps.cost = cl->costs != nullptr ? (real*)cl->costs + (size_t)s * n_env : nullptr;
+        // with the plan's PDL attribute: none on the tensor-core plans (select_tensor_core_route clears MPPI_FLAG_PDL)
         const cudaError_t e = launch_raw(mk->plant, (n_env + 127) / 128, 128, 0, stream, argv, pl->pdl != 0);
         if (e != cudaSuccess) return cuda_fail(e, "closed loop: plant step launch");
     }
@@ -231,7 +278,7 @@ inline uint64_t env_nm_bytes(const Plan* pl) {
     return pl->is_double ? sizeof(NoiseModel<double>) : sizeof(NoiseModel<float>);
 }
 inline uint64_t env_scratch_bytes(const Plan* pl) {
-    return (uint64_t)pl->p.n_env * (plant_block_bytes(pl) + env_nm_bytes(pl));
+    return (uint64_t)pl->p.n_env * (plant_block_bytes(pl->mk) + env_nm_bytes(pl));
 }
 
 // the reasons the settings are refused, before any CUDA call (MPPI_OK: none)
@@ -268,7 +315,7 @@ int set_env_params_t(Plan* pl, const MppiEnvParams* ep, cudaStream_t stream) {
         return MPPI_OK;
     }
     const int n_env = pl->p.n_env;
-    const uint64_t bb = plant_block_bytes(pl), mp_bytes = (uint64_t)n_env * bb;
+    const uint64_t bb = plant_block_bytes(pl->mk), mp_bytes = (uint64_t)n_env * bb;
     const void* env_kernel = nullptr;
     if (ep->model_params != nullptr) {
         // the per-environment kernel runs the plan's geometry (same tiles, grid and clusters, so the same reduction order):
@@ -289,7 +336,7 @@ int set_env_params_t(Plan* pl, const MppiEnvParams* ep, cudaStream_t stream) {
     unsigned char* host = new (std::nothrow) unsigned char[env_scratch_bytes(pl)];
     if (host == nullptr) return MPPI_ERR_BAD_ARG;
     memset(host, 0, env_scratch_bytes(pl));
-    if (ep->model_params != nullptr) pack_param_rows(pl, ep->model_params, n_env, ep->n_model_params, host);
+    if (ep->model_params != nullptr) pack_param_rows(pl->mk, &pl->p, ep->model_params, n_env, ep->n_model_params, host);
     NoiseModel<real>* nms = reinterpret_cast<NoiseModel<real>*>(host + mp_bytes);
     if (has_nm) {
         // environment e's noise model: the plan's parameters with e's values, through the plan's own fill_noise_model
@@ -622,6 +669,8 @@ uint64_t mppi_abi_layout(int which) {
         case 14: return offsetof(MppiEnvParams, chol);
         case 15: return offsetof(MppiEnvParams, model_params);
         case 16: return offsetof(MppiEnvParams, scratch);
+        case 17: return sizeof(MppiPlantModel);
+        case 18: return offsetof(MppiPlantModel, model_tensors);
     }
     return 0;
 }
@@ -742,14 +791,25 @@ int mppi_plan_set_model_tensors(void* plan, const MppiTensorRef* refs, int32_t n
 
 uint64_t mppi_plan_model_block_bytes(void* plan) {
     const Plan* pl = reinterpret_cast<const Plan*>(plan);
-    return pl == nullptr ? 0 : plant_block_bytes(pl);
+    return pl == nullptr ? 0 : plant_block_bytes(pl->mk);
+}
+
+uint64_t mppi_plant_block_bytes(void* plan, const MppiPlantModel* plant) {
+    PlantOf po;
+    return resolve_plant(reinterpret_cast<const Plan*>(plan), plant, &po) == MPPI_OK ? plant_block_bytes(po.mk) : 0;
+}
+
+int mppi_plan_closed_loop_plant(void* plan, const MppiClosedLoop* cl, const MppiPlantModel* plant, void* stream) {
+    Plan* pl = reinterpret_cast<Plan*>(plan);
+    PlantOf po;
+    int rc = resolve_plant(pl, plant, &po);
+    if (rc == MPPI_OK) rc = check_closed_loop(pl, cl, po, plant != nullptr);
+    if (rc) return rc;
+    return pl->is_double ? closed_loop_t<double>(pl, cl, po, (cudaStream_t)stream) : closed_loop_t<float>(pl, cl, po, (cudaStream_t)stream);
 }
 
 int mppi_plan_closed_loop(void* plan, const MppiClosedLoop* cl, void* stream) {
-    Plan* pl = reinterpret_cast<Plan*>(plan);
-    const int rc = check_closed_loop(pl, cl);
-    if (rc) return rc;
-    return pl->is_double ? closed_loop_t<double>(pl, cl, (cudaStream_t)stream) : closed_loop_t<float>(pl, cl, (cudaStream_t)stream);
+    return mppi_plan_closed_loop_plant(plan, cl, nullptr, stream);
 }
 
 uint64_t mppi_plan_env_scratch_bytes(void* plan) {

@@ -1333,25 +1333,47 @@ class MPPI:
     # ------------------------------------------------------------------------------------------
     # closed-loop episodes on the device (mppi_plan_closed_loop)
     # ------------------------------------------------------------------------------------------
-    def run_closed_loop(self, state, steps, *, plant_params=None, disturbance=None):
+    def run_closed_loop(self, state, steps, *, plant=None, plant_params=None, disturbance=None):
         """The receding-horizon loop — command, apply the first action to the plant, repeat — for `steps` control steps,
         enqueued in one call and run back to back on the GPU.  Step s is exactly ``command(x_s)`` with the device state
-        x_s, followed by ``x_{s+1} = get_rollouts(x_s, U=u_s[None])[0, 0] + disturbance[s]``; afterwards the controller
-        (nominal sequence, cost_total, beta / eta, noise / perturbed_action of the last command, RNG position, `state`)
-        is where those `steps` commands leave it.
+        x_s, followed by ``x_{s+1} = P.get_rollouts(x_s, U=u_s[None])[0, 0] + disturbance[s]``, where P is a controller
+        with this one's u_scale on the plant's model; afterwards the controller (nominal sequence, cost_total, beta /
+        eta, noise / perturbed_action of the last command, RNG position, `state`) is where those `steps` commands leave
+        it.
 
         state         (nx,) device tensor of the controller dtype
-        plant_params  None: the plant is the controller's model with its current parameters.  Else the plant's parameters
-                      in the model's own layout, ``param_blob() + param_blob_ext()`` (a CudaModel: its `params`), e.g.
-                      ``Pendulum(m=1.3).param_blob()``; a CudaModel's tensors are shared with the plant
+        plant         None: the plant is the controller's model.  Else the system the controller acts on, named apart
+                      from the model it plans with: a `Pendulum`, a `LinearPoint` or a `CudaModel` that is not
+                      step-dependent, with the controller's nx and nu.  The controller's model may then be one that is
+                      not a plant (a learned `PendulumMLP`, a `PendulumMLPEnsemble`) or a structurally different one.
+                      A CudaModel plant reads its own tensors; one compiled with copies replays copy 0
+        plant_params  None: the plant's current parameters (plant=None: the controller's model's, or with per-environment
+                      model parameters (MPPI_Batched.set_env_params) each environment's own).  Else the plant's
+                      parameters in its own layout, ``param_blob() + param_blob_ext()`` (a CudaModel: its `params`),
+                      e.g. ``Pendulum(m=1.3).param_blob()``; without `plant`, a CudaModel's tensors are shared with the
+                      plant
         disturbance   None, or a (steps, nx) device tensor of the controller dtype added to each reached state
         Returns a ClosedLoopResult of device tensors: states (steps+1, nx) (row 0 = state), actions (steps, nu), costs
-        (steps,) — the model's running cost of each reached state with its action, cost(x_{s+1}, u_s) at t = 0, under
-        the plant's parameters.  Available on the fused route (registered and CudaModel models, not the PendulumMLP
-        models or step-dependent ones) with u_per_command = 1 on one GPU."""
-        return self._closed_loop(state, steps, plant_params, disturbance, None)
+        (steps,) — the plant's running cost of each reached state with its action, cost(x_{s+1}, u_s) at t = 0, under
+        the plant's parameters.  Available on the fused route (registered and CudaModel models, not step-dependent
+        ones; the PendulumMLP models with a `plant` only) with u_per_command = 1 on one GPU."""
+        return self._closed_loop(state, steps, plant, plant_params, disturbance, None)
 
-    def _closed_loop(self, state, steps, plant_params, disturbance, N):
+    def _check_plant(self, plant):
+        """ValueError unless `plant` can be this controller's plant in a closed loop."""
+        if not isinstance(plant, AnalyticModel):
+            raise ValueError(f"plant must be an AnalyticModel (Pendulum, LinearPoint or CudaModel), got {type(plant).__name__}")
+        if plant.model_id in (_cabi.MODEL_PENDULUM_MLP, _cabi.MODEL_PENDULUM_MLP_ENSEMBLE):
+            raise ValueError("plant: a learned PendulumMLP model has no plant step (it approximates a plant)")
+        if plant.model_id not in (_cabi.MODEL_PENDULUM, _cabi.MODEL_LINEAR_POINT, _cabi.MODEL_USER):
+            raise ValueError(f"plant: {type(plant).__name__} is not a model with a plant step (Pendulum, LinearPoint or "
+                             "CudaModel)")
+        if plant.step_dependent:
+            raise ValueError("plant: a step-dependent CudaModel has no plant step (a closed loop has no horizon index)")
+        if (plant.nx, plant.nu) != (self.nx, self.nu):
+            raise ValueError(f"plant: nx={plant.nx}, nu={plant.nu} differ from the controller's nx={self.nx}, nu={self.nu}")
+
+    def _closed_loop(self, state, steps, plant, plant_params, disturbance, N):
         """run_closed_loop of one environment (N None) or of MPPI_Batched's N."""
         n_env = 1 if N is None else N
         lead = () if N is None else (N,)
@@ -1362,8 +1384,11 @@ class MPPI:
         if m is None:
             raise ValueError("run_closed_loop runs on the fused route: the dynamics and running cost must be a registered "
                              "model's or a CudaModel's (arbitrary callables take the stepped route)")
-        if m.model_id in (_cabi.MODEL_PENDULUM_MLP, _cabi.MODEL_PENDULUM_MLP_ENSEMBLE):
-            raise ValueError("run_closed_loop: a learned PendulumMLP model is not a plant (it approximates one)")
+        if plant is None and m.model_id in (_cabi.MODEL_PENDULUM_MLP, _cabi.MODEL_PENDULUM_MLP_ENSEMBLE):
+            raise ValueError("run_closed_loop: a learned PendulumMLP model is not a plant (it approximates one); name the "
+                             "system it controls with plant=, e.g. plant=Pendulum()")
+        if plant is not None:
+            self._check_plant(plant)
         if m.step_dependent:
             raise ValueError("run_closed_loop: step-dependent models have no per-step schedule in a closed loop")
         if self.u_per_command != 1:
@@ -1386,33 +1411,57 @@ class MPPI:
                     tuple(disturbance.shape) != (steps,) + lead + (self.nx,):
                 raise ValueError(f"disturbance must be a {(steps,) + lead + (self.nx,)} tensor of {self.dtype} on {self.d}")
             disturbance = disturbance.contiguous()
-        n_params = len(m.param_blob()) + len(m.param_blob_ext())
-        plant = None
+        layout = m if plant is None else plant      # the model whose layout plant_params has
+        n_params = len(layout.param_blob()) + len(layout.param_blob_ext())
+        rows = None
         if plant_params is not None:
             pt = plant_params if torch.is_tensor(plant_params) else torch.as_tensor(plant_params, dtype=torch.float64)
             if not pt.is_floating_point() or pt.device not in (torch.device("cpu"), self.d):
                 raise ValueError(f"plant_params must be floating point, on the CPU or {self.d}; got {pt.dtype} on {pt.device}")
             shapes = [(n_params,)] + ([(n_env, n_params)] if N is not None else [])
             if tuple(pt.shape) not in shapes:
-                raise ValueError(f"plant_params must have shape {' or '.join(map(str, shapes))} (the model's "
-                                 f"param_blob() + param_blob_ext()), got {tuple(pt.shape)}")
-            plant = pt.detach().to("cpu", torch.float64).reshape(-1, n_params).contiguous()
-        self._prepare()
+                raise ValueError(f"plant_params must have shape {' or '.join(map(str, shapes))} (the "
+                                 f"{'plant' if plant is not None else 'model'}'s param_blob() + param_blob_ext()), got "
+                                 f"{tuple(pt.shape)}")
+            rows = pt.detach().to("cpu", torch.float64).reshape(-1, n_params).contiguous()
+        elif plant is not None:     # the plant's current parameters, one plant for every environment
+            rows = torch.tensor([plant.param_blob() + plant.param_blob_ext()], dtype=torch.float64).reshape(1, n_params)
         lib = self._lib
+        pm = refs = None
+        if plant is not None:
+            # the plant's own kernels (a CudaModel compiled for this controller's dtype) and tensors
+            pm = _cabi.MppiPlantModel(struct_size=C.sizeof(_cabi.MppiPlantModel), model=plant.model_id)
+            if plant.model_id == _cabi.MODEL_USER:
+                refs = plant.tensor_refs(self.d) if plant.tensors else None
+                if refs is not None:
+                    pm.model_tensors = C.cast(refs[0], C.c_void_p)
+                    pm.n_model_tensors = len(refs[1])
+                with torch.cuda.device(self.d):
+                    pm.user_model = plant.rtc_handle(lib, self.dtype, self._VARIANT)
+        self._prepare()
         seed, base, stride = self._rng_block(steps)
         states = torch.empty((steps + 1,) + lead + (self.nx,), device=self.d, dtype=self.dtype)
         states[0].copy_(state)
         actions = torch.empty((steps,) + lead + (self.nu,), device=self.d, dtype=self.dtype)
         costs = torch.empty((steps,) + lead, device=self.d, dtype=self.dtype)
-        n_plant = 1 if plant is None else plant.shape[0]
-        blocks = torch.empty(n_plant * int(lib.mppi_plan_model_block_bytes(self._plan)), device=self.d, dtype=torch.uint8)
+        n_plant = 1 if rows is None else rows.shape[0]
+        block = lib.mppi_plan_model_block_bytes(self._plan) if pm is None else lib.mppi_plant_block_bytes(self._plan, C.byref(pm))
+        blocks = torch.empty(n_plant * int(block), device=self.d, dtype=torch.uint8)
         cl = _cabi.MppiClosedLoop(struct_size=C.sizeof(_cabi.MppiClosedLoop), steps=steps, seed=seed, offset=base,
                                   offset_stride=stride, states=states.data_ptr(), actions=actions.data_ptr(),
                                   costs=costs.data_ptr(), disturbance=None if disturbance is None else disturbance.data_ptr(),
-                                  plant_params=None if plant is None else plant.data_ptr(), n_plant=n_plant,
-                                  n_plant_params=n_params if plant is not None else 0, plant_blocks=blocks.data_ptr())
+                                  plant_params=None if rows is None else rows.data_ptr(), n_plant=n_plant,
+                                  n_plant_params=n_params if rows is not None else 0, plant_blocks=blocks.data_ptr())
         stream = torch._C._cuda_getCurrentRawStream(self.d.index)
-        _cabi.check(lib.mppi_plan_closed_loop(self._plan, C.byref(cl), stream), "mppi_plan_closed_loop")
+        if pm is None:
+            _cabi.check(lib.mppi_plan_closed_loop(self._plan, C.byref(cl), stream), "mppi_plan_closed_loop")
+        else:
+            _cabi.check(lib.mppi_plan_closed_loop_plant(self._plan, C.byref(cl), C.byref(pm), stream),
+                        "mppi_plan_closed_loop_plant")
+            # the queued plant steps read the plant's tensors: their memory is not reused before those steps ran, even if
+            # the plant swaps them out (set_tensors) meanwhile
+            for t in refs[1] if refs is not None else ():
+                t.record_stream(torch.cuda.current_stream(self.d))
         # ---- the last command (lazy noise / perturbed_action are materialised from its state row) ---------------------
         self._z_keep = None
         last = states[steps - 1]
@@ -1954,11 +2003,13 @@ class MPPI_Batched(MPPI):
         """Every environment's state for each of its K samples: (N*K, nx)."""
         return st.unsqueeze(1).expand(self.N, self.K, self.nx).reshape(self.N * self.K, self.nx)    # mppi.py:846
 
-    def run_closed_loop(self, states, steps, *, plant_params=None, disturbance=None):
+    def run_closed_loop(self, states, steps, *, plant=None, plant_params=None, disturbance=None):
         """`MPPI.run_closed_loop` for the N environments: states (N, nx); plant_params (n_params,) for one plant or
         (N, n_params), one plant per environment (domain randomisation); disturbance (steps, N, nx).  Returns states
-        (steps+1, N, nx), actions (steps, N, nu) and costs (steps, N)."""
-        return self._closed_loop(states, steps, plant_params, disturbance, self.N)
+        (steps+1, N, nx), actions (steps, N, nu) and costs (steps, N).  With an explicit `plant`, per-environment model
+        parameters (set_env_params) stay the controller's: the plants are `plant` with `plant_params` (default: its
+        current parameters, the same for every environment)."""
+        return self._closed_loop(states, steps, plant, plant_params, disturbance, self.N)
 
     # per-environment intermediates are not materialised lazily for the batched controller
     noise = property(lambda self: None)
