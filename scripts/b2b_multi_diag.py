@@ -4,30 +4,23 @@ per command back to back (CUDA events over 2000), with and without programmatic 
 unsharded controller on the same GPU.   usage: torchrun --nproc-per-node N scripts/b2b_multi_diag.py [K_per_gpu] [T]"""
 import os
 import sys
-import time
 
 import torch
 import torch.distributed as dist
 
+import timing
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-K = int(sys.argv[1]) if len(sys.argv) > 1 else 16384
-T = int(sys.argv[2]) if len(sys.argv) > 2 else 30
-rank = int(os.environ["LOCAL_RANK"])
-torch.cuda.set_device(rank)
-dev = torch.device("cuda", rank)
-dist.init_process_group("nccl", device_id=dev)
-world = dist.get_world_size()
-x = torch.tensor([3.14159, 1.0], device=dev)
 
 
-def run(tag, pdl, sharded):
+def run(tag, pdl, sharded, K, T, dev, x):
     os.environ["MPPI_B200_PDL"] = "1" if pdl else "0"
     import pytorch_mppi_b200 as eng
     pend = eng.Pendulum()
     torch.manual_seed(0)
     U0 = torch.randn(T, 1) * 3.16
-    kw = dict(num_samples=K * (world if sharded else 1), horizon=T, u_min=torch.tensor(-2.0), u_max=torch.tensor(2.0), device=dev,
-              rng_seed=1, U_init=U0)
+    kw = dict(num_samples=K * (dist.get_world_size() if sharded else 1), horizon=T, u_min=torch.tensor(-2.0),
+              u_max=torch.tensor(2.0), device=dev, rng_seed=1, U_init=U0)
     if sharded:
         kw["process_group"] = dist.group.WORLD
     c = eng.MPPI(pend.dynamics, pend.running_cost, 2, torch.tensor(10.0), **kw)
@@ -35,31 +28,35 @@ def run(tag, pdl, sharded):
         c.command(x)
     torch.cuda.synchronize()
     dist.barrier()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(400):
-        c.command(x)
-    host_us = (time.perf_counter() - t0) / 400 * 1e6
+    host_us = timing.host_us(lambda: c.command(x), 400, warm=0)
     torch.cuda.synchronize()
     dist.barrier()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(2000):
-        c.command(x)
-    e1.record()
-    torch.cuda.synchronize()
-    dev_us = e0.elapsed_time(e1) / 2000 * 1e3
+    dev_us = timing.back_to_back_us(lambda: c.command(x), 2000, warm=0, reps=1)
     li = c.launch_info
-    print(f"rank {rank} {tag:28s} host enqueue {host_us:6.2f} us/command   device back to back {dev_us:6.2f} us/command   "
+    print(f"rank {dist.get_rank()} {tag:28s} host enqueue {host_us:6.2f} us/command   device back to back {dev_us:6.2f} us/command   "
           f"grid {li.grid_blocks} cluster {li.cluster_size} records {li.xchg_records}", flush=True)
     dist.barrier()
 
 
-run("unsharded, PDL", True, False)
-run("unsharded, no PDL", False, False)
-run("sharded, PDL", True, True)
-run("sharded, no PDL", False, True)
-os.environ["MPPI_B200_XCHG_DIRECT"] = "0"
-run("sharded rank-record, PDL", True, True)
-dist.destroy_process_group()
+def main():
+    K = int(sys.argv[1]) if len(sys.argv) > 1 else 16384
+    T = int(sys.argv[2]) if len(sys.argv) > 2 else 30
+    rank = int(os.environ["LOCAL_RANK"])
+    torch.cuda.set_device(rank)
+    dev = torch.device("cuda", rank)
+    dist.init_process_group("nccl", device_id=dev)
+    if rank == 0:
+        print(timing.card(), flush=True)
+    x = torch.tensor([3.14159, 1.0], device=dev)
+    args = (K, T, dev, x)
+    run("unsharded, PDL", True, False, *args)
+    run("unsharded, no PDL", False, False, *args)
+    run("sharded, PDL", True, True, *args)
+    run("sharded, no PDL", False, True, *args)
+    os.environ["MPPI_B200_XCHG_DIRECT"] = "0"
+    run("sharded rank-record, PDL", True, True, *args)
+    dist.destroy_process_group()
+
+
+if __name__ == "__main__":
+    main()

@@ -1,32 +1,31 @@
 """Fixed overhead of the host round trip: command_host on a tiny problem vs the north-star one."""
-import os, sys, time
+import os
+import sys
+
 import torch
+
+import timing
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import pytorch_mppi_b200 as eng
-pend = eng.Pendulum()
-for K, T in ((32, 2), (1024, 5), (16384, 30)):
-    c = eng.MPPI(pend.dynamics, pend.running_cost, 2, torch.tensor(10.0), num_samples=K, horizon=T,
-                 u_min=torch.tensor(-2.0), u_max=torch.tensor(2.0), device="cuda", rng_seed=1)
-    x = [3.14159, 1.0]
-    for _ in range(300):
-        c.command_host(x)
+import pytorch_mppi_b200 as eng  # noqa: E402
+
+
+def main():
+    print(timing.card())
+    pend = eng.Pendulum()
     n = 3000
-    t0 = time.perf_counter()
-    for _ in range(n):
-        c.command_host(x)
-    e2e = (time.perf_counter() - t0) / n * 1e6
-    # pieces: python-only cost (no launch) approximated by timing the pre/post code paths
-    t0 = time.perf_counter()
-    for _ in range(n):
-        c._host_state(x); c._noise_source(); torch._C._cuda_getCurrentRawStream(0)
-    pre = (time.perf_counter() - t0) / n * 1e6
-    t0 = time.perf_counter()
-    for _ in range(n):
-        torch.empty_like(c._host_template).data_ptr()
-    post = (time.perf_counter() - t0) / n * 1e6
-    # device-side: launch + sync round trip without mailbox
-    t0 = time.perf_counter()
-    for _ in range(n):
-        c.command(x); torch.cuda.synchronize()
-    sync = (time.perf_counter() - t0) / n * 1e6
-    print(f"K={K} T={T}: command_host {e2e:.2f} us | python pre {pre:.2f} post {post:.2f} | command()+synchronize {sync:.2f} us")
+    for K, T in ((32, 2), (1024, 5), (16384, 30)):
+        c = eng.MPPI(pend.dynamics, pend.running_cost, 2, torch.tensor(10.0), num_samples=K, horizon=T,
+                     u_min=torch.tensor(-2.0), u_max=torch.tensor(2.0), device="cuda", rng_seed=1)
+        x = [3.14159, 1.0]
+        e2e = timing.host_us(lambda: c.command_host(x), n, warm=300)
+        # pieces: python-only cost (no launch) approximated by timing the pre/post code paths
+        pre = timing.host_us(lambda: (c._host_state(x), c._noise_source(), torch._C._cuda_getCurrentRawStream(0)), n)
+        post = timing.host_us(lambda: torch.empty_like(c._host_template).data_ptr(), n)
+        # device-side: launch + sync round trip without mailbox
+        sync = timing.host_us(lambda: (c.command(x), torch.cuda.synchronize()), n)
+        print(f"K={K} T={T}: command_host {e2e:.2f} us | python pre {pre:.2f} post {post:.2f} | command()+synchronize {sync:.2f} us")
+
+
+if __name__ == "__main__":
+    main()

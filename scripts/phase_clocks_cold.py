@@ -15,27 +15,12 @@ import sys
 import numpy as np
 import torch
 
+import timing
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import bench  # noqa: E402
 import pytorch_mppi_b200 as eng  # noqa: E402
-
-wl_name = sys.argv[1] if len(sys.argv) > 1 else "pendulum_c2"
-reps = int(sys.argv[2]) if len(sys.argv) > 2 else 30
-wl = bench.WORKLOADS[wl_name]
-dev = torch.device("cuda", 0)
-ctrl = bench.make_engine(eng, wl, wl["K"], dev, None, "p2p")
-x_dev = torch.tensor(wl["x0"], dtype=torch.float32, device=dev)
-flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)
-for _ in range(5):
-    ctrl.command(x_dev)
-torch.cuda.synchronize()
-info = ctrl.launch_info
-dbg = torch.zeros(info.grid_blocks, 16, dtype=torch.int64, device=dev)
-ctrl._debug_clocks = dbg
-ctrl._dirty = True
-ctrl.command(x_dev)
-torch.cuda.synchronize()
 
 # (label, stamp at the start, stamp at the end) on the finisher's path; "start" is the earliest CTA's stamp 0
 PHASES = [("launch -> CTA 0 start", "t0", 0), ("fill normals of tile 0, PDL wait, TMA issue", 0, 1),
@@ -48,10 +33,10 @@ TAIL = [p[0] for p in PHASES if p[1] in (6, 9, 8, 12, 10, 11)]
 MEM_FREE = ["transform", "warp fold", "cluster combine"]
 
 
-def one(cold):
+def one(ctrl, x_dev, dbg, cold):
     dbg.zero_()
     if cold:
-        flush.zero_()
+        timing.flush_l2()
     else:
         torch.cuda.synchronize()
     ctrl.command(x_dev)
@@ -66,26 +51,40 @@ def one(cold):
     return out
 
 
-runs = {False: [], True: []}
-for _ in range(reps):
-    for cold in (False, True):
-        runs[cold].append(one(cold))
-names = list(runs[False][0])
-med = {c: {n: float(np.median([r[n] for r in runs[c]])) for n in names} for c in (False, True)}
-gpu = torch.cuda.get_device_name(dev)
-try:
-    import subprocess
-    power = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader"],
-                           capture_output=True, text=True).stdout.strip()
-except OSError:
-    power = "unknown"
-print(f"{wl_name}: {gpu}, power limit {power}; grid {info.grid_blocks} x {info.block_threads} threads, "
-      f"cluster {info.cluster_size}, split {info.split_cost}, records {info.xchg_records}, "
-      f"ll_tail {getattr(info, 'll_tail', 0)}; median of {reps} repetitions")
-print(f"{'phase (CTA 0)':44s} {'warm us':>8s} {'cold us':>8s} {'cold-warm':>9s}")
-for n in names:
-    print(f"{n:44s} {med[False][n]:8.2f} {med[True][n]:8.2f} {med[True][n] - med[False][n]:9.2f}")
-tail = sum(med[True][n] - med[False][n] for n in TAIL)
-mem_free = sum(med[True][n] - med[False][n] for n in MEM_FREE if n not in TAIL)
-print(f"tail stages (stamps 6 -> 11) cold - warm: {tail:.2f} us; other memory-free phases: {mem_free:.2f} us; "
-      f"together {tail + mem_free:.2f} us")
+def main():
+    wl_name = sys.argv[1] if len(sys.argv) > 1 else "pendulum_c2"
+    reps = int(sys.argv[2]) if len(sys.argv) > 2 else 30
+    wl = bench.WORKLOADS[wl_name]
+    dev = torch.device("cuda", 0)
+    ctrl = bench.make_engine(eng, wl, wl["K"], dev, None, "p2p")
+    x_dev = torch.tensor(wl["x0"], dtype=torch.float32, device=dev)
+    for _ in range(5):
+        ctrl.command(x_dev)
+    torch.cuda.synchronize()
+    info = ctrl.launch_info
+    dbg = torch.zeros(info.grid_blocks, 16, dtype=torch.int64, device=dev)
+    ctrl._debug_clocks = dbg
+    ctrl._dirty = True
+    ctrl.command(x_dev)
+    torch.cuda.synchronize()
+
+    runs = {False: [], True: []}
+    for _ in range(reps):
+        for cold in (False, True):
+            runs[cold].append(one(ctrl, x_dev, dbg, cold))
+    names = list(runs[False][0])
+    med = {c: {n: float(np.median([r[n] for r in runs[c]])) for n in names} for c in (False, True)}
+    print(f"{wl_name}: {timing.card()}; grid {info.grid_blocks} x {info.block_threads} threads, "
+          f"cluster {info.cluster_size}, split {info.split_cost}, records {info.xchg_records}, "
+          f"ll_tail {getattr(info, 'll_tail', 0)}; median of {reps} repetitions")
+    print(f"{'phase (CTA 0)':44s} {'warm us':>8s} {'cold us':>8s} {'cold-warm':>9s}")
+    for n in names:
+        print(f"{n:44s} {med[False][n]:8.2f} {med[True][n]:8.2f} {med[True][n] - med[False][n]:9.2f}")
+    tail = sum(med[True][n] - med[False][n] for n in TAIL)
+    mem_free = sum(med[True][n] - med[False][n] for n in MEM_FREE if n not in TAIL)
+    print(f"tail stages (stamps 6 -> 11) cold - warm: {tail:.2f} us; other memory-free phases: {mem_free:.2f} us; "
+          f"together {tail + mem_free:.2f} us")
+
+
+if __name__ == "__main__":
+    main()

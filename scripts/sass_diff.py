@@ -21,13 +21,18 @@ def kernels(path):
     return out
 
 
-old, new = kernels(sys.argv[1]), kernels(sys.argv[2])
-missing = [k for k in old if k not in new]
-differing = [k for k in old if k in new and old[k] != new[k]]
-print(f"{len(old)} kernels in {sys.argv[1]}, {len(new)} in {sys.argv[2]}: {len(missing)} missing, {len(differing)} differing, "
-      f"{len(new) - len(old) + len(missing)} new")
-for k in missing:
-    print("missing  ", subprocess.run(["c++filt", k], capture_output=True, text=True).stdout.strip()[:160])
-for k in differing:
-    print("differing", subprocess.run(["c++filt", k], capture_output=True, text=True).stdout.strip()[:160])
-sys.exit(1 if missing or differing else 0)
+def main():
+    old, new = kernels(sys.argv[1]), kernels(sys.argv[2])
+    missing = [k for k in old if k not in new]
+    differing = [k for k in old if k in new and old[k] != new[k]]
+    print(f"{len(old)} kernels in {sys.argv[1]}, {len(new)} in {sys.argv[2]}: {len(missing)} missing, {len(differing)} differing, "
+          f"{len(new) - len(old) + len(missing)} new")
+    for k in missing:
+        print("missing  ", subprocess.run(["c++filt", k], capture_output=True, text=True).stdout.strip()[:160])
+    for k in differing:
+        print("differing", subprocess.run(["c++filt", k], capture_output=True, text=True).stdout.strip()[:160])
+    sys.exit(1 if missing or differing else 0)
+
+
+if __name__ == "__main__":
+    main()

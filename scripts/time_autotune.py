@@ -6,19 +6,18 @@
 2. The same generation through the sequential `Autotune`, whose evaluate_fn runs one `run_closed_loop` (the 4 starts)
    per candidate, and once more for the best point, as the reference does.
 3. µs per back-to-back `MPPI_Batched.command()` at N = 16, K = 4096, T = 30 with mixed horizons (5..30) against every
-   environment at T (CUDA events, best of 5 windows), the two alternating within each round.
+   environment at T (best of 5 windows per round), the two alternating within each round.
 
 Prints one JSON line with the card name and power limit.
 usage: python scripts/time_autotune.py [--generations 5] [--commands 1000] [--rounds 3]"""
 import argparse
-import json
 import math
 import os
-import subprocess
 import sys
-import time
 
 import torch
+
+import timing
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pytorch_mppi_b200 as eng  # noqa: E402
@@ -38,16 +37,6 @@ def params(ctrl):
     ps = [autotune.SigmaParameter(ctrl), autotune.LambdaParameter(ctrl), autotune.HorizonParameter(ctrl)]
     ps[2].max_horizon = T
     return ps
-
-
-def per_generation_ms(tuner, n):
-    tuner.optimize_step()                      # warm-up: plans, module loads
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(n):
-        tuner.optimize_step()
-    torch.cuda.synchronize()
-    return (time.perf_counter() - t0) * 1e3 / n
 
 
 def batched_tuner():
@@ -70,31 +59,17 @@ def sequential_tuner():
     return autotune.Autotune(params(ctrl), evaluate, optimizer=autotune.CMAESOpt(POP, 1.0, seed=0))
 
 
-def command_us(c, x0, n, reps=5):
-    best = float("inf")
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        a.record()
-        for _ in range(n):
-            c.command(x0)
-        b.record()
-        torch.cuda.synchronize()
-        best = min(best, a.elapsed_time(b) * 1e3 / n)
-    return best
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--generations", type=int, default=5)
     ap.add_argument("--commands", type=int, default=1000)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    out = {"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(),
-           "generation": {"candidates": POP, "starts": S, "steps": STEPS, "K": K, "max_horizon": T, "dtype": "float32"}}
-    out["batched_ms_per_generation"] = round(per_generation_ms(batched_tuner(), args.generations), 1)
-    out["sequential_ms_per_generation"] = round(per_generation_ms(sequential_tuner(), args.generations), 1)
+    out = {"generation": {"candidates": POP, "starts": S, "steps": STEPS, "K": K, "max_horizon": T, "dtype": "float32"}}
+    for name, make_tuner in (("batched", batched_tuner), ("sequential", sequential_tuner)):
+        # one window of the generations after one warm-up generation (plans, module loads)
+        us = timing.back_to_back_us(make_tuner().optimize_step, args.generations, warm=1, reps=1)
+        out[f"{name}_ms_per_generation"] = round(us / 1e3, 1)
 
     N = 16
     pend = eng.Pendulum()
@@ -103,14 +78,10 @@ def main():
     uniform, mixed = make(), make()
     mixed.set_env_horizon(torch.linspace(5, T, N).round().to(torch.int32))
     x0 = torch.tensor([[math.pi, 0.0]] * N, device="cuda")
-    for c in (uniform, mixed):
-        command_us(c, x0, 50, reps=1)
-    res = {"uniform_T": [], "mixed_5_to_30": []}
-    for _ in range(args.rounds):
-        res["uniform_T"].append(command_us(uniform, x0, args.commands))
-        res["mixed_5_to_30"].append(command_us(mixed, x0, args.commands))
+    res = timing.alternate_us({"uniform_T": (lambda: uniform.command(x0), args.commands),
+                               "mixed_5_to_30": (lambda: mixed.command(x0), args.commands)}, args.rounds, reps=5)
     out["command_us_N16"] = {k: [round(v, 2) for v in x] for k, x in res.items()}
-    print(json.dumps(out))
+    timing.emit(out)
 
 
 if __name__ == "__main__":

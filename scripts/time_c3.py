@@ -6,15 +6,15 @@ import sys
 
 import torch
 
+import timing
+
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pytorch_mppi_b200 as eng  # noqa: E402
 
 K, T, S = 8192, 40, 5
-nav = eng.LinearPoint.toy2d_nav(terminal_scale=10.0)
-x0 = torch.tensor([-3.0, -2.0], device="cuda")
 
 
-def make(kind, split, stepped=False):
+def make(nav, kind, split, stepped=False):
     os.environ["MPPI_B200_SPLIT_COST"] = "1" if split else "0"
     dyn, cost, term = nav.dynamics, nav.running_cost, nav.terminal_cost
     if stepped:
@@ -27,30 +27,22 @@ def make(kind, split, stepped=False):
     return eng.KMPPI(dyn, cost, 2, torch.eye(2), num_support_pts=S, kernel=eng.RBFKernel(sigma=2), **kw)
 
 
-def b2b(c, n):
-    for _ in range(20):
-        c.command(x0)
-    torch.cuda.synchronize()
-    best = 1e9
-    for _ in range(3):
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(n):
-            c.command(x0)
-        e1.record()
-        torch.cuda.synchronize()
-        best = min(best, e0.elapsed_time(e1) / n * 1e3)
-    return best
+def main():
+    print(timing.card(), flush=True)
+    nav = eng.LinearPoint.toy2d_nav(terminal_scale=10.0)
+    x0 = torch.tensor([-3.0, -2.0], device="cuda")
+    for kind in ("kmppi", "mppi", "smppi"):
+        for split in (0, 1):
+            c = make(nav, kind, split)
+            t_us = timing.back_to_back_us(lambda: c.command(x0), 500)
+            li = c.launch_info   # set when the first command packs the launch parameters
+            print(f"{kind:5s} fused split={li.split_cost} grid={li.grid_blocks} block={li.block_threads} tps={li.threads_per_sample} "
+                  f"regs={li.regs_per_thread} smem={li.smem_bytes}: {t_us:.2f} us/command back to back", flush=True)
+        c = make(nav, kind, 0, stepped=True)
+        print(f"{kind:5s} stepped (Python T-loop + kernels): {timing.back_to_back_us(lambda: c.command(x0), 20):.1f} us/command", flush=True)
+        c.compile()
+        print(f"{kind:5s} stepped + compile() (CUDA graph): {timing.back_to_back_us(lambda: c.command(x0), 50):.1f} us/command", flush=True)
 
 
-for kind in ("kmppi", "mppi", "smppi"):
-    for split in (0, 1):
-        c = make(kind, split)
-        t_us = b2b(c, 500)
-        li = c.launch_info   # set when the first command packs the launch parameters
-        print(f"{kind:5s} fused split={li.split_cost} grid={li.grid_blocks} block={li.block_threads} tps={li.threads_per_sample} "
-              f"regs={li.regs_per_thread} smem={li.smem_bytes}: {t_us:.2f} us/command back to back", flush=True)
-    c = make(kind, 0, stepped=True)
-    print(f"{kind:5s} stepped (Python T-loop + kernels): {b2b(c, 20):.1f} us/command", flush=True)
-    c.compile()
-    print(f"{kind:5s} stepped + compile() (CUDA graph): {b2b(c, 50):.1f} us/command", flush=True)
+if __name__ == "__main__":
+    main()

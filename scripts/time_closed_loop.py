@@ -1,19 +1,19 @@
 """Microseconds per control step of a closed-loop episode: `run_closed_loop(steps=1000)` (commands and plant steps
 enqueued from C, chained with programmatic dependent launch) against back-to-back `command()` on a device state (no
 plant) and the Python host loop it replaces (`u = command(x)`, `x = get_rollouts(x, U=u[None])[0, 0]`).  Shapes: the C2
-pendulum (MPPI, K=16384, T=30, fp32) and MPPI_Batched N=16, K=4096, T=30 (fp32 pendulum).  Warm-up first, then CUDA
-events around each measurement (best of 3).  Prints one JSON line with the card name and power limit.
+pendulum (MPPI, K=16384, T=30, fp32) and MPPI_Batched N=16, K=4096, T=30 (fp32 pendulum).  Two episodes of warm-up, then
+each timed over whole episodes (best of 3).  Prints one JSON line with the card name and power limit.
 
 usage: python scripts/time_closed_loop.py [--steps 1000] [--trace DIR]   (--trace: a torch.profiler trace of a 50-step
 episode of each shape, for launch gaps)"""
 import argparse
-import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
+
+import timing
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pytorch_mppi_b200 as eng  # noqa: E402
@@ -29,20 +29,6 @@ def batched():
     m = eng.Pendulum()
     return eng.MPPI_Batched(m.dynamics, m.running_cost, 2, torch.tensor(10.0), 16, num_samples=4096, horizon=30,
                             device="cuda", u_max=torch.tensor(2.0), rng_seed=1)
-
-
-def timed(fn, steps, reps=3):
-    """best us per step of fn() (which runs `steps` control steps), CUDA events around it"""
-    best = float("inf")
-    for _ in range(reps):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        torch.cuda.synchronize()
-        a.record()
-        fn()
-        b.record()
-        torch.cuda.synchronize()
-        best = min(best, a.elapsed_time(b) * 1e3 / steps)
-    return best
 
 
 def host_loop(c, x0, steps):
@@ -61,13 +47,11 @@ def back_to_back(c, x0, steps):
 
 def measure(name, make, x0, steps):
     c = make()
-    for _ in range(2):                                 # warm-up: plans, module loads, caches
-        c.run_closed_loop(x0, 50)
-        back_to_back(c, x0, 50)
-        host_loop(c, x0, 50)
-    out = {"closed_loop_us": timed(lambda: c.run_closed_loop(x0, steps), steps),
-           "command_b2b_us": timed(lambda: back_to_back(c, x0, steps), steps),
-           "host_loop_us": timed(lambda: host_loop(c, x0, steps), steps)}
+    # each a window of one episode of `steps` control steps, after two such episodes of warm-up; best of 3
+    out = {k: timing.back_to_back_us(fn, 1, warm=2, reps=3) / steps
+           for k, fn in (("closed_loop_us", lambda: c.run_closed_loop(x0, steps)),
+                         ("command_b2b_us", lambda: back_to_back(c, x0, steps)),
+                         ("host_loop_us", lambda: host_loop(c, x0, steps)))}
     # what the plant step adds to a control step over back-to-back commands
     out["closed_loop_minus_command_us"] = out["closed_loop_us"] - out["command_b2b_us"]
     info = c.launch_info
@@ -81,9 +65,7 @@ def main():
     ap.add_argument("--steps", type=int, default=1000)
     ap.add_argument("--trace", default=None)
     args = ap.parse_args()
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    out = {"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(),
-           "steps": args.steps}
+    out = {"steps": args.steps}
     x_c2 = torch.tensor([math.pi, 0.0], device="cuda")
     x_b = torch.tensor([[math.pi, 0.0]] * 16, device="cuda")
     out.update(measure("c2_pendulum_K16384_T30_f32", c2, x_c2, args.steps))
@@ -104,7 +86,7 @@ def main():
             plant = [e.time_range.elapsed_us() for e in ev if "plant_step" in e.name]
             out[f"trace_{name}"] = {"kernels": len(ev), "plant_kernel_us_median": sorted(plant)[len(plant) // 2] if plant else None,
                                     "gap_us_median": sorted(gaps)[len(gaps) // 2] if gaps else None}
-    print(json.dumps(out))
+    timing.emit(out)
 
 
 if __name__ == "__main__":

@@ -6,18 +6,18 @@
   (`u = command(x)`, `x = P.get_rollouts(x, U=u[None])[0, 0]` with P a controller on the plant).
 * C2 pendulum (MPPI, K=16384, T=30, fp32): `plant=Pendulum()` against `plant=None` (the same plant step).
 
-Warm-up first; the variants of each shape alternate within a repetition, CUDA events around each (best of 5).  Prints
+The variants of each shape alternate within a repetition, an episode of warm-up before each (best of 5).  Prints
 one JSON line with the card name and power limit.
 
 usage: python scripts/time_closed_loop_plant.py [--steps 1000]"""
 import argparse
-import json
 import math
 import os
-import subprocess
 import sys
 
 import torch
+
+import timing
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pytorch_mppi_b200 as eng  # noqa: E402
@@ -38,36 +38,17 @@ def c2():
                     u_min=torch.tensor(-2.0), u_max=torch.tensor(2.0), U_init=torch.zeros(30, 1), rng_seed=1)
 
 
-def time_once(fn, steps):
-    """us per step of fn() (which runs `steps` control steps), CUDA events around it"""
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    a.record()
-    fn()
-    b.record()
-    torch.cuda.synchronize()
-    return a.elapsed_time(b) * 1e3 / steps
-
-
 def alternate(variants, steps, reps=5):
-    """best us per step of each variant, the variants interleaved within every repetition"""
-    for fn in variants.values():                      # warm-up: plans, module loads, caches
-        fn(50)
-        fn(50)
-    best = {k: float("inf") for k in variants}
-    for _ in range(reps):
-        for k, fn in variants.items():
-            best[k] = min(best[k], time_once(lambda: fn(steps), steps))
-    return {k: round(v, 2) for k, v in best.items()}
+    """best us per step of each variant fn(n), which runs n control steps: episodes of `steps`, interleaved"""
+    samples = timing.alternate_us({k: ((lambda fn=fn: fn(steps)), 1) for k, fn in variants.items()}, reps, warm=1)
+    return {k: round(min(v) / steps, 2) for k, v in samples.items()}
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=1000)
     args = ap.parse_args()
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    out = {"gpu": q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name(),
-           "steps": args.steps}
+    out = {"steps": args.steps}
     plant = eng.Pendulum()
     pc = eng.MPPI(plant.dynamics, plant.running_cost, 2, torch.tensor(1.0), num_samples=64, horizon=5, device="cuda")
 
@@ -95,7 +76,7 @@ def main():
     d = c2()
     out["c2_pendulum_K16384_T30_f32"] = alternate({"plant_pendulum_us": lambda n: d.run_closed_loop(x2, n, plant=plant),
                                                    "plant_none_us": lambda n: d.run_closed_loop(x2, n)}, args.steps)
-    print(json.dumps(out))
+    timing.emit(out)
 
 
 if __name__ == "__main__":

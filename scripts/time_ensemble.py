@@ -1,16 +1,15 @@
 """Ensemble controllers (tests/ensemble_models.py: pendulum with a mass and length per copy, terminal cost) at K=16384,
-T=30, fp32, for rollout_samples M in {1, 2, 4, 8}: time per command of the fused `command()` back to back (one
-synchronise at the end), of the fused `command()` with L2 flushed before each command (CUDA events around the command
-alone), and of the stepped route (the same torch twins in the reference's M-copy Python T-loop).  M = 1 is the same
-pendulum compiled without copies, on the single-loop kernel (the one copies use) and on the split-cost kernel (the
-default for one copy at this size).  Prints one JSON line with the card name and power limit."""
-import json
+T=30, fp32, for rollout_samples M in {1, 2, 4, 8}: time per command of the fused `command()` back to back, of the
+fused `command()` with L2 flushed before each command, and of the stepped route (the same torch twins in the
+reference's M-copy Python T-loop).  M = 1 is the same pendulum compiled without copies, on the single-loop kernel
+(the one copies use) and on the split-cost kernel (the default for one copy at this size).  Prints one JSON line with
+the card name and power limit."""
 import os
-import subprocess
 import sys
-import time
 
 import torch
+
+import timing
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pytorch_mppi_b200 as eng  # noqa: E402
@@ -42,55 +41,23 @@ def make(m, M, stepped=False, split=True):
     return c
 
 
-def back_to_back_us(c, n):
-    for _ in range(20):
-        c.command(X0)
-    torch.cuda.synchronize()
-    best = float("inf")
-    for _ in range(3):
-        t0 = time.perf_counter()
-        for _ in range(n):
-            c.command(X0)
-        torch.cuda.synchronize()
-        best = min(best, (time.perf_counter() - t0) / n * 1e6)
-    return best
-
-
-def flushed_us(c, n, flush):
-    for _ in range(5):
-        c.command(X0)
-    ts = []
-    for _ in range(n):
-        flush.zero_()                               # 256 MB: evicts the 50 MB L2
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        c.command(X0)
-        e1.record()
-        e1.synchronize()
-        ts.append(e0.elapsed_time(e1) * 1e3)
-    ts.sort()
-    return ts[len(ts) // 2]
-
-
 def main():
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     out = {}
     for M in (1, 2, 4, 8):
         m = model(M)
         fused = make(m, M)
-        out[f"M{M}_fused_command_us"] = back_to_back_us(fused, 2000)
-        out[f"M{M}_fused_command_l2_flushed_us"] = flushed_us(fused, 200, flush)
+        out[f"M{M}_fused_command_us"] = timing.back_to_back_us(lambda: fused.command(X0), 2000)
+        out[f"M{M}_fused_command_l2_flushed_us"] = timing.median(timing.flushed_us(lambda: fused.command(X0), 200))
         out[f"M{M}_split_cost"] = int(fused.launch_info.split_cost)
         out[f"M{M}_regs"] = int(fused.launch_info.regs_per_thread)
         if M == 1:
             single = make(m, M, split=False)
-            out["M1_single_loop_command_us"] = back_to_back_us(single, 2000)
-            out["M1_single_loop_command_l2_flushed_us"] = flushed_us(single, 200, flush)
-        out[f"M{M}_stepped_command_us"] = back_to_back_us(make(m, M, stepped=True), 50)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    out["gpu"] = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
+            out["M1_single_loop_command_us"] = timing.back_to_back_us(lambda: single.command(X0), 2000)
+            out["M1_single_loop_command_l2_flushed_us"] = timing.median(timing.flushed_us(lambda: single.command(X0), 200))
+        stepped = make(m, M, stepped=True)
+        out[f"M{M}_stepped_command_us"] = timing.back_to_back_us(lambda: stepped.command(X0), 50)
     out["config"] = f"K={K} T={T} fp32, pendulum ensemble with terminal cost, rollout_var_cost=0.5"
-    print(json.dumps(out))
+    timing.emit(out)
 
 
 if __name__ == "__main__":

@@ -1,14 +1,14 @@
 """Microseconds per command of the global-tile kernels (tile_memory="global") against the stepped route past the
 shared-memory edge, and against the shared-memory kernels at a horizon where both plan.  (8,4) shape model, fp64,
-K = 2048; CUDA events around N back-to-back commands after a warm-up (the stepped route: 2 commands), in R windows per
-case with the cases interleaved; prints min / median / max per case.  usage: time_long_horizon.py [N [R]]"""
-import json
+K = 2048; windows of N back-to-back commands (the stepped route: 2 commands) after a warm-up, R windows per case with
+the cases interleaved; prints min / median / max per case.  usage: time_long_horizon.py [N [R]]"""
 import os
-import subprocess
 import sys
 
 import numpy as np
 import torch
+
+import timing
 
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
 import pytorch_mppi_b200 as eng  # noqa: E402
@@ -28,25 +28,10 @@ def ctrl(variant, T, route, tm):
                u_max=torch.full((nu,), 1.2, dtype=dtype), device="cuda", rng_seed=1, tile_memory=tm, **kw)
 
 
-def time_us(c, n):
-    x = torch.linspace(-0.5, 0.5, 8, dtype=torch.float64)
-    for _ in range(3):
-        c.command(x)
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        c.command(x)
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) * 1000.0 / n
-
-
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 50
     reps = int(sys.argv[2]) if len(sys.argv) > 2 else 5
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    x = torch.linspace(-0.5, 0.5, 8, dtype=torch.float64)
     cases = {}
     for v in ("mppi", "smppi", "kmppi"):
         Ts = 150 if v == "mppi" else 90          # within the shared-memory edge of each variant (185 / 97 / 99)
@@ -54,13 +39,10 @@ def main():
         cases[f"{v} T=512 stepped global"] = (ctrl(v, 512, "stepped", "global"), 2)
         cases[f"{v} T={Ts} fused shared"] = (ctrl(v, Ts, "fused", "shared"), n)
         cases[f"{v} T={Ts} fused global"] = (ctrl(v, Ts, "fused", "global"), n)
-    runs = {k: [] for k in cases}
-    for _ in range(reps):                     # the cases interleaved, so that a slow phase of the host hits all of them
-        for k, (c, m) in cases.items():
-            runs[k].append(time_us(c, m))
-    out = {"gpu": gpu, "K": 2048, "shape": "(8,4) fp64", "commands_per_window": n, "windows": reps,
+    runs = timing.alternate_us({k: ((lambda c=c: c.command(x)), m) for k, (c, m) in cases.items()}, reps, warm=3)
+    out = {"K": 2048, "shape": "(8,4) fp64", "commands_per_window": n, "windows": reps,
            "us_per_command": {k: {"min": min(r), "median": sorted(r)[len(r) // 2], "max": max(r)} for k, r in runs.items()}}
-    print(json.dumps(out, indent=1))
+    timing.emit(out)
 
 
 if __name__ == "__main__":

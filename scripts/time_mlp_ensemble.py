@@ -1,16 +1,15 @@
 """Ensembles of learned pendulum networks (PendulumMLPEnsemble: M networks of BASELINE config 4's shape, one per rollout
 copy) at K=32768, T=30, fp32, for rollout_samples M in {2, 4, 8}: time per command of the fused wgmma kernel (hi/lo-split
-bf16 operands, the default) back to back (one synchronise at the end) and with L2 flushed before each command (CUDA events
-around the command alone), of the fused FFMA kernel (tensor_cores=False) back to back, and of the stepped route (the same
-torch twin in the reference's M-copy Python T-loop).  M = 1 is one PendulumMLP on the same two kernels.  Prints one JSON
+bf16 operands, the default) back to back and with L2 flushed before each command, of the fused FFMA kernel
+(tensor_cores=False) back to back, and of the stepped route (the same torch twin in the reference's M-copy Python
+T-loop).  M = 1 is one PendulumMLP on the same two kernels.  Prints one JSON
 line with the card name and power limit."""
-import json
 import os
-import subprocess
 import sys
-import time
 
 import torch
+
+import timing
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pytorch_mppi_b200 as eng  # noqa: E402
@@ -34,55 +33,23 @@ def make(m, M, stepped=False):
     return c
 
 
-def back_to_back_us(c, n):
-    for _ in range(10):
-        c.command(X0)
-    torch.cuda.synchronize()
-    best = float("inf")
-    for _ in range(3):
-        t0 = time.perf_counter()
-        for _ in range(n):
-            c.command(X0)
-        torch.cuda.synchronize()
-        best = min(best, (time.perf_counter() - t0) / n * 1e6)
-    return best
-
-
-def flushed_us(c, n, flush):
-    for _ in range(5):
-        c.command(X0)
-    ts = []
-    for _ in range(n):
-        flush.zero_()                               # 256 MB: evicts the 50 MB L2
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        c.command(X0)
-        e1.record()
-        e1.synchronize()
-        ts.append(e0.elapsed_time(e1) * 1e3)
-    ts.sort()
-    return ts[len(ts) // 2]
-
-
 def main():
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     out = {}
     for M in (1, 2, 4, 8):
         wg = make(model(M, "bf16x3"), M)
-        out[f"M{M}_wgmma_command_us"] = back_to_back_us(wg, 500)
-        out[f"M{M}_wgmma_command_l2_flushed_us"] = flushed_us(wg, 100, flush)
+        out[f"M{M}_wgmma_command_us"] = timing.back_to_back_us(lambda: wg.command(X0), 500)
+        out[f"M{M}_wgmma_command_l2_flushed_us"] = timing.median(timing.flushed_us(lambda: wg.command(X0), 100))
         out[f"M{M}_wgmma_regs"] = int(wg.launch_info.regs_per_thread)
         out[f"M{M}_wgmma_smem_bytes"] = int(wg.launch_info.smem_bytes)
         out[f"M{M}_wgmma_ctas_per_sm"] = int(wg.launch_info.max_blocks_per_sm)
         ff = make(model(M, False), M)
-        out[f"M{M}_ffma_command_us"] = back_to_back_us(ff, 200)
+        out[f"M{M}_ffma_command_us"] = timing.back_to_back_us(lambda: ff.command(X0), 200)
         out[f"M{M}_ffma_regs"] = int(ff.launch_info.regs_per_thread)
         if M > 1:
-            out[f"M{M}_stepped_command_us"] = back_to_back_us(make(model(M, False), M, stepped=True), 10)
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    out["gpu"] = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
+            stepped = make(model(M, False), M, stepped=True)
+            out[f"M{M}_stepped_command_us"] = timing.back_to_back_us(lambda: stepped.command(X0), 10)
     out["config"] = f"K={K} T={T} fp32, MPPI, rollout_var_cost=0.5, networks of pendulum_approximate.py's shape"
-    print(json.dumps(out))
+    timing.emit(out)
 
 
 if __name__ == "__main__":

@@ -1,15 +1,15 @@
 """A tracking problem with a step-dependent user model (tests/step_models.py: double integrator with a time-varying force,
 moving target) at K=16384, T=30, fp32, with `set_params` moving the target before every control step: time per step of
-the fused `command()` (back to back, one synchronise at the end), the fused `command_host()` (the action back on the
+the fused `command()` (back to back), the fused `command_host()` (the action back on the
 host every step) and the stepped route (the same torch twins in a Python T-loop).  Prints one JSON line with the card
 name and power limit."""
-import json
+import itertools
 import os
-import subprocess
 import sys
-import time
 
 import torch
+
+import timing
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import pytorch_mppi_b200 as eng  # noqa: E402
@@ -30,23 +30,14 @@ def make(m, stepped):
 
 def per_step_us(m, c, call, n):
     p = list(m.params)
+    i = itertools.count()
 
-    def step(i):
-        p[3] = 0.5 + 0.03 * i            # the target moves every control step
+    def step():
+        p[3] = 0.5 + 0.03 * (next(i) % n)           # the target moves every control step
         m.set_params(p)
         return call(c, [0.0, 0.0])
 
-    for i in range(20):
-        step(i)
-    torch.cuda.synchronize()
-    best = float("inf")
-    for _ in range(3):
-        t0 = time.perf_counter()
-        for i in range(n):
-            step(i)
-        torch.cuda.synchronize()
-        best = min(best, (time.perf_counter() - t0) / n * 1e6)
-    return best
+    return timing.back_to_back_us(step, n)
 
 
 def main():
@@ -58,10 +49,8 @@ def main():
         "stepped_command_us": per_step_us(m, stepped, lambda c, x: c.command(x), 100),
         "split_cost": int(fused.launch_info.split_cost),
     }
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    out["gpu"] = q.stdout.strip().splitlines()[0] if q.returncode == 0 and q.stdout.strip() else torch.cuda.get_device_name()
     out["config"] = f"K={K} T={T} fp32, set_params before every step"
-    print(json.dumps(out))
+    timing.emit(out)
 
 
 if __name__ == "__main__":
