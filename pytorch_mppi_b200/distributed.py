@@ -25,12 +25,10 @@ def shard_bounds(K: int, rank: int, world: int):
     """(k_offset, K_local) of `rank`'s contiguous slice; the first K % world ranks get one extra."""
     if world < 1 or not (0 <= rank < world):
         raise ValueError(f"bad rank/world {rank}/{world}")
-    base, rem = divmod(K, world)
-    k_local = base + (1 if rank < rem else 0)
-    k_off = rank * base + min(rank, rem)
-    if k_local < 1:
+    if K < world:           # on every rank alike: a rank that went on would wait for the refused ones
         raise ValueError(f"K={K} is smaller than the world size {world}")
-    return k_off, k_local
+    base, rem = divmod(K, world)
+    return rank * base + min(rank, rem), base + (1 if rank < rem else 0)
 
 
 def combine_partials(records: torch.Tensor, lambda_: float):
@@ -45,7 +43,10 @@ def combine_partials(records: torch.Tensor, lambda_: float):
 
 
 class PeerMailboxes:
-    """One small cudaMalloc'd mailbox per rank, mapped into every peer through CUDA IPC."""
+    """One small cudaMalloc'd mailbox per rank, mapped into every peer through CUDA IPC.
+
+    The in-kernel exchange needs every rank's grid resident at the same time.  Kernels of two processes on one GPU take
+    turns instead, so a group in which two ranks share a device is refused (ValueError) before any mailbox exists."""
 
     def __init__(self, lib, group, device):
         import torch.distributed as dist
@@ -53,7 +54,15 @@ class PeerMailboxes:
         self.group = group
         self.rank = dist.get_rank(group)
         self.world = dist.get_world_size(group)
+        self.own = None
+        self._opened = []
         from . import _cabi
+        uuids = [None] * self.world
+        dist.all_gather_object(uuids, str(torch.cuda.get_device_properties(device).uuid), group=group)
+        shared = [g for g in range(self.world) if uuids.count(uuids[g]) > 1]
+        if shared:
+            raise ValueError(f"exchange='p2p' needs one GPU per rank: ranks {shared} share a device (their kernels would not "
+                             "run at the same time); use exchange='nccl'")
         with torch.cuda.device(device):
             own = C.c_void_p()
             handle = (C.c_ubyte * 64)()
@@ -62,7 +71,6 @@ class PeerMailboxes:
             handles = [None] * self.world
             dist.all_gather_object(handles, bytes(handle), group=group)
             self.ptrs = []
-            self._opened = []
             for g in range(self.world):
                 if g == self.rank:
                     self.ptrs.append(self.own)

@@ -35,10 +35,16 @@ logger = logging.getLogger(__name__)
 _DT = {torch.float32: _cabi.F32, torch.float64: _cabi.F64}
 _ES = {torch.float32: 4, torch.float64: 8}
 _TILE_MEMORY = ("shared", "global", "auto")
+_XCHG_MAX_ROWS = 1024       # entries of one rank's exchanged record (MPPI_XCHG_MAX_R, csrc/mppi_fused.cuh)
 
 
 class SpecificActionSampler:
-    """Same hook as the reference's (mppi.py:16-32)."""
+    """Same hook as the reference's (mppi.py:16-32).
+
+    `register_sample_start_end` names the rows of the rollout batch that `specific_dynamics` receives.  On a sharded
+    controller (process_group=) that batch is this rank's K_local samples, so the registered range is the part of the
+    sampler's global rows [start, end) that falls on this rank's shard, in shard-local indices (empty on a rank that
+    holds none of them): `next_state[:, self.slice]` is then this rank's share of the sampler's rows."""
 
     def __init__(self):
         self.start_idx = 0
@@ -153,6 +159,9 @@ class MPPI:
                  tile_memory: str = "shared"):
         if tile_memory not in _TILE_MEMORY:
             raise ValueError(f"tile_memory must be one of {_TILE_MEMORY}, got {tile_memory!r}")
+        if exchange not in ("p2p", "nccl"):
+            raise ValueError(f"exchange must be 'p2p' (in-kernel peer exchange) or 'nccl' (all-gather of exported records), "
+                             f"got {exchange!r}")
         self._lib = _cabi.load()          # raises if the CUDA library is not built
         self.d = torch.device(device)
         if self.d.type != "cuda":
@@ -405,6 +414,10 @@ class MPPI:
         pass
 
     def _pack(self):
+        if self._world > 1 and self._noise_rows() > _XCHG_MAX_ROWS:
+            # the stepped route would otherwise find out in its softmin kernel, after sampling and the rollout
+            raise ValueError(f"sharded controllers exchange records of at most {_XCHG_MAX_ROWS} nominal entries: "
+                             f"{'S' if self._VARIANT == _cabi.VARIANT_KMPPI else 'T'}*nu = {self._noise_rows()}")
         p = self._p
         nu = self.nu
         p.struct_size = C.sizeof(_cabi.MppiFusedParams)
@@ -522,6 +535,7 @@ class MPPI:
         if self._world > 1:
             self._setup_exchange(p)
             if self._model is not None:       # the exchange mode depends on the peers: report the geometry of the real plan
+                p.flags = self._base_flags | self._export_flag()
                 info = _cabi.MppiLaunchInfo()
                 _cabi.check(self._lib.mppi_fused_query(C.byref(p), C.byref(info)), "mppi_fused_query")
                 self.launch_info = info
@@ -586,7 +600,7 @@ class MPPI:
         """Freeze the launch state in the C library (`mppi_plan_create`): per command only the state,
         RNG counter, flags and action destination cross the boundary."""
         self._drop_plan()
-        p.flags = self._base_flags | (_cabi.FLAG_EXPORT_PARTIAL if (self._world > 1 and self._exchange != "p2p") else 0)
+        p.flags = self._base_flags | self._export_flag()
         p.z_out = None if self._z_out is None else self._z_out.data_ptr()
         p.epoch = self._epoch
         p.host_epoch = self._host_epoch      # the new plan continues the mailbox tags where the old one stopped
@@ -600,6 +614,10 @@ class MPPI:
         # build container, a clone + index of a staging tensor 4.1 us, `torch.empty(shape_tuple)` 2.7 us
         self._host_out_shape = (self.nu,) if self.u_per_command == 1 else (self.u_per_command, self.nu)
         self._host_template = torch.empty(self._host_out_shape, dtype=self.dtype)
+
+    def _export_flag(self):
+        """FLAG_EXPORT_PARTIAL on a sharded controller whose records leave the kernel (exchange='nccl'), else 0."""
+        return _cabi.FLAG_EXPORT_PARTIAL if (self._world > 1 and self._exchange != "p2p") else 0
 
     def _drop_plan(self):
         plan = getattr(self, "_plan", None)     # __del__ of a controller whose __init__ raised before _plan was set
@@ -1118,7 +1136,10 @@ class MPPI:
             acts = acts.reshape(-1, T, nu).to(self.d, self.dtype).contiguous()
             ovr_start = 1 if self.sample_null_action else 0
             n_ovr = acts.shape[0]
-            self.specific_action_sampler.register_sample_start_end(ovr_start, ovr_start + n_ovr)
+            # the kernel places the rows at their global sample indices; specific_dynamics sees this shard's rows only
+            lo = min(max(ovr_start - self._k_offset, 0), self._K_local)
+            hi = max(lo, min(ovr_start + n_ovr - self._k_offset, self._K_local))
+            self.specific_action_sampler.register_sample_start_end(lo, hi)
             self._ovr_keep = acts
             ovr_ptr = acts.data_ptr()
         nth = None if self._noise_theta_buf is None else self._noise_theta_buf.data_ptr()

@@ -23,10 +23,11 @@ def make_model(case, gold=None, **model_kw):
                            hills=[tuple(h) for h in m.get("hills", [])], terminal_scale=m.get("terminal_scale", 0.0))
 
 
-def make_engine(case, U0, device="cuda", route="fused", gold=None, model_kw=None, **extra):
+def make_engine(case, U0, device="cuda", route="fused", gold=None, model_kw=None, copy_rows=None, **extra):
     """route='fused' passes the registered model's bound methods; route='stepped' hides them behind
     plain functions so the controller takes the per-step (arbitrary-callable) path.  Cases with M>1 rollouts,
-    per-copy dynamics or a SpecificActionSampler exist on the stepped route only (case["routes"])."""
+    per-copy dynamics or a SpecificActionSampler exist on the stepped route only (case["routes"]).  `copy_rows`: the
+    samples per rollout copy the per-copy dynamics see (default K; a shard of a sharded controller sees its K_local)."""
     dt = _DT[case["dtype"]]
     model = make_model(case, gold, **(model_kw or {}))
     dyn, cost = model.dynamics, model.running_cost
@@ -39,7 +40,7 @@ def make_engine(case, U0, device="cuda", route="fused", gold=None, model_kw=None
     if case["model"].get("copy_offset") is not None:
         from tests.golden.cases import copy_offset_dynamics
         assert route == "stepped"
-        dyn = copy_offset_dynamics(model.dynamics, case["K"], case["model"]["copy_offset"])
+        dyn = copy_offset_dynamics(model.dynamics, copy_rows or case["K"], case["model"]["copy_offset"])
     kw = dict(num_samples=case["K"], horizon=case["T"], lambda_=case["lambda_"], device=device,
               u_scale=case.get("u_scale", 1), sample_null_action=case.get("sample_null_action", False),
               noise_abs_cost=case.get("noise_abs_cost", False), terminal_state_cost=term,

@@ -130,6 +130,14 @@ def test_world2_gloo_exchange_matches_single_process():
     assert len(out) == 2 and max(out.values()) < 1e-12
 
 
+@pytest.mark.parametrize("exchange", ["NCCL", "nvlink", "", None])
+def test_unknown_exchange_is_refused(exchange):
+    """Only "p2p" and "nccl" name an exchange; anything else used to select the NCCL route silently."""
+    pend = eng.Pendulum()
+    with pytest.raises(ValueError, match="exchange"):
+        eng.MPPI(pend.dynamics, pend.running_cost, 2, torch.tensor(1.0), num_samples=64, horizon=10, exchange=exchange)
+
+
 def _nominal_worker(rank, world, port, out):
     import types
     import torch.distributed as dist
