@@ -162,8 +162,9 @@ __host__ __device__ inline SmemLayout make_layout(int variant, int T, int nu, in
     // records, the cluster leader also receives its peers' through distributed shared memory
     L.off_wrec = o; o = align_up(o + cluster * (BS / 32) * (R + 2) * 8, 16);
     L.off_xstage = o; o = align_up(o + xstage * 8, 16);
-    // rescale factors of combine_records: one per record — the cluster's warp records, the staged records, or (ticket
-    // mode: the caller passes nb = number of cluster records of the grid) the records in the L2 workspace
+    // rescale factors of combine_records and combine_narrow (every combine<> in warp_tail): one per record — the cluster's
+    // warp records, the staged records, or (ticket mode: the caller passes nb = number of cluster records of the grid) the
+    // records in the L2 workspace.  A new caller of combine<> must pass at most nsq records.
     {
         int nsq = cluster * (BS / 32);
         if (xstage / (R + 2) > nsq) nsq = xstage / (R + 2);
@@ -743,11 +744,27 @@ __device__ __forceinline__ void warp_fold(const KArgs<real>& a, Smem<real>& sm, 
         // the 32 products of a warp are added in the controller's precision (as the reference's einsum does, in its own
         // order); everything ACROSS warps, CTAs and GPUs is fp64 (measured: an fp64 inner sum costs the large-K
         // geometry, where every warp folds, 5 us per command through F2F.F64 / DADD issue)
+        // The trip count is the constant 32, in batches of FB: each batch's shuffles and tile loads are issued together,
+        // ahead of its FFMAs, so only the chain on `acc` is serial (with a run-time count every iteration waited on its
+        // own shuffle and load).  Columns i >= nv (a partial last warp) are read — they lie inside the tile — but never
+        // added: their shared memory is stale, and 0 * NaN is not 0.  FB keeps a batch's values in 16 registers, and the
+        // batch loop stays rolled: fully unrolled, ptxas held every batch at once and spilled under the 64-register cap of
+        // the two-CTA-per-SM kernels (and in the global-tile softmin kernel).
+        constexpr int FB = sizeof(real) == 8 ? 4 : 8;
         real acc = (real)0;
-        for (int i = 0; i < nv; ++i) {
-            const real wi = __shfl_sync(0xffffffffu, wgt, i);
-            const real e = eps_in_tile ? row[i] : eps_of<real, VARIANT>(a.nm, row[i], us, a2);
-            acc += wi * e;                                                                      // mppi.py:268
+#pragma unroll 1
+        for (int ib = 0; ib < 32; ib += FB) {
+            real wv[FB], ev[FB];
+#pragma unroll
+            for (int u = 0; u < FB; ++u) {
+                wv[u] = __shfl_sync(0xffffffffu, wgt, ib + u);
+                ev[u] = row[ib + u];
+            }
+#pragma unroll
+            for (int u = 0; u < FB; ++u) {
+                const real e = eps_in_tile ? ev[u] : eps_of<real, VARIANT>(a.nm, ev[u], us, a2);
+                if (ib + u < nv) acc += wv[u] * e;                                              // mppi.py:268
+            }
         }
         if (jv) rec[2 + j] = rec[2 + j] * resc + (double)acc;
     }
@@ -873,51 +890,71 @@ __device__ __noinline__ void combine_global(const double* recs, int nrec, int R,
     __syncthreads();
 }
 
-// ---- the same combination for at most 64 records, WITHOUT CTA barriers or scratch -------------------------------------
-// Only the warps that own a column block take part (warp w: columns 32 w + lane, stride 32 P): each computes beta and the
-// rescale factors for itself (lane l holds those of records l and l + 32, handed round with shuffles) and adds its columns
-// over the records in ascending order (two interleaved chains).  The other warps of the CTA go straight to the one
-// barrier at the end.  This is the form the tail uses at every size that matters for latency: 16 warp records per cluster
-// and 32 cluster records per GPU at BASELINE config 2 — the barrier-and-scratch form above cost 2.3 + 2.9 us there
-// (every warp of the CTA walks its ~600 instructions, contending with the co-resident CTA at large K), this one a fraction.
+// ---- the same combination for at most 64 records, with one CTA barrier ------------------------------------------------
+// Column j's sum runs as two chains, acc0 over the even records and acc1 over the odd ones, each in ascending order, added
+// at the end as acc0 + acc1.  The chains are independent, so they run on different warps: work item u = (column block
+// u >> 1, chain u & 1) belongs to warp u mod W, W = min(warps, 2 x column blocks): two warps at C <= 32.  The W warps
+// compute beta each, and the rescale factors once (warps 0 and 1: records lane and 32 + lane) into sq[]; a named barrier
+// among them publishes the factors, and a second one hands the odd chains' sums (in part[]) to the warps that add them to
+// the even chains' sums, which already sit in numd.  A chain issues the loads of UB records and factors together, then
+// their UB DFMAs: only the chain itself is serial.  The other warps of the CTA go straight to the one CTA barrier at the
+// end.  This is the form the tail uses at every size that matters for latency: 16 warp records per cluster and 32 cluster
+// records per GPU at BASELINE config 2 — the barrier-and-scratch form above cost 2.3 + 2.9 us there (every warp of the
+// CTA walks its ~600 instructions, contending with the co-resident CTA at large K), this one a fraction.
+// sq holds nrec doubles and part C (the callers pass the layout's sqd and part2).
+// Named barrier 1 is reserved for the combining warps of combine_narrow_body (barrier 0 is __syncthreads); a kernel that
+// runs this tail must not use id 1 for anything else.
+#define MPPI_TAIL_NAMED_BARRIER 1
+__device__ __forceinline__ void combine_narrow_bar(int nthreads) {
+    asm volatile("barrier.sync.aligned %0, %1;" ::"n"(MPPI_TAIL_NAMED_BARRIER), "r"(nthreads) : "memory");
+}
 template <typename real>
-__device__ __forceinline__ void combine_narrow_body(const double* recs, int nrec, int R, double nfl, double* numd) {
+__device__ __forceinline__ void combine_narrow_body(const double* recs, int nrec, int R, double nfl, double* sq, double* part,
+                                                    double* numd) {
     typedef Ops<real> O;
     const int RW = R + 2, C = R + 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    const int P = min(nw, (C + 31) >> 5);
-    if (warp < P) {
+    // W >= 2 because every plan has at least two warps per CTA (plan_geometry: BS * tps >= 64): warps 0 and 1 write the
+    // factors of records 0..31 and 32..63, and part (the layout's part2, nw * R doubles) holds C = R + 1 doubles
+    const int W = min(nw, 2 * ((C + 31) >> 5));
+    if (warp < W) {
         const double b0 = lane < nrec ? recs[lane * RW] : (double)INFINITY;
         const double b1 = lane + 32 < nrec ? recs[(lane + 32) * RW] : (double)INFINITY;
         const double beta = warp_min<double>(fmin(b0, b1));
         // in the controller's precision (exact for equal betas; beta_q - beta is exact in fp64); an empty record weighs 0
-        const double s0 = b0 == (double)INFINITY ? 0.0 : (double)O::exp_((real)(nfl * (b0 - beta)));
-        const double s1 = b1 == (double)INFINITY ? 0.0 : (double)O::exp_((real)(nfl * (b1 - beta)));
-        for (int jb = warp * 32; jb < C; jb += P * 32) {
-            const int j = jb + lane;
-            const double* col = recs + 1 + (j < C ? j : 0);
-            double acc0 = 0.0, acc1 = 0.0;
-            for (int q0 = 0; q0 < nrec; q0 += 4) {
-                double v[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) v[u] = q0 + u < nrec ? col[(q0 + u) * RW] : 0.0;
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const int q = q0 + u;                       // q >= nrec: that lane's factor is 0 and v is 0
-                    const double sq = __shfl_sync(0xffffffffu, q < 32 ? s0 : s1, q & 31);
-                    if (u & 1) acc1 += sq * v[u];
-                    else acc0 += sq * v[u];
-                }
-            }
-            if (j < C) numd[1 + j] = acc0 + acc1;
+        if (warp < 2 && warp * 32 + lane < nrec) {
+            const double bq = warp == 0 ? b0 : b1;
+            sq[warp * 32 + lane] = bq == (double)INFINITY ? 0.0 : (double)O::exp_((real)(nfl * (bq - beta)));
         }
+        combine_narrow_bar(W * 32);
+        constexpr int UB = 8;
+        for (int u = warp; u < 2 * ((C + 31) >> 5); u += W) {
+            const int h = u & 1, j = (u >> 1) * 32 + lane;
+            const double* col = recs + 1 + (j < C ? j : 0);
+            double acc = 0.0;
+            for (int q0 = h; q0 < nrec; q0 += 2 * UB) {
+                double v[UB], s[UB];
+#pragma unroll
+                for (int k = 0; k < UB; ++k) {
+                    const int q = q0 + 2 * k;
+                    v[k] = q < nrec ? col[q * RW] : 0.0;
+                    s[k] = q < nrec ? sq[q] : 0.0;
+                }
+#pragma unroll
+                for (int k = 0; k < UB; ++k)
+                    if (q0 + 2 * k < nrec) acc += s[k] * v[k];
+            }
+            if (j < C) (h ? part[j] : numd[1 + j]) = acc;
+        }
+        combine_narrow_bar(W * 32);
+        for (int j = warp * 32 + lane; j < C; j += W * 32) numd[1 + j] = numd[1 + j] + part[j];
         if (threadIdx.x == 0) numd[0] = beta;
     }
     __syncthreads();
 }
 template <typename real>
-__device__ __noinline__ void combine_narrow(const double* recs, int nrec, int R, double nfl, double* numd) {
-    combine_narrow_body<real>(recs, nrec, R, nfl, numd);
+__device__ __noinline__ void combine_narrow(const double* recs, int nrec, int R, double nfl, double* sq, double* part, double* numd) {
+    combine_narrow_body<real>(recs, nrec, R, nfl, sq, part, numd);
 }
 #define MPPI_COMBINE_NARROW_MAX 64
 
@@ -926,10 +963,10 @@ __device__ __noinline__ void combine_narrow(const double* recs, int nrec, int R,
 template <typename real, bool INLINE = false>
 __device__ __forceinline__ void combine(Smem<real>& sm, const double* recs, int nrec, int R, double nfl) {
     if (INLINE) {
-        if (nrec <= MPPI_COMBINE_NARROW_MAX) combine_narrow_body<real>(recs, nrec, R, nfl, sm.numd);
+        if (nrec <= MPPI_COMBINE_NARROW_MAX) combine_narrow_body<real>(recs, nrec, R, nfl, sm.sqd, sm.part2, sm.numd);
         else combine_records_body<real>(recs, nrec, R, nfl, sm.part2, sm.sqd, sm.numd);
     } else {
-        if (nrec <= MPPI_COMBINE_NARROW_MAX) combine_narrow<real>(recs, nrec, R, nfl, sm.numd);
+        if (nrec <= MPPI_COMBINE_NARROW_MAX) combine_narrow<real>(recs, nrec, R, nfl, sm.sqd, sm.part2, sm.numd);
         else combine_records<real>(recs, nrec, R, nfl, sm.part2, sm.sqd, sm.numd);
     }
 }
