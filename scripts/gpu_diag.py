@@ -10,9 +10,8 @@ import timing
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from tests.golden.cases import CASES  # noqa: E402
+from tests.golden.cases import BASE, CASES  # noqa: E402
 from tests.golden.replay import OracleRunner, load  # noqa: E402
-from tests.golden.engine import make_engine  # noqa: E402
 
 out = None
 
@@ -29,11 +28,11 @@ def parity():
     for route in ("fused", "stepped"):
         for name in sorted(CASES):
             case, gold = load(name)
-            if route == "stepped" and case["K"] > 2048:
+            if route not in BASE.routes(name, case):
                 continue
             try:
-                run = OracleRunner(case)
-                ctrl = make_engine(case, run.stream.U0, route=route)
+                run = OracleRunner(case, gold)
+                ctrl = BASE.engine(case, gold, run.stream.U0, route)
                 errs, cerrs = [], []
                 for step in range(case["steps"]):
                     z = run.stream.next_z()
@@ -60,7 +59,7 @@ def parity():
         case, g32 = load("pendulum_c2_f32")
         _, g64 = load("pendulum_c2_f64")
         run = OracleRunner(case)
-        ctrl = make_engine(case, run.stream.U0)
+        ctrl = BASE.engine(case, g32, run.stream.U0, "fused")
         ctrl.inject_noise(run.stream.next_z())
         ctrl.command(np.asarray(case["x0"]))
         Ue = ctrl.U.cpu().numpy().astype(np.float64)

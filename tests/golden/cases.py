@@ -2,7 +2,8 @@
 
 A family is a table of cases plus the .npz fixtures tests/golden/make_golden.py makes from them by running the live
 reference; the tests replay those fixtures against the oracle (tests/golden/replay.py) and the CUDA engine
-(tests/golden/engine.py).  `Family` holds what differs between families; everything else is shared.
+(tests/golden/engine.py, tests/test_gpu_golden_replay.py).  `Family` holds what differs between families, on the oracle's
+side and on the engine's; everything else is shared.
 
 Each case is plain JSON-able data; a case with "N" is an MPPI_Batched case.  `draw_z` defines the injected
 standard-normal stream.
@@ -14,9 +15,18 @@ from typing import Callable
 import numpy as np
 import torch
 
+import pytorch_mppi_b200 as eng
 from oracle import mppi_oracle as orc
+from tests import ensemble_models as em
+from tests import shape_models as shm
 
 _DT = {"f32": torch.float32, "f64": torch.float64}
+
+# The engine's tolerance on U and the action against a fixture, per dtype:
+#   fp64: 1e-9   the engine reduces in a different order and accumulates the final sums in fp64
+#   fp32: 1e-5   the north-star target for the pendulum (BASELINE.json); the reference's OWN fp32-vs-fp64 gap on these
+#                draws is 1.2e-5..3.7e-5 (SURVEY.md App. C), so this is at the fp32 noise floor
+U_TOL = {"f64": 1e-9, "f32": 1e-5}
 
 PENDULUM = {"kind": "pendulum"}
 # test-suite fixture environment (reference tests/test_mppi.py:24-51)
@@ -137,6 +147,22 @@ class Family:
     fixture: Callable = lambda case: {}
     smooth_key: str = "A"           # the fixture key of SMPPI's action sequence
     scalars: bool = True            # whether the fixture stores cost_sum, beta and eta per step
+    # ---- the engine's side
+    # (case, fixture, U0, route, copy_rows=None, **controller keywords) -> the engine's controller of a case on `route`,
+    # asserted to have taken it.  `copy_rows`: the samples per rollout copy that per-copy dynamics see (default K; a
+    # shard of a sharded controller sees its K_local).
+    engine: Callable = None
+    # (name, case) -> the routes the fixture is replayed on
+    routes: Callable = lambda name, case: ["fused"]
+    # (name, case, route) -> the tolerance on U, the action and theta / the action sequence
+    u_tol: Callable = lambda name, case, route: U_TOL[case["dtype"]]
+    # (name, case, route, got, want, tol): asserts the engine's per-sample costs against the fixture's
+    check_costs: Callable = lambda name, case, route, got, want, tol: None
+    # route -> whether a single controller's replay resets the nominal to the fixture's after each command (a sharded
+    # replay always does)
+    reset_nominal: Callable = lambda route: False
+    # case -> whether the oracle can step alongside a replay that resets the nominal
+    lockable: Callable = lambda case: False
 
 
 def make_mlp_net(seed, dtype):
@@ -281,4 +307,139 @@ def _base_reference(case, prob, fixture):
     return prob.dynamics, prob.running_cost, kw
 
 
-BASE = Family("base", dict(CASES, **BATCHED_CASES), _base_model, _base_reference, _base_fixture)
+# ---- the engine's side ------------------------------------------------------------------------------------------------
+# Overrides of the fp32 north-star bound, each <= 2x the error measured on H100 (DESIGN.md §2):
+#  pendulum_small_f32: K=257, lambda=0.5 (ESS ~ 3): a 2e-7 relative (1-2 ulp) difference in a sample cost -- which
+#    sinf-vs-numpy-sin alone produces -- already moves U by 1e-5 (measured 1.04e-5).
+#  mlp_c4_f32: the network's three contractions run as FMA chains in the kernel and as BLAS calls in the reference
+#    (different summation order through two tanh layers and 30 steps).
+U_TOL_OVERRIDE = {"pendulum_small_f32": 2.1e-5, "mlp_c4_f32": 5e-5}
+# BASELINE config 4 (mlp_c4_f32) on the wgmma kernel: (PendulumMLP keywords, tolerance on U).  Hi/lo-split bf16 operands
+# keep the layer outputs at ~2^-16 relative; over 30-step rollouts of the (chaotic) learned pendulum the plan agrees with
+# the fp32 reference to 2.1e-4 (measured on H100, DESIGN.md §2) -- bound 5e-4; MUFU.TANH's 1e-3 absolute error per
+# activation shows at 2e-3.  The MLP's other routes run the FFMA kernel, whose tolerance the golden bound is.
+TENSOR_CORE_ROUTES = {"wgmma": (dict(tensor_cores="bf16x3", fast_tanh=False), 5e-4),
+                      "wgmma_mufu": (dict(tensor_cores="bf16x3", fast_tanh=True), 2e-3)}
+
+
+def plain(f):
+    """A plain function calling `f`: a controller given one takes the stepped route even where `f` is a model's method."""
+    return None if f is None else (lambda *args: f(*args))
+
+
+def controller(case, dynamics, running_cost, nx, sigma, U0=None, **kw):
+    """The MPPI / SMPPI / KMPPI controller of a single-controller case; SMPPI starts from its own (zero) nominal, the
+    others from `U0`."""
+    dt = _DT[case["dtype"]]
+    kw = dict(dict(num_samples=case["K"], horizon=case["T"], lambda_=case["lambda_"], device="cuda"), **kw)
+    if case["variant"] == "smppi":
+        sm = case["smooth"]
+        kw.update({k: torch.tensor(sm[k], dtype=dt) for k in ("action_min", "action_max") if sm.get(k) is not None})
+        return eng.SMPPI(dynamics, running_cost, nx, sigma, w_action_seq_cost=sm["w"], delta_t=sm["delta_t"], **kw)
+    if U0 is not None:
+        kw["U_init"] = U0.clone()
+    if case["variant"] == "kmppi":
+        km = case["kernel"]
+        return eng.KMPPI(dynamics, running_cost, nx, sigma, num_support_pts=km["S"], kernel=eng.RBFKernel(sigma=km["sigma"]),
+                         **kw)
+    return eng.MPPI(dynamics, running_cost, nx, sigma, **kw)
+
+
+def took_route(ctrl, model, route):
+    assert ctrl._model is (None if route == "stepped" else model), f"route {route} not taken"
+    return ctrl
+
+
+def _base_engine_model(case, gold, route):
+    m = case["model"]
+    if route == "copies":       # the per-copy dynamics as a CudaModel(copies=M) with the oracle's terminal cost
+        return em.copy_offset_linear(case["rollout_samples"], m["B"], m["goal"], m["copy_offset"],
+                                     m.get("terminal_scale", 0.0), terminal_cost=build_problem(case, gold)[0].terminal_state_cost)
+    if m["kind"] == "pendulum":
+        return eng.Pendulum()
+    if m["kind"] == "pendulum_mlp":
+        net = load_mlp_net(gold, _DT[case["dtype"]]).to("cuda")
+        return eng.PendulumMLP(net, **TENSOR_CORE_ROUTES.get(route, (dict(tensor_cores=False),))[0])
+    if m["kind"] == "shape":
+        return shm.shape_model(m["nx"], m["nu"], terminal=m["terminal"])
+    return eng.LinearPoint(B=m["B"], goal=m["goal"], Q=m.get("Q"), R=m.get("R"),
+                           hills=[tuple(h) for h in m.get("hills", [])], terminal_scale=m.get("terminal_scale", 0.0))
+
+
+def _base_engine(case, gold, U0, route, copy_rows=None, **controller_kw):
+    """route "fused" (or a tensor-core route) passes the registered model's bound methods; "stepped" hides them behind
+    plain functions so the controller takes the per-step (arbitrary-callable) path, which alone serves per-copy torch
+    dynamics and SpecificActionSamplers; "copies" runs the per-copy dynamics fused, as a CudaModel(copies=M)."""
+    dt = _DT[case["dtype"]]
+    model = _base_engine_model(case, gold, route)
+    wrap = plain if route == "stepped" else (lambda f: f)
+    dyn, cost = wrap(model.dynamics), wrap(model.running_cost)
+    sigma = torch.tensor(case["noise_sigma"], dtype=dt)
+    if "N" in case:
+        kw = dict(num_envs=case["N"], num_samples=case["K"], horizon=case["T"], lambda_=case["lambda_"], device="cuda",
+                  u_scale=case.get("u_scale", 1), u_per_command=case.get("u_per_command", 1),
+                  noise_abs_cost=case.get("noise_abs_cost", False))
+        kw.update({k: torch.tensor(case[k], dtype=dt) for k in ("noise_mu", "u_init", "u_min", "u_max") if case.get(k) is not None})
+        ctrl = eng.MPPI_Batched(dyn, cost, model.nx, sigma, **kw, **controller_kw)
+        ctrl.U = U0.clone()
+        return took_route(ctrl, model, route)
+    if case["model"].get("copy_offset") is not None and route != "copies":
+        assert route == "stepped"
+        dyn = copy_offset_dynamics(model.dynamics, copy_rows or case["K"], case["model"]["copy_offset"])
+    bd = torch.float32 if case.get("bounds_fp32") else dt
+    kw = dict(u_scale=case.get("u_scale", 1), sample_null_action=case.get("sample_null_action", False),
+              noise_abs_cost=case.get("noise_abs_cost", False),
+              terminal_state_cost=wrap(model.terminal_cost) if model.has_terminal else None,
+              rollout_samples=case.get("rollout_samples", 1), rollout_var_cost=case.get("rollout_var_cost", 0),
+              rollout_var_discount=case.get("rollout_var_discount", 0.95), u_per_command=case.get("u_per_command", 1))
+    kw.update({k: torch.tensor(case[k], dtype=bd if k in ("u_min", "u_max") else dt)
+               for k in ("noise_mu", "u_init", "u_min", "u_max") if case.get(k) is not None})
+    if case.get("sampler") is not None:
+        class Sampler(eng.SpecificActionSampler):
+            def sample_trajectories(self, state, info):
+                return sampler_actions(case, state)
+        kw["specific_action_sampler"] = Sampler()
+    return took_route(controller(case, dyn, cost, model.nx, sigma, U0, **kw, **controller_kw), model, route)
+
+
+def _is_mlp(case):
+    return case["model"]["kind"] == "pendulum_mlp"
+
+
+def _base_routes(name, case):
+    """Batched cases: fused and stepped.  Single controllers: the case's routes (default fused and stepped), the stepped
+    route only at K <= 2048 or for the MLP; the copy-offset cases also fused as a CudaModel(copies=M), and the config-4
+    MLP also on its tensor-core kernels."""
+    if "N" in case:
+        return ["fused", "stepped"]
+    routes = [r for r in case.get("routes", ["fused", "stepped"]) if r == "fused" or case["K"] <= 2048 or _is_mlp(case)]
+    if case["model"].get("copy_offset") is not None and case.get("sampler") is None:
+        routes.append("copies")
+    if name == "mlp_c4_f32":
+        routes += list(TENSOR_CORE_ROUTES)
+    return routes
+
+
+def _base_u_tol(name, case, route):
+    if route in TENSOR_CORE_ROUTES:
+        return TENSOR_CORE_ROUTES[route][1]
+    return U_TOL_OVERRIDE.get(name, U_TOL[case["dtype"]])
+
+
+def base_check_costs(name, case, route, got, want, tol, atol=None):
+    """rtol = atol: 1e-10 in fp64; in fp32 5e-6, or 2e-3 for the MLP's network (FFMA or wgmma).  The copy-offset
+    CudaModel's replay checks the plan only."""
+    if route == "copies":
+        return
+    rtol = 1e-10 if case["dtype"] == "f64" else (2e-3 if _is_mlp(case) or route in TENSOR_CORE_ROUTES else 5e-6)
+    np.testing.assert_allclose(got, want, rtol=rtol, atol=rtol if atol is None else atol)
+
+
+def base_lockable(case):
+    """Single controllers at K <= 2048 whose oracle is not the MLP (whose fp32 rollouts are chaotic)."""
+    return "N" not in case and case["K"] <= 2048 and not _is_mlp(case)
+
+
+BASE = Family("base", dict(CASES, **BATCHED_CASES), _base_model, _base_reference, _base_fixture,
+              engine=_base_engine, routes=_base_routes, u_tol=_base_u_tol, check_costs=base_check_costs,
+              reset_nominal=lambda route: route != "copies", lockable=base_lockable)

@@ -5,11 +5,12 @@ The step-dependent case hands the oracle its callables through step_cases.Horizo
 dynamics, then the running cost, once per horizon step."""
 import functools
 
+import numpy as np
 import torch
 
 from oracle import mppi_oracle as orc
 from tests import ensemble_models as em
-from tests.golden.cases import _DT, Family
+from tests.golden.cases import _DT, Family, controller, plain, took_route
 from tests.golden.step_cases import HorizonClock
 
 ENSEMBLE_CASES = {
@@ -90,4 +91,34 @@ def _reference(case, prob, fixture):
                       step_dependent_dynamics=case["model"] == "scenario_integrator")
 
 
-ENSEMBLE = Family("ensemble", ENSEMBLE_CASES, _model, _reference, smooth_key="action_sequence", scalars=False)
+def engine_model(case, K=None, params=None):
+    """The case's CudaModel(copies=M) for `K` samples per copy (default the case's), with `params` (default the case's)."""
+    K, p = K or case["K"], params or case_params(case)
+    if case["model"] == "pendulum":
+        return em.pendulum_ensemble(case["M"], K, p)
+    return em.scenario_integrator(case["M"], case["T"], K, p)
+
+
+def ensemble_controller(case, m, route="fused", U0=None, **kw):
+    """The controller of a case around the model `m`: on the fused route, or on the stepped route with m's torch twins
+    (the reference's M-copy T-loop)."""
+    dt = _DT[case["dtype"]]
+    c = controller(case, plain(m.dynamics) if route == "stepped" else m.dynamics, m.running_cost, 2,
+                   torch.tensor(case["noise_sigma"], dtype=dt), U0, **dict(dict(
+                       u_max=torch.tensor(case["u_max"], dtype=dt), terminal_state_cost=m.terminal_cost,
+                       rollout_samples=case["M"], rollout_var_cost=case["var_cost"],
+                       rollout_var_discount=case["var_discount"],
+                       step_dependent_dynamics=case["model"] == "scenario_integrator"), **kw))
+    return took_route(c, m, route)
+
+
+def _engine(case, gold, U0, route, copy_rows=None, **controller_kw):
+    return ensemble_controller(case, engine_model(case, K=copy_rows), route, U0, **controller_kw)
+
+
+def _check_costs(name, case, route, got, want, tol):
+    np.testing.assert_allclose(got, want, rtol=0, atol=tol * max(1.0, float(np.abs(want).max())))
+
+
+ENSEMBLE = Family("ensemble", ENSEMBLE_CASES, _model, _reference, smooth_key="action_sequence", scalars=False,
+                  engine=_engine, check_costs=_check_costs)

@@ -24,6 +24,7 @@ def load(name):
 
 
 FAMILIES = [BASE, SHAPES, STEP, TENSORS, ENSEMBLE, MLP_ENSEMBLE]
+FAMILY = {name: family for family in FAMILIES for name in family.cases}
 
 
 class Stream:

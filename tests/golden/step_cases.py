@@ -9,11 +9,13 @@ t = 0, ..., T-1, in order, once per command; `HorizonClock` relies on that order
 their t, and refuses any other call sequence."""
 import functools
 
+import numpy as np
 import torch
 
+import pytorch_mppi_b200 as eng
 from oracle import mppi_oracle as orc
 from tests import step_models as sm
-from tests.golden.cases import _DT, Family
+from tests.golden.cases import _DT, U_TOL, Family, controller, took_route
 
 STEPINT = {"kind": "step_integrator", "params": list(sm.SD_PARAMS), "terminal": True}
 STEP_CASES = {
@@ -83,4 +85,31 @@ def _reference(case, prob, fixture):
     return f, c, kw
 
 
-STEP = Family("step", dict(STEP_CASES, **STEP_BATCHED_CASES), _model, _reference)
+def _engine(case, gold, U0, route, copy_rows=None, **controller_kw):
+    """The CudaModel of tests/step_models.py (step_dependent=True) on the fused route."""
+    dt = _DT[case["dtype"]]
+    m = sm.step_dependent_user_model(case["model"]["params"], terminal=case["model"]["terminal"])
+    sigma, u_max = torch.tensor(case["noise_sigma"], dtype=dt), torch.tensor(case["u_max"], dtype=dt)
+    if "N" in case:
+        c = eng.MPPI_Batched(m.dynamics, m.running_cost, 2, sigma, case["N"], num_samples=case["K"], horizon=case["T"],
+                             lambda_=case["lambda_"], u_max=u_max, step_dependent_dynamics=True, device="cuda", **controller_kw)
+        c.U = U0.clone()
+    else:
+        c = controller(case, m.dynamics, m.running_cost, 2, sigma, U0, u_max=u_max, terminal_state_cost=m.terminal_cost,
+                       step_dependent_dynamics=True, **controller_kw)
+    return took_route(c, m, route)
+
+
+# stepint_kmppi_f32: the force sin(0.7 t) is CUDA's sinf in the kernel and numpy's float32 sin in the reference (1-ulp
+# differences, as the pendulum's sin: cases.U_TOL_OVERRIDE); measured 1.2e-5 on H100, bound 2e-5.  The costs, too.
+_F32_TOL = 2e-5
+
+
+def _check_costs(name, case, route, got, want, tol):
+    rtol = 1e-10 if case["dtype"] == "f64" else _F32_TOL
+    np.testing.assert_allclose(got, want, rtol=rtol, atol=rtol)
+
+
+STEP = Family("step", dict(STEP_CASES, **STEP_BATCHED_CASES), _model, _reference, engine=_engine,
+              u_tol=lambda name, case, route: U_TOL["f64"] if case["dtype"] == "f64" else _F32_TOL,
+              check_costs=_check_costs, lockable=lambda case: "N" not in case and case["K"] <= 2048)

@@ -8,7 +8,7 @@ import torch
 
 from oracle import mppi_oracle as orc
 from tests import tensor_models as tm
-from tests.golden.cases import _DT, Family
+from tests.golden.cases import _DT, Family, controller, took_route
 from tests.golden.step_cases import HorizonClock
 
 TENSOR_CASES = {
@@ -60,4 +60,19 @@ def fixture_tensors(gold, device):
             torch.from_numpy(np.asarray(gold["path"])).to(device).contiguous())
 
 
-TENSORS = Family("tensors", TENSOR_CASES, _model, _reference, _fixture, scalars=False)
+def _engine(case, gold, U0, route, copy_rows=None, **controller_kw):
+    """The CudaModel of tests/tensor_models.py on the fixture's costmap and path, on the fused route."""
+    dt = _DT[case["dtype"]]
+    m = tm.nav_model(*fixture_tensors(gold, "cuda"))
+    c = controller(case, m.dynamics, m.running_cost, 2, case["noise_sigma"] * torch.eye(2, dtype=dt), U0,
+                   u_max=torch.full((2,), case["u_max"], dtype=dt), step_dependent_dynamics=True, **controller_kw)
+    return took_route(c, m, route)
+
+
+def _check_costs(name, case, route, got, want, tol):
+    rtol = 1e-10 if case["dtype"] == "f64" else 5e-6          # the base family's
+    np.testing.assert_allclose(got, want, rtol=rtol, atol=rtol)
+
+
+TENSORS = Family("tensors", TENSOR_CASES, _model, _reference, _fixture, scalars=False, engine=_engine,
+                 check_costs=_check_costs, lockable=lambda case: case["K"] <= 2048)

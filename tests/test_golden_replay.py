@@ -5,10 +5,9 @@ import numpy as np
 import pytest
 import torch
 
-from tests.golden.replay import FAMILIES, load, runner, stored
+from tests.golden.replay import FAMILY, load, runner, stored
 
 TOL = {"f64": 1e-11, "f32": 2e-5}
-FAMILY = {name: f for f in FAMILIES for name in f.cases}
 
 
 def _assert_close(key, got, want, tol):

@@ -1,9 +1,8 @@
 """GPU: the fused command across its model envelope.
 
-  - the (1,1), (3,3) and (8,4) models of tests/shape_models.py against the live-reference fixtures of
-    tests/golden/shape_cases.py, on the fused route (CudaModel) and the stepped route (its torch twins): a 4x4 full
-    covariance, R = T*nu not a multiple of the normals per Philox call, an 8-component state buffer, K = 1 and T = 1;
-  - split-cost rollout vs single loop, resident mode, get_rollouts, MPPI_Batched and the in-kernel draws at those shapes;
+  - resident mode, get_rollouts and the in-kernel draws at the (1,1), (3,3) and (8,4) models of tests/shape_models.py
+    (their live-reference fixtures, tests/golden/shape_cases.py, and the split-cost rollout against the single loop on
+    them are replayed in tests/test_gpu_golden_replay.py);
   - the softmin tail in each of its forms (one CTA; one cluster record; LL and ticket exchange of cluster records; cluster
     sizes 8/4/2/1; one wave, two CTAs per SM, grid-stride multi-pass; 32-sample tiles; ragged K), each run first asserting
     from launch_info that it got the geometry it was written for, then compared with the fp64 oracle at 1e-10;
@@ -24,44 +23,16 @@ from oracle import mppi_oracle as orc
 from pytorch_mppi_b200._cabi import MppiLibraryError
 from tests import reports
 from tests import shape_models as shm
-from tests import test_gpu_parity as parity
-from tests.golden.shape_cases import SHAPE_BATCHED_CASES, SHAPE_CASES, SIG3
+from tests.golden.shape_cases import SIG3
 
 pytestmark = pytest.mark.gpu
 
-_MEASURED = {}
-# shape_mppi_n3u3_f32: the reference colours (z @ L^T) and weighs the noise (noise @ Sigma^-1) with fp32 matrix products,
-# the kernels with individually rounded products and sums over the 3 components: costs (down to 3.6e-3) differ by up to
-# 1.9e-5 absolute, on both routes (measured on H100; restating the kernels' order on the CPU gives the same 1.9e-5)
-COST_ATOL = {"shape_mppi_n3u3_f32": 3.8e-5}
-
 
 def _record(key, err):
-    _MEASURED[key] = max(_MEASURED.get(key, 0.0), float(err))
-    reports.write("envelope_errors.json", json.dumps(_MEASURED, indent=1, sort_keys=True))
+    reports.worst("envelope_errors.json", key, err)
 
 
-# ---- A/B: the live-reference fixtures at the new shapes -------------------------------------------------------------
-@pytest.mark.parametrize("route", ["fused", "stepped"])
-@pytest.mark.parametrize("name", sorted(SHAPE_CASES))
-def test_shape_fixture_parity(name, route):
-    """U, action, action_sequence / theta, cost_total against the fixture; omega, noise, perturbed_action and the
-    (K,T,nx) states against the oracle (tests/test_gpu_parity.py's runner and tolerances)."""
-    worst = parity._run(name, route, cost_atol=COST_ATOL.get(name))
-    _record(f"{name}/{route}", worst)
-
-
-@pytest.mark.parametrize("route", ["fused", "stepped"])
-@pytest.mark.parametrize("name", sorted(SHAPE_BATCHED_CASES))
-def test_shape_batched_fixture_parity(name, route):
-    parity.test_mppi_batched_matches_reference_golden(name, route)
-
-
-@pytest.mark.parametrize("name", sorted(n for n in SHAPE_CASES if SHAPE_CASES[n]["K"] > 1))
-def test_shape_split_cost_is_bit_identical_to_the_single_loop(name, monkeypatch):
-    parity.test_split_cost_rollout_is_bit_identical_to_the_single_loop(name, monkeypatch)
-
-
+# ---- B: resident mode, get_rollouts and the draws at the new shapes ---------------------------------------------------
 def _shape_ctrl(nx, nu, K, T, dtype, **kw):
     m = shm.shape_model(nx, nu)
     sigma = torch.tensor(SIG3 if nu == 3 else np.eye(nu) * 0.7 + 0.1, dtype=dtype)

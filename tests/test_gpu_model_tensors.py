@@ -1,7 +1,8 @@
 """GPU: user models that read device tensors (CudaModel(tensors=...)) on the fused route — a costmap read with bilinear
-interpolation and a reference path indexed by t (tests/tensor_models.py).  Parity with the oracle on both rollout shapes
-and with the live-reference fixtures, uint8 / int32 maps, in-place edits and set_tensors between commands, clamped
-lookups outside the map, resident mode, get_rollouts / states, copies=M with per-copy maps and MPPI_Batched."""
+interpolation and a reference path indexed by t (tests/tensor_models.py).  Parity with the oracle on both rollout shapes,
+uint8 / int32 maps, in-place edits and set_tensors between commands, clamped lookups outside the map, resident mode,
+get_rollouts / states, copies=M with per-copy maps and MPPI_Batched.  The live-reference fixtures are replayed in
+tests/test_gpu_golden_replay.py."""
 import functools
 
 import numpy as np
@@ -11,10 +12,7 @@ import torch
 import pytorch_mppi_b200 as eng
 from oracle import mppi_oracle as orc
 from tests import tensor_models as tm
-from tests.golden.engine import replay
-from tests.golden.replay import OracleRunner, load
 from tests.golden.step_cases import HorizonClock
-from tests.golden.tensor_cases import TENSOR_CASES, TENSORS, fixture_tensors
 
 pytestmark = pytest.mark.gpu
 
@@ -108,7 +106,7 @@ def test_fp32_c3_shape_parity_with_oracle():
     are 50..400 at lambda=1 and the effective sample size of these commands is 1.1..2.5 (omega of the oracle), so the
     update follows one or two samples, and a 1-ulp difference in their costs (6e-6 at 100; the interpolated trajectory
     W theta is a matrix product, summed in another order than the oracle's) moves U by ~1e-5 — as for pendulum_small_f32
-    (tests/test_gpu_parity.py).  Measured 1.8e-5 on H100."""
+    (tests/golden/cases.py).  Measured 1.8e-5 on H100."""
     m = _nav(40, hw=(256, 256))
     _closed_loop_vs_oracle(m, "kmppi", 8192, 40, torch.float32, 4e-5, S=5)
 
@@ -118,24 +116,6 @@ def test_integer_maps_match_oracle(map_dtype):
     m = _nav(20, map_dtype)
     assert m.tensors["costmap"].dtype == map_dtype and m.tensors["costmap"].max() > 100
     _closed_loop_vs_oracle(m, "mppi", 1024, 20, torch.float64, 1e-10)
-
-
-@pytest.mark.parametrize("name", sorted(TENSOR_CASES))
-def test_fused_matches_reference_golden(name):
-    case, gold = load(name)
-    assert case == TENSOR_CASES[name]
-    costmap, path = fixture_tensors(gold, "cuda")
-    m = tm.nav_model(costmap, path)
-    run = OracleRunner(case, gold, TENSORS)
-    dt = run.prob.dtype
-    kw = dict(lambda_=case["lambda_"])
-    if case["variant"] == "kmppi":
-        kw.update(num_support_pts=case["kernel"]["S"], kernel=eng.RBFKernel(sigma=case["kernel"]["sigma"]))
-    cls = eng.KMPPI if case["variant"] == "kmppi" else eng.MPPI
-    c = _ctrl(cls, m, case["K"], case["T"], dt, run.stream.U0.clone(), **kw)
-    ctol = 1e-10 if case["dtype"] == "f64" else 5e-6        # tests/test_gpu_parity.py
-    replay(c, run, gold, 1e-9 if case["dtype"] == "f64" else 1e-5,
-           lambda got, want: np.testing.assert_allclose(got, want, rtol=ctol, atol=ctol))
 
 
 def _single(m, T):

@@ -1,160 +1,22 @@
-"""GPU parity: the CUDA engine (through the Python API -> C-ABI -> sm_90a kernels) against
-  (1) the committed golden vectors produced by the LIVE reference, and
-  (2) the oracle stepped alongside on the same injected draws.
-
-Tolerances (max abs error on the nominal sequence U / action), stated per dtype:
-  fp64  : 1e-9   (the engine reduces in a different order and accumulates the final sums in fp64)
-  fp32  : 1e-5   north-star target for the pendulum (BASELINE.json); the reference's OWN fp32-vs-fp64
-                 gap on these draws is 1.2e-5..3.7e-5 (SURVEY.md App. C), so this is at the fp32
-                 noise floor.  LinearPoint fp32 cases have costs in the 1e2..1e3 range with
-                 library-ordered reductions in the reference: tolerance 2e-4.
-"""
+"""GPU parity: the CUDA engine (through the Python API -> C-ABI -> sm_90a kernels) against the oracle and restatements of
+the reference on injected draws, and its own properties (determinism, launch geometries, routes, the RNG streams).  The
+golden fixtures are replayed in tests/test_gpu_golden_replay.py; the tolerances on U are tests/golden/cases.py U_TOL."""
 import numpy as np
 import pytest
 import torch
 
-from tests.golden.cases import BATCHED_CASES, CASES
-from tests.golden.replay import BatchedOracleRunner, OracleRunner, load
+from tests.golden.cases import BASE
+from tests.golden.replay import OracleRunner, load
 
 pytestmark = pytest.mark.gpu
-
-U_TOL = {"f64": 1e-9, "f32": 1e-5}
-# Overrides of the fp32 north-star bound, each <= 2x the error measured on H100 (DESIGN.md §2):
-#  pendulum_small_f32: K=257, lambda=0.5 (ESS ~ 3): a 2e-7 relative (1-2 ulp) difference in a sample cost -- which
-#    sinf-vs-numpy-sin alone produces -- already moves U by 1e-5 (measured 1.04e-5).
-#  mlp_c4_f32: the network's three contractions run as FMA chains in the kernel and as BLAS calls in the reference
-#    (different summation order through two tanh layers and 30 steps).
-U_TOL_OVERRIDE = {"pendulum_small_f32": 2.1e-5, "mlp_c4_f32": 5e-5}
-_MEASURED = {}
-
-
-def _record(key, err):
-    """Worst error per (case, route), dumped to tests/_reports/parity_errors.json for the tolerance table above."""
-    import json
-    from tests import reports
-    _MEASURED[key] = max(_MEASURED.get(key, 0.0), float(err))
-    reports.write("parity_errors.json", json.dumps(_MEASURED, indent=1, sort_keys=True))
-
-
-def _run(name, route, check_oracle=True, model_kw=None, tol=None, cost_atol=None):
-    from tests.golden.engine import make_engine, replay
-    torch.set_num_threads(1)
-    case, gold = load(name)
-    run = OracleRunner(case, gold)
-    tol = tol if tol is not None else U_TOL_OVERRIDE.get(name, U_TOL[case["dtype"]])
-    ctrl = make_engine(case, run.stream.U0, route=route, gold=gold, model_kw=model_kw)
-    assert (ctrl._model is not None) == (route == "fused")
-    rtol = 1e-10 if case["dtype"] == "f64" else (5e-6 if model_kw is None and case["model"]["kind"] != "pendulum_mlp" else 2e-3)
-
-    def cost(c, want):
-        _record(f"{name}/{route}/cost_abs", np.abs(c - want).max())
-        np.testing.assert_allclose(c, want, rtol=rtol, atol=rtol if cost_atol is None else cost_atol)
-    return replay(ctrl, run, gold, tol, cost, reset_nominal=True, lock_step=check_oracle and case["K"] <= 2048,
-                  record=lambda err: _record(f"{name}/{route}" + (f"/{model_kw}" if model_kw else ""), err))
-
-
-def _routes(name):
-    return CASES[name].get("routes", ["fused", "stepped"])
-
-
-@pytest.mark.parametrize("name", sorted(n for n in CASES if "fused" in _routes(n)))
-def test_fused_matches_reference_golden(name):
-    _run(name, "fused")
-
-
-@pytest.mark.parametrize("name", sorted(n for n in CASES if "stepped" in _routes(n) and (CASES[n]["K"] <= 2048 or CASES[n]["model"]["kind"] == "pendulum_mlp")))
-def test_stepped_route_matches_reference_golden(name):
-    """Arbitrary callables (Python T-loop around the sampling / accumulation / softmin kernels), including the cases
-    only this route serves: rollout_samples M>1 with dynamics that differ between the copies (non-zero variance cost,
-    mppi.py:334-373), SpecificActionSampler rows (mppi.py:387-400), and the config-4 MLP as a plain torch module."""
-    _run(name, "stepped")
-
-
-@pytest.mark.parametrize("mode,fast,tol", [("bf16x3", False, 5e-4), ("bf16x3", True, 2e-3)])
-def test_tensor_core_mlp_matches_reference_golden(mode, fast, tol):
-    """BASELINE config 4 on the wgmma route against the LIVE-reference fixture (mlp_c4_f32): hi/lo-split bf16
-    operands keep the layer outputs at ~2^-16 relative; over 30-step rollouts of the (chaotic) learned pendulum the plan
-    agrees with the fp32 reference to 2.1e-4 (measured on H100, DESIGN.md §2) — bound 5e-4; MUFU.TANH's 1e-3 absolute error per
-    activation shows at 2e-3."""
-    _run("mlp_c4_f32", "fused", model_kw=dict(tensor_cores=mode, fast_tanh=fast), tol=tol)
-
-
-@pytest.mark.parametrize("name", sorted(BATCHED_CASES))
-@pytest.mark.parametrize("route", ["fused", "stepped"])
-def test_mppi_batched_matches_reference_golden(name, route):
-    """MPPI_Batched against fixtures produced by the live `ref.MPPI_Batched` (mppi.py:822-873)."""
-    from tests.golden.engine import make_batched_engine, replay
-    torch.set_num_threads(1)
-    case, gold = load(name)
-    run = BatchedOracleRunner(case)
-    ctrl = make_batched_engine(case, run.stream.U0, route=route)
-    assert (ctrl._model is not None) == (route == "fused")
-    rtol = 1e-10 if case["dtype"] == "f64" else 5e-6
-    replay(ctrl, run, gold, U_TOL[case["dtype"]], lambda c, want: np.testing.assert_allclose(c, want, rtol=rtol, atol=rtol),
-           reset_nominal=True, record=lambda err: _record(f"{name}/{route}", err))
-
-
-@pytest.mark.parametrize("name", sorted(n for n in CASES if "fused" in _routes(n) and CASES[n]["model"]["kind"] != "pendulum_mlp"))
-def test_split_cost_rollout_is_bit_identical_to_the_single_loop(name, monkeypatch):
-    """MPPI_FLAG_SPLIT_COST (the default for single-GPU problems small enough to run with helper threads;
-    MPPI_B200_SPLIT_COST=0 turns it off): the rollout thread runs the bare recurrence, the sample's
-    helper threads evaluate the running costs in parallel, the sum is taken in the reference's order.  Same
-    operations, same rounding, same order -> cost_total, U (A, theta) and the action must be BIT-identical to the
-    single-loop kernel on the same draws, for every golden case (all three variants, both dtypes, ragged K)."""
-    from tests.golden.engine import make_engine
-    case, gold = load(name)
-    run = OracleRunner(case)
-    monkeypatch.setenv("MPPI_B200_SPLIT_COST", "0")
-    plain = make_engine(case, run.stream.U0)
-    monkeypatch.setenv("MPPI_B200_SPLIT_COST", "1")
-    split = make_engine(case, run.stream.U0)
-    for step in range(min(case["steps"], 3)):
-        x = torch.from_numpy(gold[f"x_{step}"]).to(run.prob.dtype).numpy()
-        z = run.stream.next_z()
-        plain.inject_noise(z)
-        split.inject_noise(z)
-        a0 = plain.command(x)
-        a1 = split.command(x)
-        # the flag is honoured exactly when the problem is small enough to run with helper threads
-        assert plain.launch_info.split_cost == 0
-        assert split.launch_info.split_cost == (1 if split.launch_info.threads_per_sample > 1 else 0)
-        assert split.launch_info.threads_per_sample == plain.launch_info.threads_per_sample
-        # the rollout itself: same operations in the same order (fp32: bit for bit; fp64: the two kernels inline libdevice's
-        # double-precision sin / fmod in different surroundings, 1-ulp differences are possible)
-        if case["dtype"] == "f64":
-            rel = float(((plain.cost_total - split.cost_total).abs() / plain.cost_total.abs().clamp_min(1e-300)).max())
-            _record(f"{name}/split_vs_loop_cost_rel", rel)
-            assert rel <= 1e-13, (name, rel)
-        else:
-            assert torch.equal(plain.cost_total, split.cost_total), name
-        # the softmin reduction is fp64 in a fixed order per launch geometry; the two kernels may get different cluster
-        # sizes (different shared-memory footprints), i.e. a different — equally valid — summation order
-        close = dict(rtol=0, atol=1e-12 if case["dtype"] == "f64" else 5e-7)
-        assert torch.allclose(plain.U, split.U, **close), name
-        assert torch.allclose(a0, a1, **close), name
-        if case["variant"] == "smppi":
-            assert torch.allclose(plain.action_sequence, split.action_sequence, **close)
-        if case["variant"] == "kmppi":
-            assert torch.allclose(plain.theta, split.theta, **close)
-    # every golden case is small enough to keep its helper threads (no more tiles than SMs)
-    assert split.launch_info.split_cost == 1, (name, split.launch_info.threads_per_sample)
-    # and the split kernel meets the reference tolerance on its own (first command, golden U)
-    tol = U_TOL_OVERRIDE.get(name, U_TOL[case["dtype"]])
-    run2 = OracleRunner(case)
-    monkeypatch.setenv("MPPI_B200_SPLIT_COST", "1")
-    again = make_engine(case, run2.stream.U0)
-    again.inject_noise(run2.stream.next_z())
-    again.command(torch.from_numpy(gold["x_0"]).to(run2.prob.dtype).numpy())
-    assert float(np.abs(again.U.cpu().numpy() - gold["U_0"]).max()) <= tol
 
 
 def test_closed_loop_free_running_c2():
     """10 closed-loop commands WITHOUT resynchronising U: error vs the fp32 reference stays at the
     fp32 noise floor (SURVEY.md §8d parity check)."""
-    from tests.golden.engine import make_engine
     case, gold = load("pendulum_c2_f32")
     run = OracleRunner(case)
-    ctrl = make_engine(case, run.stream.U0)
+    ctrl = BASE.engine(case, gold, run.stream.U0, "fused")
     x = torch.tensor(case["x0"], dtype=torch.float32)
     model = ctrl._model
     errs = []
@@ -171,11 +33,10 @@ def test_philox_stream_matches_oracle_and_parity_holds():
     """Speed mode: in-kernel Philox.  (a) the normals the kernel used equal the numpy statement of the
     stream; (b) feeding exactly those normals to the oracle reproduces the engine's update."""
     from oracle import philox_oracle as po
-    from tests.golden.engine import make_engine
     for name, np_dt in (("pendulum_small_f32", np.float32), ("linear_mppi_f64", np.float64), ("nav2d_kmppi_f64", np.float64)):
         case, gold = load(name)
         run = OracleRunner(case)
-        ctrl = make_engine(case, run.stream.U0, rng_seed=0xC0FFEE1234)
+        ctrl = BASE.engine(case, gold, run.stream.U0, "fused", rng_seed=0xC0FFEE1234)
         ctrl.record_noise(True)
         x = torch.tensor(case["x0"], dtype=run.prob.dtype)
         rows = ctrl._noise_rows()

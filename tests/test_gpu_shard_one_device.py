@@ -344,96 +344,33 @@ def _tail_jobs(world):
 
 
 # ---- golden fixtures, sharded ----------------------------------------------------------------------------------------
-def _families():
+def _sharded_route(fam, case, route):
+    """The single-controller replay's routes a fixture also runs sharded on: fused, the stepped route at K <= 2048 (or
+    for the MLP), and the config-4 MLP's bf16x3 kernel with the exact tanh.  Not the copy-offset CudaModel, the MUFU
+    tanh or the ensembles' tensor-core kernel."""
+    if route == "stepped":
+        return case["K"] <= 2048 or case["model"]["kind"] == "pendulum_mlp"
+    return route == "fused" or (route == "wgmma" and fam.name == "base")
+
+
+def _fixture_ids():
+    """(world, name, route) of every single-controller fixture a sharded controller accepts (K >= world)."""
     from tests.golden.replay import FAMILIES
-    return FAMILIES
-
-
-def _fixture_list(world):
-    """(name, route) of every single-controller fixture a sharded controller accepts (K >= world)."""
-    from tests.golden.cases import BASE
-    from tests.golden.shape_cases import SHAPES
-    out = []
-    for fam in _families():
-        for name, case in sorted(fam.cases.items()):
-            if "N" in case or case["K"] < world:
-                continue
-            if fam in (BASE, SHAPES):
-                mlp = case["model"]["kind"] == "pendulum_mlp"
-                routes = [r for r in case.get("routes", ["fused", "stepped"]) if r == "fused" or case["K"] <= 2048 or mlp]
-                if name == "mlp_c4_f32":
-                    routes.append("wgmma")
-            else:
-                routes = ["fused"]
-            out += [(name, r) for r in routes]
-    return out
-
-
-def _family_of(name):
-    return next(f for f in _families() if name in f.cases)
-
-
-def _lock_step(fam, case):
-    """Whether the oracle steps alongside (omega, noise and perturbed_action per shard), as tests/test_gpu_parity.py."""
-    from tests.golden.cases import BASE
-    from tests.golden.shape_cases import SHAPES
-    from tests.golden.step_cases import STEP
-    from tests.golden.tensor_cases import TENSORS
-    kind = case["model"].get("kind") if isinstance(case.get("model"), dict) else None
-    return fam in (BASE, SHAPES, STEP, TENSORS) and case["K"] <= 2048 and kind != "pendulum_mlp"
-
-
-def _fixture_engine(fam, case, gold, U0, route, pg, K_local):
-    import pytorch_mppi_b200 as eng
-    from tests.golden.cases import _DT, BASE
-    from tests.golden.engine import make_engine
-    from tests.golden.shape_cases import SHAPES
-    from tests.golden.step_cases import STEP
-    from tests.golden.tensor_cases import TENSORS, fixture_tensors
-    if fam in (BASE, SHAPES):
-        model_kw = dict(tensor_cores="bf16x3") if route == "wgmma" else None
-        return make_engine(case, U0, route="fused" if route == "wgmma" else route, gold=gold, model_kw=model_kw,
-                           copy_rows=K_local, **_kw(pg))
-    dt = _DT[case["dtype"]]
-    kw = dict(_kw(pg), lambda_=case["lambda_"]) if fam in (STEP, TENSORS) else _kw(pg)
-    if case["variant"] != "smppi":
-        kw["U_init"] = U0.clone()
-    if case["variant"] == "kmppi" and fam in (STEP, TENSORS):
-        kw.update(num_support_pts=case["kernel"]["S"], kernel=eng.RBFKernel(sigma=case["kernel"]["sigma"]))
-    cls = eng.KMPPI if case["variant"] == "kmppi" else eng.MPPI
-    if fam is STEP:
-        from tests import step_models as um
-        m = um.step_dependent_user_model(case["model"]["params"])
-        return cls(m.dynamics, m.running_cost, 2, torch.tensor(case["noise_sigma"], dtype=dt), num_samples=case["K"],
-                   horizon=case["T"], u_max=torch.tensor(case["u_max"], dtype=dt), terminal_state_cost=m.terminal_cost,
-                   step_dependent_dynamics=True, device="cuda", **kw)
-    if fam is TENSORS:
-        from tests import tensor_models as tm
-        m = tm.nav_model(*fixture_tensors(gold, "cuda"))
-        return cls(m.dynamics, m.running_cost, 2, case["noise_sigma"] * torch.eye(2, dtype=dt), num_samples=case["K"],
-                   horizon=case["T"], u_max=torch.full((2,), case["u_max"], dtype=dt), step_dependent_dynamics=True,
-                   device="cuda", **kw)
-    if fam.name == "ensemble":
-        from tests import test_gpu_ensemble as te
-        return te._ctrl(case, te._model(case, K=K_local), **kw)
-    from tests import test_gpu_mlp_ensemble as tme
-    from tests.golden.mlp_ensemble_cases import load_nets
-    ens = eng.PendulumMLPEnsemble([n.cuda() for n in load_nets(case, gold)], max_torque=case["u_max"], tensor_cores=False)
-    return tme._ctrl(case, ens, **kw)
+    return [(w, name, route) for w in WORLDS for fam in FAMILIES for name, case in sorted(fam.cases.items())
+            if "N" not in case and case["K"] >= w for route in fam.routes(name, case) if _sharded_route(fam, case, route)]
 
 
 def job_fixture(pg, name, route):
     """Replays a fixture at its states with its draws; after each command the nominal is the fixture's (replay.py)."""
-    from tests.golden.replay import OracleRunner, load
-    case, gold = load(name)
-    fam = _family_of(name)
-    run = OracleRunner(case, gold, fam)
-    from pytorch_mppi_b200.distributed import shard_bounds
     import torch.distributed as dist
+    from pytorch_mppi_b200.distributed import shard_bounds
+    from tests.golden.replay import FAMILY, OracleRunner, load
+    case, gold = load(name)
+    fam = FAMILY[name]
+    run = OracleRunner(case, gold, fam)
     k0, n = shard_bounds(case["K"], dist.get_rank(pg), dist.get_world_size(pg))
-    c = _fixture_engine(fam, case, gold, run.stream.U0, route, pg, n)
-    assert (c._model is None) == (route == "stepped")
-    lock = _lock_step(fam, case)
+    c = fam.engine(case, gold, run.stream.U0, route, copy_rows=n, **_kw(pg))
+    lock = fam.lockable(case)
     steps = []
     for step in range(case["steps"]):
         c.inject_noise(run.stream.next_z())
@@ -448,7 +385,8 @@ def job_fixture(pg, name, route):
 
 
 def _fixture_jobs(world):
-    return {f"fixture_{name}_{route}": (job_fixture, dict(name=name, route=route)) for name, route in _fixture_list(world)}
+    return {f"fixture_{name}_{route}": (job_fixture, dict(name=name, route=route))
+            for w, name, route in _fixture_ids() if w == world}
 
 
 # ---- refusals --------------------------------------------------------------------------------------------------------
@@ -587,15 +525,10 @@ def runs():
     return _Runs()
 
 
-_WORST = {}
-
-
 def _record(key, err):
     """Worst errors per family and dtype, in tests/_reports/shard_one_device_errors.json."""
-    import json
     from tests import reports
-    _WORST[key] = max(_WORST.get(key, 0.0), float(err))
-    reports.write("shard_one_device_errors.json", json.dumps(_WORST, indent=1, sort_keys=True))
+    reports.worst("shard_one_device_errors.json", key, err)
 
 
 def _cat(ranks, step, key):
@@ -618,50 +551,15 @@ def _same_on_every_rank(ranks, step, keys=("U", "action", "theta", "A")):
 # ----------------------------------------------------------------------------------------------------------------------
 # (a) every fixture of every family, sharded, against the fixture and the oracle in lock step
 # ----------------------------------------------------------------------------------------------------------------------
-def _fixture_tol(fam, name, case, route):
-    from tests.golden.cases import BASE
-    from tests.golden.shape_cases import SHAPES
-    from tests.test_gpu_parity import U_TOL, U_TOL_OVERRIDE
-    if route == "wgmma":
-        return 5e-4
-    if fam in (BASE, SHAPES):
-        return U_TOL_OVERRIDE.get(name, U_TOL[case["dtype"]])
-    if fam.name == "step" and case["dtype"] == "f32":
-        return 2e-5                                     # tests/test_gpu_step_dependent.py
-    if fam.name == "mlp_ensemble":
-        from tests.test_gpu_mlp_ensemble import FIXTURE_TOL, TOL
-        return FIXTURE_TOL.get((name, False), TOL[(case["dtype"], False)])
-    return U_TOL[case["dtype"]]
-
-
-def _check_costs(fam, case_name, case, route, got, want, tol):
-    """The cost check of the family's own fixture test, on the concatenated shards."""
-    if fam.name == "ensemble":
-        np.testing.assert_allclose(got, want, rtol=0, atol=tol * max(1.0, float(np.abs(want).max())))
-    elif fam.name == "mlp_ensemble":
-        from tests.test_gpu_mlp_ensemble import _assert_costs_close
-        _assert_costs_close(got, want, tol, torch.float64 if case["dtype"] == "f64" else torch.float32)
-    else:                                               # tests/test_gpu_parity.py `_run`
-        f64 = case["dtype"] == "f64"
-        mlp = isinstance(case.get("model"), dict) and case["model"].get("kind") == "pendulum_mlp"
-        from tests.test_gpu_envelope import COST_ATOL
-        rtol = 1e-10 if f64 else (2e-3 if (mlp or route == "wgmma") else (2e-5 if fam.name == "step" else 5e-6))
-        np.testing.assert_allclose(got, want, rtol=rtol, atol=COST_ATOL.get(case_name, rtol))
-
-
-def _fixture_ids():
-    return [(w, n, r) for w in WORLDS for n, r in _fixture_list(w)]
-
-
 @pytest.mark.parametrize("world,name,route", _fixture_ids())
 def test_sharded_fixture_replay(runs, world, name, route):
     from tests.golden.engine import ORACLE_TOL
-    from tests.golden.replay import OracleRunner, load
+    from tests.golden.replay import FAMILY, OracleRunner, load
     ranks = runs.ranks(world, DEFAULT, f"fixture_{name}_{route}")
     case, gold = load(name)
-    fam = _family_of(name)
+    fam = FAMILY[name]
     run = OracleRunner(case, gold, fam)
-    tol = _fixture_tol(fam, name, case, route)
+    tol = fam.u_tol(name, case, route)
     _spans_partition(ranks, case["K"])
     otol = ORACLE_TOL[case["dtype"]]
     worst = 0.0
@@ -679,7 +577,7 @@ def test_sharded_fixture_replay(runs, world, name, route):
             if f"{key}_{step}" in gold:
                 assert float(np.abs(got[attr] - gold[f"{key}_{step}"]).max()) <= tol, key
         if f"cost_total_{step}" in gold:
-            _check_costs(fam, name, case, route, _cat(ranks, step, "cost"), gold[f"cost_total_{step}"], tol)
+            fam.check_costs(name, case, route, _cat(ranks, step, "cost"), gold[f"cost_total_{step}"], tol)
         if "omega" in got:
             r = run.step(x, z)
             om = _cat(ranks, step, "omega")

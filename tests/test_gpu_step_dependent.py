@@ -1,6 +1,6 @@
 """GPU: step-dependent user models on the fused route (CudaModel(step_dependent=True), step_dependent_dynamics=True) —
-parity with the oracle on both rollout shapes, resident mode, get_rollouts, MPPI_Batched, and set_params between
-commands."""
+parity with the oracle on both rollout shapes, resident mode, get_rollouts, and set_params between commands.  Their
+golden fixtures, MPPI_Batched's among them, are replayed in tests/test_gpu_golden_replay.py."""
 import functools
 
 import numpy as np
@@ -98,7 +98,7 @@ def test_single_loop_rollout_matches_oracle():
 
 def test_split_cost_rollout_equals_single_loop_bit_for_bit(monkeypatch):
     """The split-cost rollout (helper thread per t) and the single-loop kernel (step t's cost in iteration t) give the
-    same per-sample costs bit for bit, as for the registered models (tests/test_gpu_parity.py); the softmin reduction
+    same per-sample costs bit for bit, as for the registered models (tests/test_gpu_golden_replay.py); the softmin reduction
     order follows each kernel's cluster size, so U and the action agree to fp32 rounding of that order."""
     m = um.step_dependent_user_model()
     ctrls = {}
@@ -158,44 +158,6 @@ def test_get_rollouts_equals_torch_loop():
         p = list(m.params)
         p[1] = -p[1]
         m.set_params(p)                     # get_rollouts uses the current parameters, before any command took them
-
-
-def test_mppi_batched_matches_reference_golden():
-    from tests.golden.engine import replay
-    from tests.golden.replay import BatchedOracleRunner, load
-    from tests.golden.step_cases import STEP
-    case, gold = load("stepint_batched_f64")
-    run = BatchedOracleRunner(case, family=STEP)
-    m = um.step_dependent_user_model(case["model"]["params"], terminal=False)
-    dt = torch.float64
-    c = eng.MPPI_Batched(m.dynamics, m.running_cost, 2, torch.tensor(case["noise_sigma"], dtype=dt), case["N"],
-                         num_samples=case["K"], horizon=case["T"], lambda_=case["lambda_"], u_max=torch.tensor(case["u_max"], dtype=dt),
-                         step_dependent_dynamics=True, device="cuda")
-    assert c._model is m
-    c.U = run.stream.U0.clone()
-    replay(c, run, gold, 1e-9, lambda got, want: np.testing.assert_allclose(got, want, rtol=1e-10, atol=1e-10))
-
-
-# stepint_kmppi_f32: the force sin(0.7 t) is CUDA's sinf in the kernel and numpy's float32 sin in the reference (1-ulp
-# differences, as the pendulum's sin: tests/test_gpu_parity.py U_TOL_OVERRIDE); measured 1.2e-5 on H100, bound 2e-5
-@pytest.mark.parametrize("name,tol", [("stepint_mppi_f64", 1e-9), ("stepint_kmppi_f32", 2e-5)])
-def test_fused_matches_reference_golden(name, tol):
-    from tests.golden.engine import replay
-    from tests.golden.replay import OracleRunner, load
-    from tests.golden.step_cases import STEP
-    case, gold = load(name)
-    run = OracleRunner(case, family=STEP)
-    dt = run.prob.dtype
-    m = um.step_dependent_user_model(case["model"]["params"])
-    kw = dict(lambda_=case["lambda_"])
-    if case["variant"] == "kmppi":
-        kw.update(num_support_pts=case["kernel"]["S"], kernel=eng.RBFKernel(sigma=case["kernel"]["sigma"]))
-    cls = eng.KMPPI if case["variant"] == "kmppi" else eng.MPPI
-    c = cls(m.dynamics, m.running_cost, 2, torch.tensor(case["noise_sigma"], dtype=dt), num_samples=case["K"],
-            horizon=case["T"], U_init=run.stream.U0.clone(), u_max=torch.tensor(case["u_max"], dtype=dt),
-            terminal_state_cost=m.terminal_cost, step_dependent_dynamics=True, device="cuda", **kw)
-    assert c._model is m
-    replay(c, run, gold, tol)
 
 
 def test_set_params_takes_effect_at_the_next_command_without_a_new_plan():
